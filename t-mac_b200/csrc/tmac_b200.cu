@@ -1386,7 +1386,8 @@ static int seq_build_chain(Sequence &S) {
     std::vector<ChainOp> ops(n);
     std::vector<size_t> coff(n, (size_t)-1), lloff(n, 0);
     size_t ctot = 0, max_blk = 0, lltot = 0;
-    int max_nrsb = 0, pb = 0, qch = 0, agq = 0, bits = 0, rsbsz = 0;
+    int max_nrsb = 0, max_bpw = 0, pb = 0, qch = 0, agq = 0, bits = 0, rsbsz = 0;
+    auto chain_bpw = [](int nchunk) { return (nchunk + kChainCS * kChainWarps - 1) / (kChainCS * kChainWarps); };
     for (int i = 0; i < n; ++i) {
         const Resident &R = g.res.find(S.ops[i].handle)->second;
         const StreamLayout &L = R.L;
@@ -1398,16 +1399,27 @@ static int seq_build_chain(Sequence &S) {
         else if (S.ops[i].in_off % ((g.chain_flags & kChainBarrier) ? 4 : 2) || S.ops[S.ops[i].in_op].out_f16) return 0;    // float4 loads (16-byte word pairs in data-flow mode) of an fp32 producer
         max_blk = std::max(max_blk, (L.blk + 127) & ~(size_t)127);
         max_nrsb = std::max(max_nrsb, L.nrsb);
+        max_bpw = std::max(max_bpw, chain_bpw(L.nchunk));
         if (!S.ops[i].C) { coff[i] = ctot; ctot += ((size_t)L.nrsb * L.rsb * sizeof(float) + 255) & ~(size_t)255; }
         lloff[i] = lltot; lltot += ((size_t)L.nrsb * L.rsb * sizeof(uint2) + 255) & ~(size_t)255;
     }
     chain_fn fn = pick_chain(pb, qch, agq);
     if (!fn) return 0;
     const int grid = max_nrsb * kChainCS;
-    const size_t smem = (size_t)(kChainCS + kChainWarps) * rsbsz * 4 + (size_t)kChainWarps * (2 * max_blk + (size_t)qch * 4 * 8) + kChainWarps * 16 + 32;
-    if (smem > 48 * 1024 && cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
     cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    {   // every cluster must be resident at once: the grid barrier spins
+    // Ring depth: the deepest per-warp stage ring, up to one op of blocks ahead (max_bpw + 1 stages), with which every cluster is
+    // still resident at once -- the waits between clusters spin.  The kernel's dynamic shared-memory limit is only ever raised, so
+    // that sequences built earlier on the same kernel with a deeper ring keep launching.
+    cudaFuncAttributes fa{};
+    if (cudaFuncGetAttributes(&fa, (const void *)fn) != cudaSuccess) { cudaGetLastError(); return 0; }
+    int smem_limit = fa.maxDynamicSharedSizeBytes, nstage = 0;
+    size_t smem = 0;
+    for (int s = max_bpw + 1; s >= 2 && !nstage; --s) {
+        smem = (size_t)(kChainCS + kChainWarps) * rsbsz * 4 + (size_t)kChainWarps * (s * max_blk + (size_t)qch * 4 * 8) + (size_t)kChainWarps * s * 8 + 32;
+        if ((int)smem > smem_limit) {
+            if (cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); continue; }
+            smem_limit = (int)smem;
+        }
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kChainWarps * 32); cfg.dynamicSmemBytes = smem;
         cudaLaunchAttribute attr[1];
@@ -1415,9 +1427,10 @@ static int seq_build_chain(Sequence &S) {
         attr[0].val.clusterDim.x = kChainCS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
         int nc = 0;
-        if (cudaOccupancyMaxActiveClusters(&nc, (const void *)fn, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
-        if (nc < max_nrsb) return 0;
+        if (cudaOccupancyMaxActiveClusters(&nc, (const void *)fn, &cfg) != cudaSuccess) { cudaGetLastError(); continue; }
+        if (nc >= max_nrsb) nstage = s;
     }
+    if (!nstage) return 0;
     if (cudaMalloc(&S.d_cops, n * sizeof(ChainOp)) != cudaSuccess || cudaMalloc(&S.d_bar, 256) != cudaSuccess ||
         cudaMalloc(&S.d_epochs, grid * sizeof(unsigned)) != cudaSuccess || cudaMalloc(&S.d_err, sizeof(int)) != cudaSuccess ||
         cudaMalloc(&S.d_cint, std::max<size_t>(ctot, 256)) != cudaSuccess || cudaMalloc(&S.d_y, lltot) != cudaSuccess) { cudaGetLastError(); S.release(); return fail("seq_build: out of device memory"); }
@@ -1432,7 +1445,7 @@ static int seq_build_chain(Sequence &S) {
         o.C = S.ops[i].C ? S.ops[i].C : (void *)((char *)S.d_cint + coff[i]);
         o.x = S.ops[i].x_ext ? (const float *)S.ops[i].x_ext : (const float *)ops[S.ops[i].in_op].C + S.ops[i].in_off;
         o.rsb_stride = L.rsb_stride; o.K = L.K; o.Mout = L.Mout; o.nrsb = L.nrsb; o.nchunk = L.nchunk;
-        o.blk_bytes = (int)L.blk; o.bpw = (L.nchunk + kChainCS * kChainWarps - 1) / (kChainCS * kChainWarps);
+        o.blk_bytes = (int)L.blk; o.bpw = chain_bpw(L.nchunk);
         o.zp = L.zp; o.one_scale = L.one_scale; o.sd = L.sd; o.out_f16 = S.ops[i].out_f16; o.scale0 = L.scale0;
         o.in_op = S.ops[i].x_ext ? -1 : S.ops[i].in_op;
         o.npeer = S.ops[i].npeer; o.pad_ = 0;
@@ -1443,7 +1456,7 @@ static int seq_build_chain(Sequence &S) {
     }
     CUDA_OK(cudaMemcpyAsync(S.d_cops, ops.data(), n * sizeof(ChainOp), cudaMemcpyHostToDevice, g.stream()));
     CUDA_OK(cudaStreamSynchronize(g.stream()));
-    S.cparams.ops = (const ChainOp *)S.d_cops; S.cparams.nops = n; S.cparams.max_blk = (int)max_blk;
+    S.cparams.ops = (const ChainOp *)S.d_cops; S.cparams.nops = n; S.cparams.max_blk = (int)max_blk; S.cparams.nstage = nstage;
     S.cparams.bar = (unsigned *)S.d_bar; S.cparams.epochs = (unsigned *)S.d_epochs; S.cparams.err = (int *)S.d_err;
     S.cparams.flags = g.chain_flags; S.cparams.trace = nullptr;
 

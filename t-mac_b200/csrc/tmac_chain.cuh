@@ -10,10 +10,13 @@
 //   * the cluster-wide rendezvous of the reduction becomes one DSMEM hop: peers send their partial sums with st.async, whose
 //     completion bytes are counted on the leader's mbarrier (data and signal travel together); a split-phase cluster barrier,
 //     waited for a whole op later, only guards the re-use of the buffers;
-//   * the exposed weight stream: every warp requests its block of op i+1 (one cp.async.bulk, 4.6 KB, second stage buffer) when
-//     it starts op i's lookups -- weights do not depend on activations -- so the stream overlaps the ALU-bound phase and is out
-//     of the way of the latency-critical words (requesting it earlier, across the hand-over, puts 12.7 MB of bulk traffic in
-//     front of the words everybody waits for);
+//   * the exposed weight stream: a warp's blocks over the whole chain form one sequence (op 0's chunks of this warp, then op 1's,
+//     ...), loaded by one cp.async.bulk each (4.6 KB) into a per-warp ring of ChainParams::nstage stages.  When the warp starts
+//     the lookups of block j it requests block j + nstage - 1 into the stage block j - 1 has vacated -- weights do not depend on
+//     activations -- so the stream overlaps the ALU-bound phase and is out of the way of the latency-critical words (requesting
+//     earlier, across the hand-over, puts 12.7 MB of bulk traffic in front of the words everybody waits for).  With nstage =
+//     bpw + 1 every block is requested one full op before it is consumed; the host picks the deepest ring that keeps every
+//     cluster resident;
 //   * CTA placement is fixed for the whole chain (344 CTAs of 128 threads for 11008 rows, all resident).
 // bench.py times it on the bench chain (32 x 11008x4096 W2, x[i+1] = first K outputs of op i) beside the launch chain and
 // tmac_seq.cuh; flags bit 0 selects the grid-barrier form this kernel started as, kept for comparison.  Per-phase stamps
@@ -39,7 +42,7 @@ struct ChainOp {
     void *C;                                // output [Mout]
     unsigned long long rsb_stride;
     int K, Mout, nrsb, nchunk;
-    int blk_bytes, bpw;                     // bytes per block; chunks per warp = ceil(nchunk / 32)
+    int blk_bytes, bpw;                     // bytes per block; chunks per warp = ceil(nchunk / (kChainCS * kChainWarps))
     int zp, one_scale, sd, out_f16;
     float scale0;
     int in_op;                              // producer op of x, or -1 (external input)
@@ -53,7 +56,8 @@ struct ChainOp {
 struct ChainParams {
     const ChainOp *ops;
     int nops;
-    int max_blk;                            // stage bytes per warp
+    int max_blk;                            // bytes per stage
+    int nstage;                             // stages per warp (>= 2): blocks are requested nstage - 1 blocks ahead
     unsigned int *bar;                      // grid barrier counter (barrier form; monotonic over launches)
     unsigned int *epochs;                   // [grid] launches seen by each CTA
     int *err;
@@ -120,36 +124,53 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
     const int rank = (int)cluster_ctarank(), rsb = blockIdx.x / CS;
     const int nclusters = gridDim.x / CS;
     const bool flow = !(p.flags & kChainBarrier);
-    // shared memory: cl [CS][RSB] (cluster partials, leader) | red [WPC][RSB] | per warp: 2 stages (max_blk) + table (NG * 8) |
-    //                mbar [WPC][2] (bulk copies) | rmbar (leader: the peers' partial sums have landed)
+    const int NS = p.nstage;
+    // shared memory: cl [CS][RSB] (cluster partials, leader) | red [WPC][RSB] | per warp: NS stages (max_blk) + table (NG * 8) |
+    //                mbar [WPC][NS] (bulk copies) | rmbar (leader: the peers' partial sums have landed)
     float *cl = reinterpret_cast<float *>(smem);
     float *red = cl + CS * RSB;
     unsigned char *wbase = reinterpret_cast<unsigned char *>(red + WPC * RSB);
-    const int per_warp = 2 * p.max_blk + NG * 8;
+    const int per_warp = NS * p.max_blk + NG * 8;
     unsigned char *stage0 = wbase + (size_t)warp * per_warp;
-    unsigned char *tab = stage0 + 2 * p.max_blk;
-    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + (size_t)WPC * per_warp) + 2 * warp;
-    uint64_t *rmbar = reinterpret_cast<uint64_t *>(wbase + (size_t)WPC * per_warp) + 2 * WPC;
+    unsigned char *tab = stage0 + (size_t)NS * p.max_blk;
+    uint64_t *mbar = reinterpret_cast<uint64_t *>(wbase + (size_t)WPC * per_warp) + NS * warp;
+    uint64_t *rmbar = reinterpret_cast<uint64_t *>(wbase + (size_t)WPC * per_warp) + NS * WPC;
     int nred = 0;                                                  // leader: reductions waited for (mbarrier phase)
     const unsigned epoch0 = p.epochs[blockIdx.x];                 // launches before this one
     const unsigned bar_base = epoch0 * (unsigned)p.nops * (unsigned)nclusters;
 
-    if (lane == 0) { mbar_init1(mbar); mbar_init1(mbar + 1); if (warp == 0) mbar_init1(rmbar); mbar_fence_init(); }
+    if (lane == 0) {
+        for (int s = 0; s < NS; ++s) mbar_init1(mbar + s);
+        if (warp == 0) mbar_init1(rmbar);
+        mbar_fence_init();
+    }
     __syncwarp();
     cluster_sync_all();                                            // every CTA of the cluster runs: its shared memory may be written
 
-    // stage buffer b <- the block of chunk c of op `op` for this warp (one bulk copy), if the warp has one
-    auto request = [&](int op, int c, int b) {
-        const ChainOp &o = p.ops[op];
-        if (rsb < o.nrsb && c < o.nchunk && lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            bulk_load(stage0 + (size_t)b * p.max_blk, o.W + (size_t)rsb * o.rsb_stride + (size_t)c * o.blk_bytes, (uint32_t)o.blk_bytes, mbar + b);
+    // The warp's block sequence: for op 0, 1, ... the chunks c_slot * bpw .. min(nchunk, (c_slot + 1) * bpw) - 1 (none where the CTA
+    // or the warp has no chunk).  Block j goes to stage j % NS, whose mbarrier it completes; stages are filled and consumed in ring
+    // order, so the consumer's mbarrier phase flips once per lap.
+    const int c_slot = rank * WPC + warp;
+    int rop = -1, rc = 0, rc_end = 0, rs = 0;                      // next block to request: op, chunk, end of the op's chunks; stage
+    // stage rs <- the next block of the sequence (one bulk copy), if there is one
+    auto request_next = [&]() {
+        while (rc >= rc_end) {
+            if (rop + 1 >= p.nops) return;
+            const ChainOp &o = p.ops[++rop];
+            rc = c_slot * o.bpw;
+            rc_end = rsb < o.nrsb ? min(o.nchunk, rc + o.bpw) : rc;
         }
+        const ChainOp &o = p.ops[rop];
+        if (lane == 0) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            bulk_load(stage0 + (size_t)rs * p.max_blk, o.W + (size_t)rsb * o.rsb_stride + (size_t)rc * o.blk_bytes, (uint32_t)o.blk_bytes, mbar + rs);
+        }
+        ++rc;
+        if (++rs == NS) rs = 0;
     };
-    int nload[2] = {0, 0};                                         // bulk copies waited for per stage (mbarrier phase)
-    const int c_slot = rank * WPC + warp;                          // this warp's chunk slot: chunks c_slot * bpw .. + bpw - 1
-    // op i's FIRST chunk always goes to stage (i & 1); further chunks of a multi-chunk op reuse the same stage
-    request(0, c_slot * p.ops[0].bpw, 0);
+    for (int s = 1; s < NS; ++s) request_next();                   // blocks 0 .. NS - 2
+    int cs = 0;                                                    // stage of the next block to consume
+    uint32_t cph = 0;                                              // its mbarrier phase
 
     for (int op = 0; op < p.nops; ++op) {
         const ChainOp &o = p.ops[op];
@@ -158,7 +179,6 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         const float *x = o.x;
         const bool active = rsb < o.nrsb;
         const int c_first = c_slot * bpw, c_end = min(nchunk, c_first + bpw);
-        const int sb = op & 1;                                     // this op's stage
         const uint32_t ep_in = epoch0 * (uint32_t)p.nops + (uint32_t)o.in_op + 1u, ep_out = epoch0 * (uint32_t)p.nops + (uint32_t)op + 1u;
         long long *tr = (p.trace && tid == 0) ? p.trace + ((size_t)op * gridDim.x + blockIdx.x) * 16 : nullptr;
         if (tr) tr[0] = chain_now();
@@ -176,7 +196,6 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         if (tr) tr[2] = chain_now();
         float cacc[RW];
         int iacc[RW];
-        bool requested = false;
 #pragma unroll
         for (int i = 0; i < RW; ++i) { cacc[i] = 0.f; iacc[i] = 0; }
         if (active)
@@ -229,15 +248,14 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                         lbsum += bias;
                     }
                 }
-                if (c > c_first) request(op, c, sb);               // later chunks of this op: same stage, reloaded
                 if (tr) tr[3] = chain_now();
-                if (!chain_mbar_wait(mbar + sb, nload[sb] & 1)) atomicExch(p.err, 2);
-                ++nload[sb];
+                if (!chain_mbar_wait(mbar + cs, cph)) atomicExch(p.err, 2);
                 __syncwarp();
                 if (tr) tr[4] = chain_now();
-                // the weight stream of the NEXT op starts with this op's lookups (other stage: its tenant, op - 1, is done)
-                if (c == c_first && op + 1 < p.nops) { request(op + 1, c_slot * p.ops[op + 1].bpw, sb ^ 1); requested = true; }
-                const unsigned char *stage = stage0 + (size_t)sb * p.max_blk;
+                // block j + NS - 1 is requested as block j's lookups start, into the stage of block j - 1 (its lookups ended with the
+                // __syncwarp at the end of the previous chunk; the proxy fence in request_next orders them before the bulk copy)
+                request_next();
+                const unsigned char *stage = stage0 + (size_t)cs * p.max_blk;
                 const uint4 *wp = reinterpret_cast<const uint4 *>(stage) + lane;
                 float facc[RW];
 #pragma unroll
@@ -263,10 +281,10 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                         cacc[i] = v;
                     }
                 }
-                __syncwarp();                                      // stage / table are rewritten by the next chunk
+                __syncwarp();                                      // stage / table are rewritten by later chunks
+                if (++cs == NS) { cs = 0; cph ^= 1u; }
             }
         if (tr) tr[5] = chain_now();
-        if (!requested && op + 1 < p.nops) request(op + 1, c_slot * p.ops[op + 1].bpw, sb ^ 1);   // warps without a block in this op
 
         // ---- CTA reduction (fixed warp order), cluster reduction in the leader's shared memory (rank order), leader stores the rows ----
         if (flow && op > 0) cluster_wait_acq();                    // every thread of the cluster is past op-1's reduction: red / cl may be rewritten
