@@ -151,9 +151,14 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
     // or the warp has no chunk).  Block j goes to stage j % NS, whose mbarrier it completes; stages are filled and consumed in ring
     // order, so the consumer's mbarrier phase flips once per lap.
     const int c_slot = rank * WPC + warp;
-    int rop = -1, rc = 0, rc_end = 0, rs = 0;                      // next block to request: op, chunk, end of the op's chunks; stage
-    // stage rs <- the next block of the sequence (one bulk copy), if there is one
-    auto request_next = [&]() {
+    int rop = -1, rc = 0, rc_end = 0, rs = 0;                      // sequence position: op, chunk, end of the op's chunks; stage
+    // The ChainOp fields of the next block to request are loaded one request ahead and only combined at the request: the request
+    // is made as a block's lookups start, and waiting there for global loads would delay the lookups once per block.
+    const unsigned char *nw = nullptr;                             // the next block to request: tensor (NULL: none left), super-
+    unsigned long long nstride = 0;                                // block stride, bytes per block, chunk
+    int nbytes = 0, nc = 0;
+    auto advance = [&]() {
+        nw = nullptr;
         while (rc >= rc_end) {
             if (rop + 1 >= p.nops) return;
             const ChainOp &o = p.ops[++rop];
@@ -161,13 +166,20 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
             rc_end = rsb < o.nrsb ? min(o.nchunk, rc + o.bpw) : rc;
         }
         const ChainOp &o = p.ops[rop];
+        nw = o.W; nstride = o.rsb_stride; nbytes = o.blk_bytes; nc = rc;
+        ++rc;
+    };
+    // stage rs <- the next block of the sequence (one bulk copy), if there is one
+    auto request_next = [&]() {
+        if (!nw) return;
         if (lane == 0) {
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            bulk_load(stage0 + (size_t)rs * p.max_blk, o.W + (size_t)rsb * o.rsb_stride + (size_t)rc * o.blk_bytes, (uint32_t)o.blk_bytes, mbar + rs);
+            bulk_load(stage0 + (size_t)rs * p.max_blk, nw + (size_t)rsb * nstride + (size_t)nc * nbytes, (uint32_t)nbytes, mbar + rs);
         }
-        ++rc;
         if (++rs == NS) rs = 0;
+        advance();
     };
+    advance();
     for (int s = 1; s < NS; ++s) request_next();                   // blocks 0 .. NS - 2
     int cs = 0;                                                    // stage of the next block to consume
     uint32_t cph = 0;                                              // its mbarrier phase
