@@ -21,9 +21,10 @@
 // bench.py times it on the bench chain (32 x 11008x4096 W2, x[i+1] = first K outputs of op i) beside the launch chain and
 // tmac_seq.cuh; flags bit 0 selects the grid-barrier form this kernel started as, kept for comparison.  Per-phase stamps
 // (ChainParams::trace) are read by tools/seq_bench.py --trace.
-// Same arithmetic as gemv3's fused path: LUT bytes identical to the preprocessor, fp32 sums in fixed (warp, then cluster rank)
-// order; the K split differs from the lone launch's, so results equal tmac_b200_gemv's up to fp32 re-association.  Waits are
-// bounded (error flag).
+// The LUT slices are built by lut_group, lut_addv8 and lut_bias (tmac_kernels.cuh), the functions the preprocessor and gemv3's
+// fused path build theirs with, so LUT bytes, scales and biases are identical to the preprocessor's; fp32 sums in fixed (warp,
+// then cluster rank) order; the K split differs from the lone launch's, so results equal tmac_b200_gemv's up to fp32
+// re-association.  Waits are bounded (error flag).
 #pragma once
 #include "tmac_kernels.cuh"
 #include "tmac_seq.cuh"     // {value, epoch} words: seq_publish
@@ -212,7 +213,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         for (int i = 0; i < RW; ++i) { cacc[i] = 0.f; iacc[i] = 0; }
         if (active)
             for (int c = c_first; c < c_end; ++c) {
-                // ---- LUT slice of this chunk -> warp-private table (lane = group); arithmetic = lut_ctor.cc:119-215 / :242-256 ----
+                // ---- LUT slice of this chunk -> warp-private table (lane = group) ----
                 float lsv[NAG], lbsum = 0.f;
                 {
                     float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
@@ -223,41 +224,15 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                         const float4 f = __ldcg(reinterpret_cast<const float4 *>(x + ((size_t)c * NG + lane) * 4));   // L2: written by other SMs
                         b0 = f.x; b1 = f.y; b2 = f.z; b3 = f.w;
                     }
-                    float m = __fadd_rn(__fadd_rn(fabsf(b0), fabsf(b1)), __fadd_rn(fabsf(b2), fabsf(b3)));
-#pragma unroll
-                    for (int s = WL / 2; s >= 1; s >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, s));
-                    const float scale = __fdiv_rn(m, 127.0f);
-                    const float ts = (scale != 0.0f) ? __fdiv_rn(1.0f, scale) : 0.0f;
-                    float od[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int idx = 2 * e + 1;
-                        float v = b0;
-                        v = (idx & 2) ? __fadd_rn(v, b1) : __fsub_rn(v, b1);
-                        v = (idx & 4) ? __fadd_rn(v, b2) : __fsub_rn(v, b2);
-                        v = (idx & 8) ? __fadd_rn(v, b3) : __fsub_rn(v, b3);
-                        od[e] = v;
-                    }
-                    uint32_t lo = 0, hi = 0;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const float lv = (e & 1) ? od[e >> 1] : -od[(15 - e) >> 1];
-                        int q = __float2int_rn(__fmul_rn(lv, ts));
-                        q = max(-128, min(127, q));
-                        if (e < 4) lo |= (uint32_t)(q & 0xff) << (8 * e); else hi |= (uint32_t)(q & 0xff) << (8 * (e - 4));
-                    }
+                    uint32_t lo, hi;
+                    float scale;
+                    const float l0 = lut_group<WL>(b0, b1, b2, b3, lo, hi, scale);
                     if (lane < NG) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
-                    float v = -od[7];
-                    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
-                    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-                    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
+                    const float blk = lut_addv8(l0);
 #pragma unroll
                     for (int a = 0; a < NAG; ++a) {
                         lsv[a] = __shfl_sync(0xffffffffu, scale, a * WL);
-                        float bias = 0.f;
-#pragma unroll
-                        for (int k = 0; k < WL / 8; ++k) bias = __fadd_rn(bias, __shfl_sync(0xffffffffu, v, a * WL + 8 * k));
-                        lbsum += bias;
+                        lbsum += lut_bias<WL>(blk, a * WL);
                     }
                 }
                 if (tr) tr[3] = chain_now();

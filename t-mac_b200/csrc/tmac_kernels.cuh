@@ -209,6 +209,70 @@ __device__ __forceinline__ float load_scale(const unsigned char *p, int sd, int 
     return sd == 2 ? __half2float(reinterpret_cast<const __half *>(p)[i]) : reinterpret_cast<const float *>(p)[i];
 }
 
+// ------------------------------------------------------------------------------------------
+// The activation LUT: the operation order of the AVX2 branch of lut_ctor.cc, with explicit round-to-nearest operations so
+// that no FMA contraction can change a rounding.  Every kernel that builds LUT bytes, LUT scales or LUT biases
+// (preprocessor_kernel, gemv3_kernel's FUSED path, chain_kernel, seq_kernel) builds them with these functions.
+// ------------------------------------------------------------------------------------------
+// abs-sum of one K-group, whose maximum over the activation group gives the LUT scale (lut_ctor.cc:242-256; association :251)
+__device__ __forceinline__ float lut_abs_sum(float x0, float x1, float x2, float x3) {
+    return __fadd_rn(__fadd_rn(fabsf(x0), fabsf(x1)), __fadd_rn(fabsf(x2), fabsf(x3)));
+}
+__device__ __forceinline__ float lut_scale(float abs_sum_max) { return __fdiv_rn(abs_sum_max, 127.0f); }              // :256
+__device__ __forceinline__ float lut_ts(float scale) { return (scale != 0.0f) ? __fdiv_rn(1.0f, scale) : 0.0f; }     // :124
+// odd entries od[i] = LUT[2i + 1] = ((x0 +- x1) +- x2) +- x3 (:133-151); LUT[14 - 2i] = -od[i] (:153-155), so LUT[0] = -od[7]
+__device__ __forceinline__ void lut_odd_entries(float x0, float x1, float x2, float x3, float *od) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const int idx = 2 * i + 1;
+        float v = x0;
+        v = (idx & 2) ? __fadd_rn(v, x1) : __fsub_rn(v, x1);
+        v = (idx & 4) ? __fadd_rn(v, x2) : __fsub_rn(v, x2);
+        v = (idx & 8) ? __fadd_rn(v, x3) : __fsub_rn(v, x3);
+        od[i] = v;
+    }
+}
+// int8 table entry: round half-even (:160-171), saturate as the packs (:173-176)
+__device__ __forceinline__ int lut_q8(float v, float ts) { return max(-128, min(127, __float2int_rn(__fmul_rn(v, ts)))); }
+// The 8 stored entries LUT[0..7] of the odd-symmetric table as int8 bytes lo | hi; returns LUT[0].
+__device__ __forceinline__ float lut_stored(float x0, float x1, float x2, float x3, float ts, uint32_t &lo, uint32_t &hi) {
+    float od[8];
+    lut_odd_entries(x0, x1, x2, x3, od);
+    lo = 0; hi = 0;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const uint32_t q = (uint32_t)(lut_q8((e & 1) ? od[e >> 1] : -od[(15 - e) >> 1], ts) & 0xff);
+        if (e < 4) lo |= q << (8 * e); else hi |= q << (8 * (e - 4));
+    }
+    return -od[7];
+}
+// _mm256_addv_ps of 8 consecutive lanes' values (lut_ctor.cc:24-31), the result in all 8 lanes.  All 32 lanes must call it.
+__device__ __forceinline__ float lut_addv8(float v) {
+    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
+    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
+    return __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
+}
+// Warp form, lane = K-group, WL lanes per activation group: the group's LUT scale and the lane's stored entries lo | hi; returns
+// the lane's LUT[0], whose lut_addv8 lut_bias sums into the group's bias.  All 32 lanes must call it.  (The kernels store lo | hi
+// before the addv8 shuffles: issued after them, the store costs the hot kernels extra instructions.)
+template <int WL>
+__device__ __forceinline__ float lut_group(float x0, float x1, float x2, float x3, uint32_t &lo, uint32_t &hi, float &scale) {
+    float m = lut_abs_sum(x0, x1, x2, x3);
+#pragma unroll
+    for (int s = WL / 2; s >= 1; s >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, s));
+    scale = lut_scale(m);
+    return lut_stored(x0, x1, x2, x3, lut_ts(scale), lo, hi);
+}
+// LUT bias of the activation group whose first lane is `first`, from blk = lut_addv8(LUT[0]): the serial sum over the group's
+// 8-lane blocks from 0 (:157), in every lane.
+template <int WL>
+__device__ __forceinline__ float lut_bias(float blk, int first) {
+    float bias = 0.f;
+#pragma unroll
+    for (int k = 0; k < WL / 8; ++k) bias = __fadd_rn(bias, __shfl_sync(0xffffffffu, blk, first + 8 * k));
+    return bias;
+}
+
 // ==========================================================================================
 // gemv3_kernel -- the production GEMV.
 //
@@ -329,9 +393,9 @@ constexpr int kG3MaxWarps = 8;
 
 // MINB = minimum resident CTAs per SM the register allocation is tuned for: 3 (85 registers, more ILP;
 // best for a single launch per tensor) or 4 (64 registers, more CTAs in flight; best for grouped launches).
-// FUSED = build the LUT slice of each chunk inside the GEMV from the activation row (same fp32 operation
-// order as preprocessor_kernel / lut_ctor.cc, so QLUT bytes, LUT scales and LUT biases are bit-identical to
-// the two-kernel path) instead of reading QLUT / LUT_Scales / LUT_Biases.  Requires SYM.  AGQ > 0: activation
+// FUSED = build the LUT slice of each chunk inside the GEMV from the activation row (with the LUT functions above,
+// as preprocessor_kernel, so QLUT bytes, LUT scales and LUT biases are bit-identical to the two-kernel path)
+// instead of reading QLUT / LUT_Scales / LUT_Biases.  Requires SYM.  AGQ > 0: activation
 // group inside a chunk, scale and bias per chunk by warp shuffles.  AGQ == 0 (integer path, ONE activation group
 // = the whole row, BitNet): every CTA scans the row once (K * 4 bytes, L2-resident) for the row-wide abs-sum
 // maximum -- cheaper than a cluster-wide exchange, which costs a rendezvous -- and the cluster leader also forms
@@ -379,6 +443,17 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     }
     const unsigned char *rsb_base = Wb + (size_t)rsb * p.rsb_stride;
     const int nag = p.K / p.ags;
+    // fused: the 4 activations from element k of the row, fp32 or fp16
+    auto load_group = [&](size_t k, float4 &x) {
+        const size_t k0 = (size_t)n * p.K + k;
+        if (p.act_f16) {
+            const uint2 h = __ldg(reinterpret_cast<const uint2 *>(reinterpret_cast<const __half *>(p.act) + k0));
+            const float2 f01 = __half22float2(*reinterpret_cast<const __half2 *>(&h.x)), f23 = __half22float2(*reinterpret_cast<const __half2 *>(&h.y));
+            x.x = f01.x; x.y = f01.y; x.z = f23.x; x.w = f23.y;
+        } else {
+            x = __ldg(reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p.act) + k0));
+        }
+    };
 
     // ---- first chunk: HBM -> shared, issued before the dependency wait -------------------------
     if (lane == 0) {
@@ -414,30 +489,18 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         float *wmax = iscr + nblk, *bias_out = wmax + kG3MaxWarps, *cmax = bias_out + 4;
         scan_split = p.cs > 1 && ngrp > 4 * nth;
         const bool bias_cta = rank == p.cs - 1;
-        auto load_group = [&](int gi, float &b0, float &b1, float &b2, float &b3) {
-            const size_t k0 = (size_t)n * p.K + (size_t)gi * 4;
-            if (p.act_f16) {
-                const uint2 h = __ldg(reinterpret_cast<const uint2 *>(reinterpret_cast<const __half *>(p.act) + k0));
-                const float2 f01 = __half22float2(*reinterpret_cast<const __half2 *>(&h.x)), f23 = __half22float2(*reinterpret_cast<const __half2 *>(&h.y));
-                b0 = f01.x; b1 = f01.y; b2 = f23.x; b3 = f23.y;
-            } else {
-                const float4 f = __ldg(reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p.act) + k0));
-                b0 = f.x; b1 = f.y; b2 = f.z; b3 = f.w;
-            }
-        };
-        // K-groups [gbeg, gend): LUT[0] = -LUT[15] of every group (:133-155), _mm256_addv_ps tree per block of 32 activations = 8
-        // lanes (lut_ctor.cc:24-31, as in the fp path below), block sums -> the bias CTA; returns the abs-sum maximum (:242-256)
+        // K-groups [gbeg, gend): LUT[0] of every group, addv8 per block of 32 activations = 8 lanes, block sums -> the bias CTA;
+        // returns the abs-sum maximum
         auto scan = [&](int gbeg, int gend, bool want_max, bool remote) {
             float mm = 0.f;
             for (int g0 = gbeg + warp * 32; g0 < gend; g0 += nth) {   // lane = K-group (coalesced 16-byte loads)
                 const int gi = g0 + lane;
-                float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
-                if (gi < gend) load_group(gi, b0, b1, b2, b3);
-                if (want_max) mm = fmaxf(mm, __fadd_rn(__fadd_rn(fabsf(b0), fabsf(b1)), __fadd_rn(fabsf(b2), fabsf(b3))));
-                float v = -__fadd_rn(__fadd_rn(__fadd_rn(b0, b1), b2), b3);
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
+                float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (gi < gend) load_group((size_t)gi * 4, x);
+                if (want_max) mm = fmaxf(mm, lut_abs_sum(x.x, x.y, x.z, x.w));
+                float od[8];
+                lut_odd_entries(x.x, x.y, x.z, x.w, od);
+                const float v = lut_addv8(-od[7]);
                 if ((lane & 7) == 0 && gi < gend) {
                     if (remote) st_cluster_f32(iscr + (gi >> 3), p.cs - 1, v); else iscr[gi >> 3] = v;
                 }
@@ -454,15 +517,15 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             // request at a time)
             const int off = (int)(((long long)blockIdx.x * 160) % ngrp);
             for (int g = tid; g < ngrp; g += 4 * nth) {
-                float b[4][4];
+                float4 b[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int gj = g + j * nth;
-                    b[j][0] = b[j][1] = b[j][2] = b[j][3] = 0.f;
-                    if (gj < ngrp) { int gi = gj + off; if (gi >= ngrp) gi -= ngrp; load_group(gi, b[j][0], b[j][1], b[j][2], b[j][3]); }
+                    b[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (gj < ngrp) { int gi = gj + off; if (gi >= ngrp) gi -= ngrp; load_group((size_t)gi * 4, b[j]); }
                 }
 #pragma unroll
-                for (int j = 0; j < 4; ++j) m = fmaxf(m, __fadd_rn(__fadd_rn(fabsf(b[j][0]), fabsf(b[j][1])), __fadd_rn(fabsf(b[j][2]), fabsf(b[j][3]))));
+                for (int j = 0; j < 4; ++j) m = fmaxf(m, lut_abs_sum(b[j].x, b[j].y, b[j].z, b[j].w));
             }
             if (bias_cta) scan(0, ngrp, false, false);           // L1 hits
         }
@@ -478,8 +541,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             m = cmax[0];
             for (int r = 1; r < p.cs; ++r) m = fmaxf(m, cmax[r]);
         }
-        row_scale = __fdiv_rn(m, 127.0f);
-        row_ts = (row_scale != 0.0f) ? __fdiv_rn(1.0f, row_scale) : 0.0f;
+        row_scale = lut_scale(m);
+        row_ts = lut_ts(row_scale);
         if (bias_cta && warp == WPC - 1) {
             // serial over the blocks of the (single) activation group, from 0 (:157).  32 values per shared-memory round trip,
             // the 32 shuffles of a round issued ahead of the dependent adds (fixed trip count); the tail is padded with +0.0,
@@ -500,63 +563,21 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         // ---- LUT slice of this chunk -> warp-private table (lane = group) ---------------------
         float lsv[NAG], lbsum = 0.f;
         if (FUSED) {
-            // lane = K-group of the chunk; W = lanes per activation group.  Arithmetic = lut_ctor.cc:119-215
-            // (AVX2 branch) and partial_max_g4_int8_k8 (:242-256), all with explicit round-to-nearest ops.
+            // lane = K-group of the chunk; W = lanes per activation group
             constexpr int NG = QCH * 4, W = (AGQ ? AGQ : 1) * 4;
-            float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
-            if (lane < NG) {
-                const size_t k0 = (size_t)n * p.K + ((size_t)c * NG + lane) * 4;
-                if (p.act_f16) {
-                    const uint2 h = __ldg(reinterpret_cast<const uint2 *>(reinterpret_cast<const __half *>(p.act) + k0));
-                    const float2 f01 = __half22float2(*reinterpret_cast<const __half2 *>(&h.x)), f23 = __half22float2(*reinterpret_cast<const __half2 *>(&h.y));
-                    b0 = f01.x; b1 = f01.y; b2 = f23.x; b3 = f23.y;
-                } else {
-                    const float4 f = __ldg(reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p.act) + k0));
-                    b0 = f.x; b1 = f.y; b2 = f.z; b3 = f.w;
-                }
-            }
-            float scale, ts;
-            if (INT_PATH) { scale = row_scale; ts = row_ts; }
-            else {
-                float m = __fadd_rn(__fadd_rn(fabsf(b0), fabsf(b1)), __fadd_rn(fabsf(b2), fabsf(b3)));
-#pragma unroll
-                for (int o = W / 2; o >= 1; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                scale = __fdiv_rn(m, 127.0f);
-                ts = (scale != 0.0f) ? __fdiv_rn(1.0f, scale) : 0.0f;
-            }
-            float od[8];                                   // odd entries 1,3,...,15
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const int idx = 2 * e + 1;
-                float v = b0;
-                v = (idx & 2) ? __fadd_rn(v, b1) : __fsub_rn(v, b1);
-                v = (idx & 4) ? __fadd_rn(v, b2) : __fsub_rn(v, b2);
-                v = (idx & 8) ? __fadd_rn(v, b3) : __fsub_rn(v, b3);
-                od[e] = v;
-            }
-            // stored entries 0..7: even e = -LUT[15-e] (= -od[(15-e)/2]), odd e = od[e/2]
-            uint32_t lo = 0, hi = 0;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const float lv = (e & 1) ? od[e >> 1] : -od[(15 - e) >> 1];
-                int q = __float2int_rn(__fmul_rn(lv, ts));
-                q = max(-128, min(127, q));
-                if (e < 4) lo |= (uint32_t)(q & 0xff) << (8 * e); else hi |= (uint32_t)(q & 0xff) << (8 * (e - 4));
-            }
+            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (lane < NG) load_group(((size_t)c * NG + lane) * 4, x);
+            uint32_t lo, hi;
+            float scale, l0;
+            if (INT_PATH) lut_stored(x.x, x.y, x.z, x.w, row_ts, lo, hi);
+            else l0 = lut_group<W>(x.x, x.y, x.z, x.w, lo, hi, scale);
             if (lane < NG) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
             if (!INT_PATH) {
-                // LUT bias: _mm256_addv_ps tree per 8 groups (lut_ctor.cc:24-31), serial over the blocks of a group (:157)
-                float v = -od[7];                          // LUT[0] = -LUT[15]
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-                v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
+                const float blk = lut_addv8(l0);
 #pragma unroll
                 for (int a = 0; a < NAG; ++a) {
                     lsv[a] = __shfl_sync(0xffffffffu, scale, a * W);
-                    float bias = 0.f;
-#pragma unroll
-                    for (int k = 0; k < W / 8; ++k) bias = __fadd_rn(bias, __shfl_sync(0xffffffffu, v, a * W + 8 * k));
-                    lbsum += bias;
+                    lbsum += lut_bias<W>(blk, a * W);
                 }
             }
         } else {
@@ -726,8 +747,7 @@ static __global__ void cbits_kernel(const unsigned char *W, const int8_t *qlut, 
 // ------------------------------------------------------------------------------------------
 // preprocessor_kernel.  grid = (ceil(nag / agb), N); block = 256.
 // Each CTA handles `agb` consecutive activation groups of one activation row (agb == nag when
-// act_group_size == K, i.e. a single CTA per row).  fp32 op order identical to the AVX2 branch of
-// lut_ctor.cc (no FMA: only adds, one IEEE division, one IEEE reciprocal, one multiply per entry).
+// act_group_size == K, i.e. a single CTA per row).  Entries and scales by the LUT functions above.
 // ------------------------------------------------------------------------------------------
 constexpr int kPreThreads = 256;
 
@@ -759,43 +779,29 @@ __global__ void __launch_bounds__(kPreThreads) preprocessor_kernel(const TIn *B,
     for (int a = tid; a < a_end - a_begin; a += kPreThreads) smax[a] = 0;
     asm volatile("griddepcontrol.wait;" ::: "memory");
     __syncthreads();
-    // pass 1: abs-sum max per act group (lut_ctor.cc:242-256; association (a0+a1)+(a2+a3) :251)
+    // pass 1: abs-sum max per act group
     for (int g = tid; g < ng; g += kPreThreads) {
         const size_t k0 = (size_t)(g_begin + g) * 4;
-        const float a0 = fabsf(ld_act(b, k0)), a1 = fabsf(ld_act(b, k0 + 1));
-        const float a2 = fabsf(ld_act(b, k0 + 2)), a3 = fabsf(ld_act(b, k0 + 3));
-        const float s = __fadd_rn(__fadd_rn(a0, a1), __fadd_rn(a2, a3));
-        atomicMax(&smax[g / gpa], __float_as_int(s));
+        const float b0 = ld_act(b, k0), b1 = ld_act(b, k0 + 1), b2 = ld_act(b, k0 + 2), b3 = ld_act(b, k0 + 3);
+        atomicMax(&smax[g / gpa], __float_as_int(lut_abs_sum(b0, b1, b2, b3)));
     }
     __syncthreads();
     // pass 2: tables
     for (int g = tid; g < ng; g += kPreThreads) {
         const size_t k0 = (size_t)(g_begin + g) * 4;
         const float b0 = ld_act(b, k0), b1 = ld_act(b, k0 + 1), b2 = ld_act(b, k0 + 2), b3 = ld_act(b, k0 + 3);
-        const float scale = __fdiv_rn(__int_as_float(smax[g / gpa]), 127.0f);      // :256
-        const float ts = (scale != 0.0f) ? __fdiv_rn(1.0f, scale) : 0.0f;          // :124
-        float lut[16];
+        const float ts = lut_ts(lut_scale(__int_as_float(smax[g / gpa])));
+        float od[8], lut[16];
+        lut_odd_entries(b0, b1, b2, b3, od);
 #pragma unroll
-        for (int e = 1; e < 16; e += 2) {                                          // :133-151
-            float v = b0;
-            v = (e & 2) ? __fadd_rn(v, b1) : __fsub_rn(v, b1);
-            v = (e & 4) ? __fadd_rn(v, b2) : __fsub_rn(v, b2);
-            v = (e & 8) ? __fadd_rn(v, b3) : __fsub_rn(v, b3);
-            lut[e] = v;
-        }
-#pragma unroll
-        for (int e = 0; e < 16; e += 2) lut[e] = -lut[15 - e];                     // :153-155
+        for (int e = 0; e < 16; e += 2) { lut[e + 1] = od[e / 2]; lut[e] = -od[(15 - e) / 2]; }
         l0[g] = lut[0];
         uint32_t packed[4];
 #pragma unroll
         for (int w = 0; w < 4; ++w) {
             uint32_t acc = 0;
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                int q = __float2int_rn(__fmul_rn(lut[4 * w + e], ts));             // :160-171 (rne)
-                q = max(-128, min(127, q));                                       // packs saturation :173-176
-                acc |= (uint32_t)(q & 0xff) << (8 * e);
-            }
+            for (int e = 0; e < 4; ++e) acc |= (uint32_t)(lut_q8(lut[4 * w + e], ts) & 0xff) << (8 * e);
             packed[w] = acc;
         }
         reinterpret_cast<uint4 *>(qlut + (size_t)n * K * 4)[g_begin + g] = make_uint4(packed[0], packed[1], packed[2], packed[3]);
@@ -815,7 +821,7 @@ __global__ void __launch_bounds__(kPreThreads) preprocessor_kernel(const TIn *B,
         float bias = 0.0f;
         for (int k = 0; k < bpa; ++k) bias = __fadd_rn(bias, blk[a * bpa + k]);
         lut_biases[(size_t)n * nag + a_begin + a] = bias;
-        lut_scales[(size_t)n * nag + a_begin + a] = __fdiv_rn(__int_as_float(smax[a]), 127.0f);
+        lut_scales[(size_t)n * nag + a_begin + a] = lut_scale(__int_as_float(smax[a]));
     }
 }
 

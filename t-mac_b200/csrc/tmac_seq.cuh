@@ -12,9 +12,10 @@
 //     slot is reused when every consumer warp has published a progress counter beyond it.  HBM therefore runs
 //     ~2 GEMVs ahead of the arithmetic, across the data dependencies, because weights do not depend on activations;
 //   * 20 consumer warps per CTA do, per op: (A) build the LUT slices of the CTA's K chunks from the op's input
-//     vector (same fp32 operation order as preprocessor_kernel / lut_ctor.cc -> bit-identical tables), (B) the
-//     PRMT + DP4A lookups (Quad<>::run, as gemv3) over an arithmetic "stream-K" share of the op's blocks -- CTA c owns
-//     blocks [T*c/G, T*(c+1)/G), a warp owns a contiguous run of activation-group units inside them --, (C) reduce
+//     vector (lut_group, lut_addv8 and lut_bias of tmac_kernels.cuh, the LUT functions preprocessor_kernel uses
+//     -> bit-identical tables), (B) the PRMT + DP4A lookups (Quad<>::run, as gemv3) over an arithmetic "stream-K"
+//     share of the op's blocks -- CTA c owns blocks [T*c/G, T*(c+1)/G), a warp owns a contiguous run of
+//     activation-group units inside them --, (C) reduce
 //     the warps through shared memory in fixed order and finish the rows;
 //   * rows whose K range is split between CTAs are finished by the LAST CTA that touches them: the earlier ones
 //     publish their partial sums through 8-byte {value, epoch} slots in global memory (one store, one polling load
@@ -121,42 +122,6 @@ __device__ __forceinline__ bool seq_mbar_wait(uint64_t *b, uint32_t parity) {
 __device__ __forceinline__ int ld_volatile_s32(const int *p) { int v; asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory"); return v; }
 __device__ __forceinline__ void st_volatile_s32(int *p, int v) { asm volatile("st.volatile.shared.s32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory"); }
 
-// One K-group of the activation LUT: lanes = consecutive K-groups, WL lanes per activation group.  Arithmetic = lut_ctor.cc:119-215
-// (AVX2 branch) and partial_max_g4_int8_k8 (:242-256) with explicit round-to-nearest operations, as preprocessor_kernel:
-// lo | hi = the 8 stored int8 entries, scale = LUT scale of the lane's activation group, bias = its LUT bias (valid in the
-// group's first lane).  All 32 lanes must call it.
-template <int WL>
-__device__ __forceinline__ void lut_group(float x0, float x1, float x2, float x3, int lane, uint32_t &lo, uint32_t &hi, float &scale, float &bias) {
-    float m = __fadd_rn(__fadd_rn(fabsf(x0), fabsf(x1)), __fadd_rn(fabsf(x2), fabsf(x3)));
-#pragma unroll
-    for (int s = WL / 2; s >= 1; s >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, s));
-    scale = __fdiv_rn(m, 127.0f);
-    const float ts = (scale != 0.0f) ? __fdiv_rn(1.0f, scale) : 0.0f;
-    // odd entries 1, 3, ..., 15: ((x0 +- x1) +- x2) +- x3
-    const float p01 = __fadd_rn(x0, x1), m01 = __fsub_rn(x0, x1);
-    const float a0 = __fsub_rn(m01, x2), a1 = __fsub_rn(p01, x2), a2 = __fadd_rn(m01, x2), a3 = __fadd_rn(p01, x2);
-    float od[8];
-    od[0] = __fsub_rn(a0, x3); od[1] = __fsub_rn(a1, x3); od[2] = __fsub_rn(a2, x3); od[3] = __fsub_rn(a3, x3);
-    od[4] = __fadd_rn(a0, x3); od[5] = __fadd_rn(a1, x3); od[6] = __fadd_rn(a2, x3); od[7] = __fadd_rn(a3, x3);
-    lo = 0; hi = 0;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {               // stored entry e: even = -LUT[15-e], odd = LUT[e]
-        const float lv = (e & 1) ? od[e >> 1] : -od[(15 - e) >> 1];
-        // round-to-nearest-even of lv * ts as the reference's cvtps_epi32 (:160-171), through the 1.5 * 2^23 trick on the
-        // FMA pipe instead of 8 F2I on the conversion unit; |lv * ts| <= 127.0001 (ts = 1 / (max / 127)), so the
-        // saturating pack (:173-176) never clips a finite input and the low byte is the int8 value.
-        const uint32_t q = __float_as_uint(__fadd_rn(__fmul_rn(lv, ts), 12582912.0f));
-        if (e < 4) lo |= (q & 0xffu) << (8 * e); else hi |= (q & 0xffu) << (8 * (e - 4));
-    }
-    // LUT bias: _mm256_addv_ps tree per 8 groups (lut_ctor.cc:24-31), serial over the blocks of a group (:157)
-    float v = -od[7];
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 4));
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    bias = 0.f;
-#pragma unroll
-    for (int k = 0; k < WL / 8; ++k) bias = __fadd_rn(bias, __shfl_sync(0xffffffffu, v, (lane & ~(WL - 1)) + 8 * k));
-}
 __device__ __forceinline__ void seq_publish16(uint4 *slot, uint32_t a, uint32_t b, uint32_t epoch) {
     // two 8-byte {value, epoch} words written by ONE 16-byte store; each half is valid on its own
     asm volatile("st.relaxed.gpu.global.v4.u32 [%0], {%1, %2, %3, %2};" ::"l"(slot), "r"(a), "r"(epoch), "r"(b) : "memory");
@@ -322,8 +287,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                     }
                 }
                 uint32_t lo, hi;
-                float scale, bias;
-                lut_group<WL>(x0, x1, x2, x3, lane, lo, hi, scale, bias);
+                float scale;
+                const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(x0, x1, x2, x3, lo, hi, scale)), lane & ~(WL - 1));
                 if (valid) reinterpret_cast<uint2 *>(tabs + (size_t)ci * TAB)[gl] = make_uint2(lo, hi);
                 if (valid && (gl % WL) == 0) {
                     d[gl / WL] = scale;
@@ -483,7 +448,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
         }
         if (lut_out) {
             // the consumer's preprocessor for the rows finished here (row super-blocks that end in this CTA): thread = K-group of
-            // 4 consecutive rows, same arithmetic as the consumer-side build
+            // 4 consecutive rows, built as on the consumer side
             const int nfin = nseg - last_open;
             constexpr int GPS = RSB / 4;                        // K-groups per row super-block
             constexpr int GPSW = (GPS + 31) & ~31;              // ... rounded up to whole warps
@@ -498,8 +463,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                         const float4 f = valid ? reinterpret_cast<const float4 *>(yfin)[s * GPS + t] : make_float4(0.f, 0.f, 0.f, 0.f);
                         if (tw) tw[9] = clock64() + (f.x == 1.2345e-30f);
                         uint32_t lo, hi;
-                        float scale, bias;
-                        lut_group<WL>(f.x, f.y, f.z, f.w, lane, lo, hi, scale, bias);
+                        float scale;
+                        const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(f.x, f.y, f.z, f.w, lo, hi, scale)), lane & ~(WL - 1));
                         if (tw) tw[10] = clock64() + (lo == 0x12345678u);
                         if (valid) {
                             const size_t g = (size_t)(sb_first + s) * GPS + t;
@@ -515,8 +480,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                     const bool valid = t < nfin * GPS;
                     const float4 f = valid ? reinterpret_cast<const float4 *>(yfin)[t] : make_float4(0.f, 0.f, 0.f, 0.f);
                     uint32_t lo, hi;
-                    float scale, bias;
-                    lut_group<WL>(f.x, f.y, f.z, f.w, lane, lo, hi, scale, bias);
+                    float scale;
+                    const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(f.x, f.y, f.z, f.w, lo, hi, scale)), lane & ~(WL - 1));
                     if (valid) {
                         const size_t g = (size_t)sb_first * GPS + t;    // finished super-blocks are my first nfin ones
                         seq_publish16(lut_out + g, lo, hi, epoch);
