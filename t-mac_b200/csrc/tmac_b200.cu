@@ -117,9 +117,9 @@ struct Context {
     int seq_impl = 2;                    // decode sequences: 0 = stream-K sequence kernel (tmac_seq.cuh), 1 = resident gemv3 chain (tmac_chain.cuh), 2 = chain when the sequence qualifies
     int seq_smem_kb = 200;               // decode sequences: shared-memory budget; the rest of the 228 KB stays L1 (descriptor / polling loads, spills)
     int seq_grid = 0;                    // decode sequences: grid override (tests: CTA-boundary placements); 0 = one CTA per SM
-    int use_prefill16 = 1;               // fp16-operand prefill tile for N >= 64 (tmac_prefill16.cuh); 0 = the exact int8 tile for every N >= prefill_min_n
+    int use_prefill16 = 1;               // fp16-operand prefill tile for N >= 64 (tmac_prefill16.cuh); 0 = the exact int8 tile for every N >= tile_min_n
     int pf_streamk = 0;                  // stream-K over all SMs when a prefill call has fewer tiles than SMs (measured slower: B delivery from L2 is the bound)
-    int use_prefill = 1, prefill_min_n = 32;   // N >= prefill_min_n: wgmma int8 tile (W2 g128 act64)
+    int use_prefill = 1, prefill_min_n = 0;    // N >= prefill_min_n: the wgmma tiles (W2, W3/W4 g128 act64); 0 = by shape (tile_min_n)
     int npeer = 0; void *peer_out[7] = {};   // one-shot: peer output vectors of the next N = 1 launch (tmac_b200_peer_outputs)
     int64_t next_hint = 0;               // one-shot: tensor whose blocks the next launch prefetches into L2
     std::map<int64_t, Resident> res;
@@ -409,16 +409,27 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
     return 0;
 }
 
+// Smallest N that takes a prefill tile (unless set with the prefill_min_n knob).  W2: 32.  W3/W4: 32 as well, but a tensor of fewer
+// than 64 row tiles of 128 rows (the 4096-row Llama-2 projections: 32) fills a quarter of the SMs with one token tile, and there the
+// tiles overtake the W4 GEMV only between N = 64 and 128 (H100 SXM at 400 W, DESIGN.md 3.3): 128.
+int tile_min_n(const StreamLayout &L) {
+    if (g.prefill_min_n > 0) return g.prefill_min_n;
+    return (L.pb == 4 && (L.nrsb + 1) / 2 < 64) ? 128 : 32;
+}
+
 // Prefill tile on the tensor cores (wgmma, tmac_prefill.cuh).  Returns 1 if the shape is not covered (caller falls back to the GEMV
 // kernel per activation row), 0 on launch, -1 on error.
 int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls, const float *lb, void *C, int ldc, int out_f16, bool sym) {
     const StreamLayout &L = R.L;
-    if (!g.use_prefill || N < g.prefill_min_n || !sym) return 1;
-    if (L.pb != 2 || L.qch != 8 || L.act_group_size != 64 || L.one_scale || L.ck != 128) return 1;
+    if (!g.use_prefill || N < tile_min_n(L) || !sym) return 1;
+    if ((L.pb != 2 && L.pb != 4) || L.qch != 8 || L.act_group_size != 64 || L.one_scale || L.ck != 128) return 1;
     const size_t rawsz = (L.blk + 127) & ~(size_t)127;
+    // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
+    const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
+    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = L.pb == 4 ? 512 * 8 : 0;   // + the PB 4 expansion table
     if (g.use_prefill16 && N >= 64) {   // fp path: scales folded into fp16 operands, fp32 accumulation over K in registers (tmac_prefill16.cuh)
         const int nmain = L.K / 64, nextra = (L.nchunk + 31) / 32, ntile16 = (N + kP16NT - 1) / kP16NT;
-        const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + 2 * rawsz + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
+        const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + xtab + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
         if (smem16 <= 227 * 1024) {
             if (g.d_tiles.ensure((size_t)ntile16 * (nmain + nextra) * kP16BBytes)) return fail("out of device memory (LUT tiles)");
             lut_tile16_kernel<<<dim3(nmain + nextra, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, nmain, nextra);
@@ -427,7 +438,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
             q.W = R.d; q.C = C; q.N = N; q.K = L.K; q.Mout = L.Mout; q.ldc = ldc; q.out_f16 = out_f16;
             q.nchunk = L.nchunk; q.zp = L.zp; q.sd = L.sd; q.blk_bytes = (int)L.blk; q.nmain = nmain; q.nextra = nextra;
             q.rsb_stride = L.rsb_stride; q.tiles = (const unsigned char *)g.d_tiles.p;
-            q.nrsb = L.nrsb; q.ntiles = L.nrsb * ntile16;
+            q.nrsb = L.nrsb; q.nrt = nrt; q.bits = L.bits; q.ntiles = nrt * ntile16;
             // fewer tiles than SMs (e.g. 86 at N = 256): stream-K over all SMs, partial tiles through `scratch`
             q.streamk = (g.pf_streamk && q.ntiles < g.sms && (long)q.ntiles * (nmain + nextra) >= 2L * g.sms) ? 1 : 0;
             const int grid = q.streamk ? g.sms : q.ntiles;
@@ -440,15 +451,17 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
                 }
                 q.scratch = (float *)g.d_pf_scratch.p; q.flags = (int *)g.d_pf_flags.p;
             }
-            CUDA_OK(cudaFuncSetAttribute((const void *)prefill16_w2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
-            prefill16_w2_kernel<<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
+            const void *fn16 = L.pb == 4 ? (const void *)prefill16_kernel<4> : (const void *)prefill16_kernel<2>;
+            CUDA_OK(cudaFuncSetAttribute(fn16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
+            if (L.pb == 4) prefill16_kernel<4><<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
+            else prefill16_kernel<2><<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
             CUDA_OK(cudaGetLastError());
             g.last_launch[0] = 16; g.last_launch[1] = kP16Threads / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = q.streamk; g.last_launch[4] = grid;
             g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;
             return 0;
         }
     }
-    const size_t smem = (size_t)kPfStages * (kPfStageBytes + kPfRec) + 2 * rawsz + 256 * 8 + (2 * kPfStages + 4) * 8 + 1024;
+    const size_t smem = (size_t)kPfStages * (kPfStageBytes + kPfRec) + rawall + (L.pb == 4 ? 512 : 256) * 8 + (2 * kPfStages + 4) * 8 + 1024;
     if (smem > 225 * 1024) return 1;
     const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;
     if (g.d_tiles.ensure((size_t)ntile * nag * kPfRec)) return fail("out of device memory (LUT tiles)");
@@ -459,16 +472,19 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
     p.lut_tiles = (const unsigned char *)g.d_tiles.p;
     p.N = N; p.K = L.K; p.Mout = L.Mout; p.ldc = ldc; p.out_f16 = out_f16;
     p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride;
+    p.nrsb = L.nrsb; p.bits = L.bits;
     if (g.trace) {
         if (g.d_trace.ensure(8192)) return fail("out of device memory (trace)");
         CUDA_OK(cudaMemsetAsync(g.d_trace.p, 0, 3 * 32 * 4 * sizeof(long long), g.stream()));
         p.dbg = (long long *)g.d_trace.p; g.trace_ctas = 12;   // 96 rows of 4 = 48 rows of 8
     }
-    CUDA_OK(cudaFuncSetAttribute((const void *)prefill_w2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(L.nrsb, ntile);
-    prefill_w2_kernel<<<grid, kPfThreads2, smem, g.stream()>>>(p);
+    const void *fn = L.pb == 4 ? (const void *)prefill_kernel<4> : (const void *)prefill_kernel<2>;
+    CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid(nrt, ntile);
+    if (L.pb == 4) prefill_kernel<4><<<grid, kPfThreads2, smem, g.stream()>>>(p);
+    else prefill_kernel<2><<<grid, kPfThreads2, smem, g.stream()>>>(p);
     CUDA_OK(cudaGetLastError());
-    g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = 1; g.last_launch[4] = L.nrsb;
+    g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = 1; g.last_launch[4] = nrt;
     g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;   // batch < 0 marks the tensor-core prefill tile
     return 0;
 }
@@ -1223,7 +1239,7 @@ int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {
     const int kind_b = ptr_kind(B, &pinB), kind_c = ptr_kind(C, &pinC);
     const bool dev_b = kind_b == 2, dev_c = kind_c == 2;
     const bool int_path = L.one_scale && L.act_group_size == L.K;
-    const bool prefill_shape = g.use_prefill && N >= g.prefill_min_n && L.pb == 2 && L.qch == 8 && L.act_group_size == 64 && !L.one_scale;
+    const bool prefill_shape = g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && L.qch == 8 && L.act_group_size == 64 && !L.one_scale;
     const bool can_fuse = g.use_fused && (int_path || L.act_group_size <= L.ck) && g.lut_mode != 1 && !prefill_shape;
     auto launch_compute = [&](const void *dB, void *dC) -> int {
         if (can_fuse)   // one launch: the GEMV builds each chunk's LUT slice itself (bit-identical tables)

@@ -15,13 +15,15 @@
 // rank-(K/group_size) correction added once per chunk.
 //
 //   warpgroups 0, 1  consumers: 4 wgmma per step on rows 64*wg .. 64*wg+63, int32 -> fp32 fold, final store.
-//   warpgroup  2     producers: cp.async the (row super-block, chunk) block, expand the packed codes of "their"
-//                    weight row into S (one 64-bit one-hot-signed vector per (row, group), through a 256-entry
-//                    shared-memory table) in the K-major no-swizzle canonical layout; fence.proxy.async; arrive
-//                    full[s].  Thread 0 also issues the step's LUT record as one bulk copy (TMA) into the same stage.
+//   warpgroup  2     producers: cp.async the (row super-block, chunk) block(s), expand the packed codes of "their"
+//                    weight row into S (one 64-bit one-hot-signed vector per (row, group), through a 256-entry (W2) or
+//                    512-entry (W3/W4: two planes per lookup, two lookups added byte-wise) shared-memory table) in the
+//                    K-major no-swizzle canonical layout; fence.proxy.async; arrive full[s].  Thread 0 also issues the
+//                    step's LUT record as one bulk copy (TMA) into the same stage.
 //
-// Supported: PB == 2 (W2), chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points),
-// symmetric LUT.  Everything else takes the GEMV kernel once per activation row.
+// Supported: PB == 2 (W2: a 128-row tile is one super-block) and PB == 4 (W3/W4: two 64-row super-blocks, one per consumer
+// warpgroup), chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points), symmetric LUT.  Everything else
+// takes the GEMV kernel once per activation row.
 #pragma once
 #include "tmac_kernels.cuh"
 
@@ -37,6 +39,7 @@ struct PrefillParams {
     size_t rsb_stride;
     const unsigned char *lut_tiles; // output of lut_tile_kernel: [token tile][step][kPfRec]
     long long *dbg;                // optional trace [role][step][4] (TMAC_ENABLE_TRACE builds)
+    int nrsb, bits;                // row super-blocks of the tensor (PB 4: the last row tile may hold only one), bit width
 };
 #ifdef TMAC_ENABLE_TRACE
 #define PF_TRACE(role, step, k) do { if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && (step) < 32) p.dbg[((role) * 32 + (step)) * 4 + (k)] = clock64(); } while (0)
@@ -131,60 +134,101 @@ __device__ __forceinline__ void pf_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(pf_s32(bar)), "r"(bytes) : "memory");
 }
 
-// grid = (row super-blocks of 128 rows, ceil(N / 128)), block = 384 threads, 1 CTA per SM.
+// PB 4 expansion table: 512 entries, each indexed by one byte of a row's 16-bit code field (two planes, nibble = neg << 3 | j),
+//   [0, 256)    planes 0, 1: +-w0 at byte j0 plus +-w1 at byte j1
+//   [256, 512)  planes 2, 3: +-w2 at byte j2 plus +-w3 at byte j3
+// w_b = 2*alpha_b from plane_weight_regs: {1, 2, 4, 8}, W3 {1, 2, 4, 0} (its padded fourth plane is code 0 and must add nothing).
+// biased == false: signed bytes, one entry of each half added byte-wise (__vadd4) is S[e].  biased == true: the bytes of the two
+// halves carry +3 and +13 (|w0| + |w1| <= 3, |w2| + |w3| <= 12), so every byte is non-negative and a plain 32-bit add of one entry
+// of each half holds S[e] + 16 in [1, 31] per byte without a carry between bytes.
+__device__ __forceinline__ void pf_build_xtab4(uint64_t *xtab, int bits, bool biased, int tid, int nthreads) {
+    uint32_t wtx, wty;
+    plane_weight_regs(bits, true, &wtx, &wty);
+    for (int e = tid; e < 512; e += nthreads) {
+        const int h = e >> 8, wa = (int)((wtx >> (16 * h)) & 0xff), wb = (int)((wtx >> (16 * h + 8)) & 0xff);
+        const int bias = biased ? (h ? 13 : 3) : 0;
+        const int ja = e & 7, jb = (e >> 4) & 7, va = (e & 8) ? -wa : wa, vb = (e & 0x80) ? -wb : wb;
+        uint64_t x = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) x |= (uint64_t)(uint8_t)(bias + (i == ja ? va : 0) + (i == jb ? vb : 0)) << (8 * i);
+        xtab[e] = x;
+    }
+}
+
+// grid = (row tiles of 128 rows, ceil(N / 128)), block = 384 threads, 1 CTA per SM.
 //   warps 0..7  : consumers, warpgroup wg = rows 64*wg .. 64*wg+63 of the tile (wgmma accumulator layout)
 //   warps 8..11 : producers, thread = weight row; thread 0 also issues the record copy of each step
-__global__ void __launch_bounds__(kPfThreads2, 1) prefill_w2_kernel(const PrefillParams p) {
+// PB 2 (W2): a row tile is one 128-row super-block.  PB 4 (W3/W4): two 64-row super-blocks 2*tile + wg, one per consumer
+// warpgroup; when nrsb is odd the last tile's second super-block does not exist and its A rows are zero.
+template <int PB>
+__global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
+    static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
+    constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [S][16 KB]
     unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][kPfRec] B tile + lut scales + lut bias pairs
-    unsigned char *raw = sR + kPfStages * kPfRec;                          // [2][blk_bytes] packed block (codes + scales)
+    unsigned char *raw = sR + kPfStages * kPfRec;                          // [2][NSB][blk_bytes] packed blocks (codes + scales)
     const int rawsz = (p.blk_bytes + 127) & ~127;
-    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * rawsz);        // [256] expansion table
-    uint64_t *bars = xtab + 256;
+    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // [256] (PB 2) / [512] (PB 4) expansion table
+    uint64_t *bars = xtab + (PB == 4 ? 512 : 256);
     uint64_t *full = bars, *empty = bars + kPfStages;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int rsb = blockIdx.x, tile = blockIdx.y, n0 = tile * kPfNT;
+    const int rt = blockIdx.x, tile = blockIdx.y, n0 = tile * kPfNT;
     const int ntok = min(kPfNT, p.N - n0);
     const int nag = p.K / 64;
 
-    for (int e = tid; e < 256; e += kPfThreads2) {
-        // index byte: low nibble = plane 0 (neg<<3 | j), high nibble = plane 1; value = +-1 at byte j0, +-2 at byte j1
-        int v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        v[e & 7] += (e & 8) ? -1 : 1;
-        v[(e >> 4) & 7] += (e & 0x80) ? -2 : 2;
-        uint64_t x = 0;
-        for (int i = 0; i < 8; ++i) x |= (uint64_t)(uint8_t)(int8_t)v[i] << (8 * i);
-        xtab[e] = x;
+    if constexpr (PB == 2) {
+        for (int e = tid; e < 256; e += kPfThreads2) {
+            // index byte: low nibble = plane 0 (neg<<3 | j), high nibble = plane 1; value = +-1 at byte j0, +-2 at byte j1
+            int v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            v[e & 7] += (e & 8) ? -1 : 1;
+            v[(e >> 4) & 7] += (e & 0x80) ? -2 : 2;
+            uint64_t x = 0;
+            for (int i = 0; i < 8; ++i) x |= (uint64_t)(uint8_t)(int8_t)v[i] << (8 * i);
+            xtab[e] = x;
+        }
+    } else {
+        pf_build_xtab4(xtab, p.bits, false, tid, kPfThreads2);
     }
     if (tid == 0) {
         for (int i = 0; i < kPfStages; ++i) { pf_mbar_init(full + i, kPfProdWarps + 1); pf_mbar_init(empty + i, kPfConsWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const unsigned char *rsb_base = p.W + (size_t)rsb * p.rsb_stride;
+    const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
     const int nsteps = 2 * p.nchunk;                 // activation groups (two per chunk)
 
     if (warp >= kPfConsWarps) {
         // ======================= producers: thread = weight row of the tile =======================
         const int r = tid - kPfConsWarps * 32;
-        const int wl = r >> 2, wi = r & 3;           // lane / row-in-lane of the stream layout (RW = 4)
+        // PB 2: lane / row-in-lane of the stream layout (RW = 4).  PB 4: super-block sb of the tile, lane, row-in-lane (RW = 2);
+        // the 64 threads of a super-block load its blocks.
+        const int sb = PB == 4 ? r >> 6 : 0;
+        const int wl = PB == 4 ? (r & 63) >> 1 : r >> 2, wi = PB == 4 ? r & 1 : r & 3;
+        const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
+        const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
         const int n16 = p.blk_bytes >> 4;
         const unsigned char *rec_src = p.lut_tiles + (size_t)tile * nag * kPfRec;
-        for (int i = r; i < n16; i += 128) cp_async16_plain(raw + i * 16, rsb_base + i * 16);
+        auto load_blocks = [&](int c, unsigned char *dst) {   // chunk c of the tile's super-block(s) -> dst [NSB][rawsz]
+            if constexpr (PB == 2) {
+                for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c * p.blk_bytes + i * 16);
+            } else if (live) {
+                for (int i = r & 63; i < n16; i += 64) cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c * p.blk_bytes + i * 16);
+            }
+        };
+        load_blocks(0, raw);
         cp_async_commit();
         for (int c = 0; c < p.nchunk; ++c) {
-            unsigned char *rb = raw + (size_t)(c & 1) * rawsz;
+            unsigned char *rb = raw + (size_t)(c & 1) * NSB * rawsz;
             cp_async_wait_all();
             asm volatile("bar.sync 1, 128;" ::: "memory");                 // block c visible to all producers; block c-1 dead
             if (c + 1 < p.nchunk) {
-                unsigned char *nb = raw + (size_t)((c + 1) & 1) * rawsz;
-                const unsigned char *src = rsb_base + (size_t)(c + 1) * p.blk_bytes;
-                for (int i = r; i < n16; i += 128) cp_async16_plain(nb + i * 16, src + i * 16);
+                load_blocks(c + 1, raw + (size_t)((c + 1) & 1) * NSB * rawsz);
                 cp_async_commit();
             }
-            const uint32_t *words = reinterpret_cast<const uint32_t *>(rb);
+            const uint32_t *words = reinterpret_cast<const uint32_t *>(rb + (size_t)sb * rawsz);
 #pragma unroll 1
             for (int h = 0; h < 2; ++h) {
                 const int step = 2 * c + h, s = step % kPfStages;
@@ -204,9 +248,18 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_w2_kernel(const Prefil
                         const int gq = h * 16 + kc * 2 + u;                // group within the chunk (0..31)
                         const int q = gq >> 2, k = gq & 3;
                         const uint32_t *w4 = words + ((size_t)q * 32 + wl) * 4;
-                        const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;
-                        const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;
-                        v2[u] = xtab[jb | (ng << 3)];
+                        if constexpr (PB == 2) {
+                            const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;
+                            const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;
+                            v2[u] = xtab[jb | (ng << 3)];
+                        } else {
+                            // nibble 4*wi + b of word k = full code of plane b: planes (0, 1) and (2, 3) index the two table halves,
+                            // added byte-wise (|S| <= 15: no byte overflows, no borrow crosses into the next entry)
+                            const uint32_t cw = w4[k] >> (16 * wi);
+                            const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + ((cw >> 8) & 0xffu)];
+                            const uint32_t s0 = __vadd4((uint32_t)lo, (uint32_t)hi), s1 = __vadd4((uint32_t)(lo >> 32), (uint32_t)(hi >> 32));
+                            v2[u] = live ? ((uint64_t)s1 << 32 | s0) : 0ull;
+                        }
                     }
                     *reinterpret_cast<uint4 *>(a_dst + ((size_t)(kc * 16 + (r >> 3)) * 128 + (r & 7) * 16)) =
                         make_uint4((uint32_t)v2[0], (uint32_t)(v2[0] >> 32), (uint32_t)v2[1], (uint32_t)(v2[1] >> 32));
@@ -227,9 +280,16 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_w2_kernel(const Prefil
         uint32_t acc[64];
 #pragma unroll
         for (int j = 0; j < 64; ++j) accf[j] = 0.f;
-        // weight scale / zero point of (row, chunk), prefetched one chunk ahead (L2 hits, latency off the critical path)
-        auto ld_s = [&](int c, int r) { return 0.5f * load_scale(rsb_base + (size_t)c * p.blk_bytes + 4096, p.sd, r); };
-        auto ld_z = [&](int c, int r) { return p.zp ? load_scale(rsb_base + (size_t)c * p.blk_bytes + 4096 + (size_t)128 * p.sd, p.sd, r) : 0.f; };
+        // weight scale / zero point of (row, chunk), prefetched one chunk ahead (L2 hits, latency off the critical path).
+        // PB 4: the warpgroup's super-block, row r & 63 in it; zero for the missing second super-block of the last tile.
+        const unsigned char *wg_base = rsb_base + (size_t)(PB == 4 ? wg : 0) * p.rsb_stride;
+        const bool live = PB == 2 || rt * NSB + wg < p.nrsb;
+        auto ld_s = [&](int c, int r) {
+            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + 4096, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+        };
+        auto ld_z = [&](int c, int r) {
+            return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + 4096 + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+        };
         float hs[2], zz[2], hs_n[2], zz_n[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h] = ld_s(0, r0 + 8 * h); zz[h] = zz_n[h] = ld_z(0, r0 + 8 * h); }
@@ -285,7 +345,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_w2_kernel(const Prefil
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const int row = rsb * 128 + r0 + 8 * h;
+            const int row = rt * 128 + r0 + 8 * h;
             if (row >= p.Mout) continue;
 #pragma unroll
             for (int c8 = 0; c8 < 16; ++c8)

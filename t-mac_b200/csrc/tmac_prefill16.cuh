@@ -9,14 +9,15 @@
 // codes, B = fp16(ls*T8) is laid out once per call by lut_tile16_kernel, the accumulator stays in registers for the whole K and
 // is read once.  The bias term is one more contraction step with exact operands: A columns (0.5s, 0.5s, z, z) against B columns
 // (LBhi, LBlo, LBhi, LBlo), LB split into two fp16 so that their sum carries 22 bits.  Operand rounding (2^-11 per B entry)
-// keeps the result inside north_star's 1e-3 of the CPU kernel (tools/sim_fp16_prefill.py: 1.4e-4 W2, 2.4e-4 W4) -- NOT inside
+// keeps the result inside north_star's 1e-3 of the CPU kernel (tools/sim_fp16_prefill.py: 1.4e-4 W2, 2.2-2.7e-4 W3/W4) -- NOT inside
 // the 2e-5 the exact paths hold, so this tile has its own tolerance and never serves the int32 (BitNet) path.
 //
 // Tile: 128 weight rows x 256 tokens per CTA, wgmma.mma_async m64n256k16.f32.f16.f16, 8 MMAs per warpgroup per activation group.
 //   warpgroups 0, 1 : consumers (rows 64*wg .. 64*wg+63, 128 fp32 accumulators per thread), then the epilogue.
-//   warpgroup  2    : producers (thread = weight row, the step's 16 K-groups): code byte -> 8 fp16 entries, one 16-byte store per
-//                     group into the K-major canonical A tile; thread 0 also issues the step's 64 KB B tile as one bulk copy (TMA).
-// Supported: W2 (PB 2), chunk 128, act group 64, per-row scales (+ zero points), symmetric LUT -- as the int8 tile.
+//   warpgroup  2    : producers (thread = weight row, the step's 16 K-groups): plane codes -> 8 fp16 entries fp16(k * hs), one 16-byte
+//                     store per group into the K-major canonical A tile; thread 0 also issues the step's 64 KB B tile as one bulk copy (TMA).
+// Supported: W2 (PB 2) and W3/W4 (PB 4: a 128-row tile is two 64-row super-blocks), chunk 128, act group 64, per-row scales
+// (+ zero points), symmetric LUT -- as the int8 tile.
 #pragma once
 #include "tmac_prefill.cuh"
 
@@ -38,7 +39,8 @@ struct Prefill16Params {
     int nmain, nextra;                               // activation-group steps, bias steps (128 columns = 32 weight groups each)
     size_t rsb_stride;
     const unsigned char *tiles;                      // lut_tile16_kernel output: [token tile][nmain + nextra][kP16BBytes]
-    int nrsb, ntiles, streamk;                       // row super-blocks, tiles = nrsb * token tiles, stream-K split (see the kernel)
+    int nrsb, ntiles, streamk;                       // row super-blocks, tiles = nrt * token tiles, stream-K split (see the kernel)
+    int nrt, bits;                                   // row tiles of 128 rows (PB 2: nrsb, PB 4: ceil(nrsb / 2)), bit width
     float *scratch;                                  // [2][grid][256 tokens][128 rows] fp32 partial tiles (stream-K): published parts, finishers' own parts
     int *flags;                                      // [grid] partial tile ready
 };
@@ -114,13 +116,22 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
 //
 // Pipeline.  One 2-deep ring; a stage holds the A tile (producers) and the B tile (TMA) of one step, released by the consumers once
 // the step's MMAs have completed.
-__global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Prefill16Params p) {
+//
+// Row tile = 128 rows.  PB 2 (W2): one super-block.  PB 4 (W3/W4): super-blocks 2*rt and 2*rt + 1 (64 rows each), producer
+// threads 0..63 / 64..127 and consumer warpgroups 0 / 1; when nrsb is odd the last tile's second super-block does not exist and
+// its A rows are zero.
+template <int PB>
+__global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill16Params p) {
+    static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
+    constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [NA][32 KB]
     unsigned char *sB = sA + kP16NA * kP16SubA;                            // [NB][64 KB]
-    unsigned char *raw = sB + kP16NB * kP16SubB;                           // [2][blk] packed block (codes + scales)
+    unsigned char *raw = sB + kP16NB * kP16SubB;                           // [2][NSB][blk] packed blocks (codes + scales)
     const int rawsz = (p.blk_bytes + 127) & ~127;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(raw + 2 * rawsz);
+    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // PB 4: [512] expansion table (pf_build_xtab4, biased)
+    uint64_t *bars = xtab + (PB == 4 ? 512 : 0);
     uint64_t *full = bars, *empty = full + kP16NA;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -141,6 +152,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
         x = fs1[0]; fs1[0] = fs1[1]; fs1[1] = x;
     }
 
+    if constexpr (PB == 4) pf_build_xtab4(xtab, p.bits, true, tid, kP16Threads);
     if (tid == 0) {
         for (int i = 0; i < kP16NA; ++i) { pf_mbar_init(full + i, kP16ProdWarps + 1); pf_mbar_init(empty + i, kP16ConsWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -151,7 +163,11 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
         // ======================= producers: thread = weight row, all 16 K-groups of the step =======================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");           // registers go to the consumers' accumulators
         const int r = tid - kP16ConsWarps * 32;
-        const int wl = r >> 2, wi = r & 3;           // lane / row-in-lane of the stream layout (RW = 4)
+        // PB 2: lane / row-in-lane of the stream layout (RW = 4).  PB 4: super-block sb of the tile, lane, row-in-lane (RW = 2);
+        // the 64 threads of a super-block load its blocks.
+        const int sb = PB == 4 ? r >> 6 : 0;
+        const int wl = PB == 4 ? (r & 63) >> 1 : r >> 2, wi = PB == 4 ? r & 1 : r & 3;
+        const int srow = wl * (8 / PB) + wi;         // row within the super-block = scale index
         const int n16 = p.blk_bytes >> 4;
         int it = 0;                                  // running step counter over both fragments
         auto stage_in = [&](int f, int u) {          // wait for a free stage, request its B tile; returns the A tile
@@ -159,7 +175,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
             pf_mbar_wait(empty + s, ((it / kP16NA) & 1) ^ 1);   // the MMAs that read this stage have completed
             if (r == 0) {
                 pf_expect_tx(full + s, kP16SubB);
-                pf_bulk_g2s(sB + (size_t)s * kP16SubB, p.tiles + ((size_t)(ft[f] / p.nrsb) * nsteps + u) * kP16BBytes, kP16SubB, full + s);
+                pf_bulk_g2s(sB + (size_t)s * kP16SubB, p.tiles + ((size_t)(ft[f] / p.nrt) * nsteps + u) * kP16BBytes, kP16SubB, full + s);
             }
             return sA + (size_t)s * kP16SubA;
         };
@@ -173,28 +189,35 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
 #pragma unroll
         for (int f = 0; f < 2; ++f) {
             if (f == nfrag) break;
-            const int rsb = ft[f] % p.nrsb;
-            const unsigned char *rsb_base = p.W + (size_t)rsb * p.rsb_stride;
+            const int rt = ft[f] % p.nrt;
+            const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
+            const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
+            const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
+            auto load_blocks = [&](int c, unsigned char *dst) {   // chunk c of the tile's super-block(s) -> dst [NSB][rawsz]
+                if constexpr (PB == 2) {
+                    for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c * p.blk_bytes + i * 16);
+                } else if (live) {
+                    for (int i = r & 63; i < n16; i += 64) cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c * p.blk_bytes + i * 16);
+                }
+            };
             const int s0 = fs0[f], s1m = min(fs1[f], p.nmain);
             if (s0 < s1m) {
                 const int c_first = s0 >> 1, c_last = (s1m - 1) >> 1;
                 asm volatile("bar.sync 1, 128;" ::: "memory");             // the previous fragment's last block is dead
-                for (int i = r; i < n16; i += 128) cp_async16_plain(raw + (size_t)(c_first & 1) * rawsz + i * 16, rsb_base + (size_t)c_first * p.blk_bytes + i * 16);
+                load_blocks(c_first, raw + (size_t)(c_first & 1) * NSB * rawsz);
                 cp_async_commit();
                 for (int c = c_first; c <= c_last; ++c) {
-                    unsigned char *rb = raw + (size_t)(c & 1) * rawsz;
+                    unsigned char *rb = raw + (size_t)(c & 1) * NSB * rawsz;
                     cp_async_wait_all();
                     asm volatile("bar.sync 1, 128;" ::: "memory");         // block c visible to all producers; block c-1 dead
                     if (c + 1 <= c_last) {
-                        unsigned char *nb = raw + (size_t)((c + 1) & 1) * rawsz;
-                        const unsigned char *src = rsb_base + (size_t)(c + 1) * p.blk_bytes;
-                        for (int i = r; i < n16; i += 128) cp_async16_plain(nb + i * 16, src + i * 16);
+                        load_blocks(c + 1, raw + (size_t)((c + 1) & 1) * NSB * rawsz);
                         cp_async_commit();
                     }
-                    const uint32_t *words = reinterpret_cast<const uint32_t *>(rb);
-                    // the row's 8 A entries of one K-group: +-hs at entry j0 (plane 0) plus +-2hs at entry j1 (plane 1), hs = fp16(0.5 * scale),
-                    // built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the exact k * hs
-                    const __half hsh = __float2half_rn(0.5f * load_scale(rb + 4096, p.sd, wl * 4 + wi));
+                    const uint32_t *words = reinterpret_cast<const uint32_t *>(rb + (size_t)sb * rawsz);
+                    // hs = fp16(0.5 * scale).  PB 2: the row's 8 A entries of one K-group are +-hs at entry j0 (plane 0) plus +-2hs at
+                    // entry j1 (plane 1), built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the exact k * hs.
+                    const __half hsh = __float2half_rn(live ? 0.5f * load_scale(rb + (size_t)sb * rawsz + 4096, p.sd, srow) : 0.f);
                     const uint32_t c1 = __half_as_ushort(hsh), c2 = __half_as_ushort(__hadd(hsh, hsh));
                     const int u0 = (c == c_first) ? (s0 & 1) : 0, u1 = (c == c_last) ? ((s1m - 1) & 1) : 1;   // steps of this chunk
 #pragma unroll 1
@@ -205,16 +228,33 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
                             const int gqc = u * 16 + gl;                       // group within the chunk (0..31)
                             const int q = gqc >> 2, k = gqc & 3;
                             const uint32_t *w4 = words + ((size_t)q * 32 + wl) * 4;
-                            const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;                                   // j0 | j1 << 4
-                            const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;   // neg0 | neg1 << 4
-                            const uint32_t j0 = jb & 7u, j1 = jb >> 4;
-                            const uint32_t v0 = (c1 ^ ((ng & 1u) << 15)) << ((j0 & 1u) * 16), v1 = (c2 ^ ((ng & 0x10u) << 11)) << ((j1 & 1u) * 16);
                             uint32_t o4[4];
+                            if constexpr (PB == 2) {
+                                const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;                                   // j0 | j1 << 4
+                                const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;   // neg0 | neg1 << 4
+                                const uint32_t j0 = jb & 7u, j1 = jb >> 4;
+                                const uint32_t v0 = (c1 ^ ((ng & 1u) << 15)) << ((j0 & 1u) * 16), v1 = (c2 ^ ((ng & 0x10u) << 11)) << ((j1 & 1u) * 16);
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const uint32_t a = (j0 >> 1) == (uint32_t)e ? v0 : 0u, b = (j1 >> 1) == (uint32_t)e ? v1 : 0u;
-                                const __half2 x = __hadd2(*reinterpret_cast<const __half2 *>(&a), *reinterpret_cast<const __half2 *>(&b));
-                                o4[e] = *reinterpret_cast<const uint32_t *>(&x);
+                                for (int e = 0; e < 4; ++e) {
+                                    const uint32_t a = (j0 >> 1) == (uint32_t)e ? v0 : 0u, b = (j1 >> 1) == (uint32_t)e ? v1 : 0u;
+                                    const __half2 x = __hadd2(*reinterpret_cast<const __half2 *>(&a), *reinterpret_cast<const __half2 *>(&b));
+                                    o4[e] = *reinterpret_cast<const uint32_t *>(&x);
+                                }
+                            } else {
+                                // PB 4: the integer k = S[e] (|S| <= 15) of the row's four planes from the two biased table halves: the plain
+                                // 32-bit add holds k + 16 in [1, 31] per byte.  fp16 bits 0x6400 | m are 1024 + m, minus 1040 is
+                                // k exactly; k and hs are exact fp16 values, so the HMUL2 rounds the exact product k * hs once.
+                                const uint32_t cw = w4[k] >> (16 * wi);
+                                const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + ((cw >> 8) & 0xffu)];
+                                const uint32_t sk[2] = {(uint32_t)lo + (uint32_t)hi, (uint32_t)(lo >> 32) + (uint32_t)(hi >> 32)};
+                                const __half2 hs2 = __halves2half2(hsh, hsh), off = __float2half2_rn(1040.f);
+#pragma unroll
+                                for (int e = 0; e < 4; ++e) {
+                                    const uint32_t m = __byte_perm(sk[e >> 1], 0x64u, (e & 1) ? 0x4342u : 0x4140u);   // entries 2e, 2e + 1
+                                    const __half2 kk = __hsub2(*reinterpret_cast<const __half2 *>(&m), off);
+                                    const __half2 x = __hmul2(kk, hs2);
+                                    o4[e] = *reinterpret_cast<const uint32_t *>(&x);
+                                }
                             }
                             *reinterpret_cast<uint4 *>(a_dst + ((size_t)(gl * 16 + (r >> 3)) * 128 + (r & 7) * 16)) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
                         }
@@ -233,10 +273,10 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
                     for (int u = 0; u < 2; ++u) {
                         const int wg = e * 32 + kc * 2 + u;
                         float hs = 0.f, zz = 0.f;
-                        if (wg < p.nchunk) {
-                            const unsigned char *sp = rsb_base + (size_t)wg * p.blk_bytes + 4096;
-                            hs = 0.5f * load_scale(sp, p.sd, wl * 4 + wi);
-                            if (p.zp) zz = load_scale(sp + (size_t)128 * p.sd, p.sd, wl * 4 + wi);
+                        if (live && wg < p.nchunk) {
+                            const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + 4096;
+                            hs = 0.5f * load_scale(sp, p.sd, srow);
+                            if (p.zp) zz = load_scale(sp + (size_t)RSB * p.sd, p.sd, srow);
                         }
                         const __half2 a = __floats2half2_rn(hs, hs), b = __floats2half2_rn(zz, zz);
                         o[2 * u] = *reinterpret_cast<const uint32_t *>(&a); o[2 * u + 1] = *reinterpret_cast<const uint32_t *>(&b);
@@ -273,11 +313,11 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
                 __syncwarp();
             }
             const bool whole = fs0[f] == 0 && fs1[f] == nsteps, last = fs1[f] == nsteps;
-            const int rsb = ft[f] % p.nrsb, tile = ft[f] / p.nrsb, n0 = tile * kP16NT, ntok = min(kP16NT, p.N - n0);
+            const int rt = ft[f] % p.nrt, tile = ft[f] / p.nrt, n0 = tile * kP16NT, ntok = min(kP16NT, p.N - n0);
             if (whole) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    const int row = rsb * 128 + r0 + 8 * h;
+                    const int row = rt * 128 + r0 + 8 * h;
 #pragma unroll
                     for (int c8 = 0; c8 < 32; ++c8)
 #pragma unroll
@@ -320,7 +360,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_w2_kernel(const Pref
                 }
             asm volatile("bar.sync 2, 256;" ::: "memory");
             for (int i = tid; i < ntok * 128; i += kP16ConsWarps * 32) {
-                const int t = i >> 7, er = i & 127, row = rsb * 128 + er;
+                const int t = i >> 7, er = i & 127, row = rt * 128 + er;
                 float sum = 0.f;
                 for (int c2 = c_first; c2 < cta; ++c2) sum += __ldcg(p.scratch + ((size_t)c2 * kP16NT + t) * 128 + er);
                 sum += __ldcg(mine + (size_t)t * 128 + er);

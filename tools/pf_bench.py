@@ -1,22 +1,85 @@
-import os, sys, time
+"""Prefill tile timing: for each shape and N, CUDA events over repeated calls after a warm-up, of
+    pre+tile   tb.gemv (LUT build + the tile, the one-call form)
+    tile only  tb.qgemm_lut on a prepared LUT
+    gemv       the same qgemm_lut call with the tiles disabled (debug knob prefill = 0): the GEMV kernel per activation row
+The tile's minimum N is set to the smallest N of the run, so that the tile is timed below the library's threshold too.
+
+    python tools/pf_bench.py                          # W2 g128 zp 11008 x 4096, N = 32 .. 512 (as before)
+    python tools/pf_bench.py --bits 4                 # W4 g128 zp: 4096x4096, 11008x4096, 4096x11008, 18944x3584, N = 16 .. 512
+    python tools/pf_bench.py --bits 3 --shapes 11008x4096
+
+Rates: dense-equivalent = 2*N*M*K / time; MMA = the tile's tensor-core work (padded to whole 128-row x token tiles, contraction
+2K entries + the fp16 tile's bias columns) / time, against the H100 SXM data-sheet peaks (dense): 989 TFLOP/s fp16, 1979 TOP/s int8.
+"""
+import argparse
+import os
+import subprocess
+import sys
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "t-mac_b200")); sys.path.insert(0, ROOT)
-import torch, numpy as np
-import tmac_b200 as tb, bench
+sys.path.insert(0, os.path.join(ROOT, "t-mac_b200")); sys.path.insert(0, os.path.join(ROOT, "oracle")); sys.path.insert(0, ROOT)
+import torch  # noqa: E402
+import tmac_b200 as tb, bench  # noqa: E402
+import tmac_oracle as T  # noqa: E402
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--bits", type=int, default=2)
+ap.add_argument("--shapes", default=None, help="comma-separated MxK (rows x K); default: 11008x4096 for W2, the Llama-2 / Qwen2 W4 shapes otherwise")
+ap.add_argument("--ns", default=None, help="comma-separated N; default: 32..512 for W2, 16..512 otherwise")
+ap.add_argument("--reps", type=int, default=20)
+ap.add_argument("--sym", action="store_true", help="no zero points")
+a = ap.parse_args()
+shapes = a.shapes or ("%dx%d" % (bench.MOUT, bench.K) if a.bits == 2 else "4096x4096,11008x4096,4096x11008,18944x3584")
+shapes = [tuple(int(v) for v in s.split("x")) for s in shapes.split(",")]
+ns = [int(v) for v in a.ns.split(",")] if a.ns else ([32, 64, 128, 256, 512] if a.bits == 2 else [16, 32, 64, 128, 256, 512])
+
+print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv"], capture_output=True, text=True).stdout.strip())
 lib = tb.load(); tb.check(lib.tmac_b200_init(0), "init")
 st = torch.cuda.Stream(); torch.cuda.set_stream(st); tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "ss")
-w, sc, z = bench.synth(9)
-cfg = tb.make_kcfg(bench.MOUT, bench.K, 2, 128, 16, 128, 64, True, False)
-wt = tb.upload_plain(cfg, w, sc, z)
-for N in (32, 64, 128, 256, 512):
-    x = torch.randn((N, bench.K), device="cuda"); o = torch.zeros((N, bench.MOUT), device="cuda")
-    q = torch.zeros((N, bench.K // 4, 16), dtype=torch.int8, device="cuda"); ls = torch.zeros((N, 64), device="cuda"); lb = torch.zeros_like(ls)
-    tb.preprocessor(bench.K, N, 64, x, ls, lb, q)
-    for name, fn in (("pre+tile", lambda: tb.gemv(wt, N, x, o)), ("tile only", lambda: tb.qgemm_lut(wt, N, q, ls, lb, o))):
-        fn(); torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(st)
-        for _ in range(5): fn()
-        e1.record(st); torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / 5
-        print("N=%4d %-10s %8.1f us   dense-equivalent %7.1f TFLOP/s   int8 MMA rate %6.1f TOP/s  launch=%s" % (N, name, ms * 1e3, 2.0 * N * bench.MOUT * bench.K / ms / 1e9, 2.0 * ((N + 127) // 128 * 128) * 11008 * (2 * bench.K) / ms / 1e9, tb.last_launch()["batch"]))
+tb.debug_set("prefill_min_n", min(ns))
+
+
+def time_us(fn):
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(st)
+    for _ in range(a.reps):
+        fn()
+    e1.record(st); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / a.reps * 1e3
+
+
+try:
+    for M, K in shapes:
+        w, sc, z = bench.synth(9, mout=M, k=K, bits=a.bits, zp=not a.sym)
+        cfg = tb.make_kcfg(M, K, a.bits, T.default_bm(M * a.bits, a.bits), 16, 128, 64, not a.sym, False)
+        wt = tb.upload_plain(cfg, w, sc, z)
+        nag = K // 64
+        print("W%d %s %d x %d" % (a.bits, "sym" if a.sym else "zp", M, K))
+        for N in ns:
+            x = torch.randn((N, K), device="cuda"); o = torch.zeros((N, M), device="cuda")
+            q = torch.zeros((N, K // 4, 16), dtype=torch.int8, device="cuda"); ls = torch.zeros((N, nag), device="cuda"); lb = torch.zeros_like(ls)
+            tb.preprocessor(K, N, 64, x, ls, lb, q)
+            row = {}
+            for name, fn in (("pre+tile", lambda: tb.gemv(wt, N, x, o)), ("tile only", lambda: tb.qgemm_lut(wt, N, q, ls, lb, o)),
+                             ("gemv", lambda: tb.qgemm_lut(wt, N, q, ls, lb, o))):
+                tb.debug_set("prefill", 0 if name == "gemv" else 1)
+                us = time_us(fn)
+                ll = tb.last_launch()
+                row[name] = us
+                dense = 2.0 * N * M * K / us / 1e6
+                if ll["batch"] >= 0:
+                    kind, mma = "GEMV", ""
+                elif ll["cluster"] == 16:    # fp16 tile: 256-token tiles, K/64 + ceil(K/128/32) steps of 128 entries
+                    work = 2.0 * ((N + 255) // 256 * 256) * ((M + 127) // 128 * 128) * 128 * (K // 64 + (K // 128 + 31) // 32)
+                    kind, mma = "fp16 tile", "  MMA %6.1f TFLOP/s (%4.1f%% of 989)" % (work / us / 1e6, 100.0 * work / us / 1e6 / 989)
+                else:                        # int8 tile: 128-token tiles, contraction 2K bytes
+                    work = 2.0 * ((N + 127) // 128 * 128) * ((M + 127) // 128 * 128) * (2 * K)
+                    kind, mma = "int8 tile", "  MMA %6.1f TOP/s (%4.1f%% of 1979)" % (work / us / 1e6, 100.0 * work / us / 1e6 / 1979)
+                print("  N=%4d %-10s %9.1f us   dense-equivalent %6.1f TFLOP/s  [%s]%s" % (N, name, us, dense, kind, mma))
+            print("  N=%4d tile/gemv = %.2f  (tile %s)" % (N, row["tile only"] / row["gemv"], "faster" if row["tile only"] < row["gemv"] else "SLOWER"))
+        wt.free()
+finally:
+    tb.debug_set("prefill", 1); tb.debug_set("prefill_min_n", 0)

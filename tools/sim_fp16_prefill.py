@@ -1,8 +1,9 @@
-"""CPU study for the next prefill tile (DESIGN.md section 8, item 2): how far from the reference kernel is the formulation that
-folds both scales into fp16 operands -- A = 0.5*scale[m][wg]*S[m][g][e], B = lut_scale[n][ag]*T8[n][g][e] -- and accumulates the
-whole K in fp32, with the LUT-bias / zero-point terms kept exact?  Uses the oracle (TEST INFRASTRUCTURE) as the truth.
+"""CPU study of the fp16 prefill tile (tmac_prefill16.cuh): how far from the reference kernel is the formulation that folds both
+scales into fp16 operands -- A = 0.5*scale[m][wg]*S[m][g][e], B = lut_scale[n][ag]*T8[n][g][e] -- and accumulates the whole K in
+fp32, with the LUT-bias / zero-point terms kept exact?  W2 and the 4-plane layouts (W3, W4) that the tile serves, at 512 x 4096
+and at the Llama-2 / Qwen2 K of 11008 and 18944.  Uses the oracle (TEST INFRASTRUCTURE) as the truth.
 
-    python tools/sim_fp16_prefill.py         # W2 / W4, 512 x 4096, 8 tokens: max|dC|/max|C| 1.4e-4 / 2.4e-4 (bar: 1e-3)
+    python tools/sim_fp16_prefill.py         # 8 tokens, seed 3: max|dC|/max|C| 1.4e-4 (W2) .. 2.7e-4 (W4 512 x 4096 sym); bar 1e-3
 """
 import os
 import sys
@@ -14,8 +15,10 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import tmac_oracle as T   # noqa: E402
 
 o = T.load_oracle()
-for bits in (2, 4):
-    cfg = T.Config(512, 4096, bits, zero_point=True).resolved()
+CASES = [(512, 4096, 2, True), (512, 4096, 4, True), (512, 4096, 4, False), (384, 4096, 3, True), (256, 11008, 4, False),
+         (256, 18944, 4, True), (384, 11008, 3, True)]
+for Mout, Kc, bits, zp in CASES:
+    cfg = T.Config(Mout, Kc, bits, zero_point=zp).resolved()
     N = 8
     w, sc, z, x = T.make_problem(cfg, seed=3, N=N)
     A, S_ = T.pack_reference_layout(w, sc, z, cfg)
@@ -35,6 +38,7 @@ for bits in (2, 4):
     Aop = (0.5 * s_g[:, :, None] * S).astype(np.float16).astype(np.float32).reshape(M, -1)
     Bop = (ls_g[:, :, None] * T8).astype(np.float16).astype(np.float32).reshape(N, -1)
     LB = lb.reshape(N, K // gs, gs // ags).sum(-1)
-    rest = LB.astype(np.float64) @ (0.5 * sc + z).astype(np.float64).T
+    rest = LB.astype(np.float64) @ (0.5 * sc + (z if zp else 0.0)).astype(np.float64).T
     C = (Bop @ Aop.T).astype(np.float64) + rest
-    print("W%d fp16 operands, fp32 accumulate: max|dC|/max|C| = %.2e   nmse %.2e" % (bits, np.abs(C - Cref).max() / np.abs(Cref).max(), T.nmse(Cref, C.astype(np.float32))))
+    print("W%d %4d x %5d %-3s fp16 operands, fp32 accumulate: max|dC|/max|C| = %.2e   nmse %.2e"
+          % (bits, M, K, "zp" if zp else "sym", np.abs(C - Cref).max() / np.abs(Cref).max(), T.nmse(Cref, C.astype(np.float32))))
