@@ -21,10 +21,10 @@
 // bench.py times it on the bench chain (32 x 11008x4096 W2, x[i+1] = first K outputs of op i) beside the launch chain and
 // tmac_seq.cuh; flags bit 0 selects the grid-barrier form this kernel started as, kept for comparison.  Per-phase stamps
 // (ChainParams::trace) are read by tools/seq_bench.py --trace.
-// The LUT slices are built by lut_group, lut_addv8 and lut_bias (tmac_kernels.cuh), the functions the preprocessor and gemv3's
-// fused path build theirs with, so LUT bytes, scales and biases are identical to the preprocessor's; fp32 sums in fixed (warp,
-// then cluster rank) order; the K split differs from the lone launch's, so results equal tmac_b200_gemv's up to fp32
-// re-association.  Waits are bounded (error flag).
+// The LUT slices are built by lut_slice and the blocks run by TMAC_BLOCK_LOOKUPS / TMAC_BLOCK_SCALES (tmac_kernels.cuh), the
+// code gemv3's fused path runs, so LUT bytes, scales and biases are identical to the preprocessor's and a block's fp32
+// operation order is gemv3's; fp32 sums in fixed (warp, then cluster rank) order; the K split differs from the lone launch's,
+// so results equal tmac_b200_gemv's up to fp32 re-association.  Waits are bounded (error flag, mbar_wait_bounded).
 #pragma once
 #include "tmac_kernels.cuh"
 #include "tmac_seq.cuh"     // {value, epoch} words: seq_publish
@@ -66,12 +66,6 @@ struct ChainParams {
     long long *trace;                       // debug: [nops][grid][16] globaltimer stamps of thread 0, or NULL
 };
 
-// The split-phase barrier of the data-flow form guards only the RE-USE of shared-memory buffers (red, cl): the readers have
-// consumed their values before they arrive, the writers write after they have waited.  It carries no data, so it needs neither
-// release on the arrive side -- which ptxas turns into MEMBAR.ALL.GPU per thread and op.  (barrier.cluster.wait has only the
-// acquire form.)
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait_acq() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
 // partial sum -> the leader's shared memory, completion counted on the leader's mbarrier
 __device__ __forceinline__ void st_async_f32(float *local_ptr, uint64_t *local_bar, uint32_t rank, float v) {
     uint32_t ra, rb;
@@ -105,14 +99,6 @@ __device__ __forceinline__ void chain_wait_x(const uint2 *src, bool active, uint
     }
     b0 = __uint_as_float(v0.x); b1 = __uint_as_float(v0.z); b2 = __uint_as_float(v1.x); b3 = __uint_as_float(v1.z);
 }
-__device__ __forceinline__ long long chain_now() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-__device__ __forceinline__ bool chain_mbar_wait(uint64_t *b, uint32_t parity) {
-    uint32_t ok = 0;
-    for (int spins = 0; spins < kChainSpin && !ok; ++spins)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(smem_u32(b)), "r"(parity) : "memory");
-    return ok != 0;
-}
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) { unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 
 template <int PB, int QCH, int AGQ>
@@ -141,9 +127,10 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
     const unsigned bar_base = epoch0 * (unsigned)p.nops * (unsigned)nclusters;
 
     if (lane == 0) {
-        for (int s = 0; s < NS; ++s) mbar_init1(mbar + s);
-        if (warp == 0) mbar_init1(rmbar);
+        for (int s = 0; s < NS; ++s) mbar_init(mbar + s, 1);
+        if (warp == 0) mbar_init(rmbar, 1);
         mbar_fence_init();
+        fence_proxy_async();
     }
     __syncwarp();
     cluster_sync_all();                                            // every CTA of the cluster runs: its shared memory may be written
@@ -174,7 +161,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
     auto request_next = [&]() {
         if (!nw) return;
         if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bulk_load(stage0 + (size_t)rs * p.max_blk, nw + (size_t)rsb * nstride + (size_t)nc * nbytes, (uint32_t)nbytes, mbar + rs);
         }
         if (++rs == NS) rs = 0;
@@ -194,7 +181,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         const int c_first = c_slot * bpw, c_end = min(nchunk, c_first + bpw);
         const uint32_t ep_in = epoch0 * (uint32_t)p.nops + (uint32_t)o.in_op + 1u, ep_out = epoch0 * (uint32_t)p.nops + (uint32_t)op + 1u;
         long long *tr = (p.trace && tid == 0) ? p.trace + ((size_t)op * gridDim.x + blockIdx.x) * 16 : nullptr;
-        if (tr) tr[0] = chain_now();
+        if (tr) tr[0] = globaltimer_ns();
         if (op > 0 && !flow) {
             // ---- barrier form: every cluster has stored op-1's rows (release-increment by its leader); one polling thread per CTA ----
             if (tid == 0) {
@@ -203,10 +190,10 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                 while ((int)(ld_acquire_u32(p.bar) - target) < 0 && ++spins < kChainSpin) { }
                 if (spins >= kChainSpin) atomicExch(p.err, 1);
             }
-            if (tr) tr[1] = chain_now();
+            if (tr) tr[1] = globaltimer_ns();
             __syncthreads();
         }
-        if (tr) tr[2] = chain_now();
+        if (tr) tr[2] = globaltimer_ns();
         float cacc[RW];
         int iacc[RW];
 #pragma unroll
@@ -214,80 +201,47 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         if (active)
             for (int c = c_first; c < c_end; ++c) {
                 // ---- LUT slice of this chunk -> warp-private table (lane = group) ----
-                float lsv[NAG], lbsum = 0.f;
-                {
-                    float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
-                    if (flow && o.ll_in) {                         // the producer's rows, as soon as they exist
-                        chain_wait_x(o.ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, b0, b1, b2, b3);
-                        if (lane >= NG) b0 = b1 = b2 = b3 = 0.f;
-                    } else if (lane < NG) {
-                        const float4 f = __ldcg(reinterpret_cast<const float4 *>(x + ((size_t)c * NG + lane) * 4));   // L2: written by other SMs
-                        b0 = f.x; b1 = f.y; b2 = f.z; b3 = f.w;
-                    }
-                    uint32_t lo, hi;
-                    float scale;
-                    const float l0 = lut_group<WL>(b0, b1, b2, b3, lo, hi, scale);
-                    if (lane < NG) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
-                    const float blk = lut_addv8(l0);
-#pragma unroll
-                    for (int a = 0; a < NAG; ++a) {
-                        lsv[a] = __shfl_sync(0xffffffffu, scale, a * WL);
-                        lbsum += lut_bias<WL>(blk, a * WL);
-                    }
+                float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
+                if (flow && o.ll_in) {                             // the producer's rows, as soon as they exist
+                    chain_wait_x(o.ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, b0, b1, b2, b3);
+                    if (lane >= NG) b0 = b1 = b2 = b3 = 0.f;
+                } else if (lane < NG) {
+                    const float4 f = __ldcg(reinterpret_cast<const float4 *>(x + ((size_t)c * NG + lane) * 4));   // L2: written by other SMs
+                    b0 = f.x; b1 = f.y; b2 = f.z; b3 = f.w;
                 }
-                if (tr) tr[3] = chain_now();
-                if (!chain_mbar_wait(mbar + cs, cph)) atomicExch(p.err, 2);
+                float lsv[NAG];
+                const float lbsum = lut_slice<WL, NAG>(b0, b1, b2, b3, lane, tab, lsv);
+                if (tr) tr[3] = globaltimer_ns();
+                if (!mbar_wait_bounded<kChainSpin>(mbar + cs, cph)) atomicExch(p.err, 2);
                 __syncwarp();
-                if (tr) tr[4] = chain_now();
+                if (tr) tr[4] = globaltimer_ns();
                 // block j + NS - 1 is requested as block j's lookups start, into the stage of block j - 1 (its lookups ended with the
                 // __syncwarp at the end of the previous chunk; the proxy fence in request_next orders them before the bulk copy)
                 request_next();
                 const unsigned char *stage = stage0 + (size_t)cs * p.max_blk;
-                const uint4 *wp = reinterpret_cast<const uint4 *>(stage) + lane;
                 float facc[RW];
-#pragma unroll
-                for (int i = 0; i < RW; ++i) facc[i] = 0.f;
-#pragma unroll
-                for (int q = 0; q < QCH; ++q) {
-                    const uint4 wq = wp[q * 32];
-                    const uint4 a = reinterpret_cast<const uint4 *>(tab)[2 * q], b2 = reinterpret_cast<const uint4 *>(tab)[2 * q + 1];
-                    const uint32_t t[8] = {a.x, a.y, a.z, a.w, b2.x, b2.y, b2.z, b2.w};
-                    Quad<PB, true>::run(wq, t, iacc, wtx, wty);
-                    if (((q + 1) % AGQ) == 0) {
-#pragma unroll
-                        for (int i = 0; i < RW; ++i) { facc[i] = fmaf(lsv[q / AGQ], (float)iacc[i], facc[i]); iacc[i] = 0; }
-                    }
-                }
-                {
-                    const unsigned char *sp = stage + (size_t)QCH * 512;
-#pragma unroll
-                    for (int i = 0; i < RW; ++i) {
-                        const float s = one_scale ? scale0 : load_scale(sp, sd, lane * RW + i);
-                        float v = fmaf(0.5f * s, facc[i] + lbsum, cacc[i]);
-                        if (zp) v = fmaf(load_scale(sp + (size_t)RSB * sd, sd, lane * RW + i), lbsum, v);
-                        cacc[i] = v;
-                    }
-                }
+                TMAC_BLOCK_LOOKUPS(PB, true, QCH, AGQ, stage, tab, lane, wtx, wty, lsv, iacc, facc);
+                TMAC_BLOCK_SCALES(PB, QCH, stage, lane, one_scale, scale0, sd, zp, facc, lbsum, cacc);
                 __syncwarp();                                      // stage / table are rewritten by later chunks
                 if (++cs == NS) { cs = 0; cph ^= 1u; }
             }
-        if (tr) tr[5] = chain_now();
+        if (tr) tr[5] = globaltimer_ns();
 
         // ---- CTA reduction (fixed warp order), cluster reduction in the leader's shared memory (rank order), leader stores the rows ----
-        if (flow && op > 0) cluster_wait_acq();                    // every thread of the cluster is past op-1's reduction: red / cl may be rewritten
+        if (flow && op > 0) cluster_wait();                        // every thread of the cluster is past op-1's reduction: red / cl may be rewritten
         {
             float *r = red + (size_t)warp * RSB + lane * RW;
 #pragma unroll
             for (int i = 0; i < RW; ++i) r[i] = cacc[i];
         }
         __syncthreads();
-        if (tr) tr[6] = chain_now();
+        if (tr) tr[6] = globaltimer_ns();
         if (flow) {
             // peers send their partial with st.async (completion bytes counted on the leader's mbarrier); the leader sums in rank
             // order once (CS-1) x RSB floats have landed: one DSMEM hop instead of a cluster-wide rendezvous
             if (active) {
                 if (rank == 0 && tid == 0)
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(rmbar)), "r"((uint32_t)((CS - 1) * RSB * 4)) : "memory");
+                    expect_tx(rmbar, (uint32_t)((CS - 1) * RSB * 4));
                 for (int t = tid; t < RSB; t += WPC * 32) {
                     float fsum = 0.f;
 #pragma unroll
@@ -295,9 +249,9 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                     if (rank == 0) cl[t] = fsum;                   // read back by the same thread below
                     else st_async_f32(cl + (size_t)rank * RSB + t, rmbar, 0, fsum);
                 }
-                if (tr) tr[7] = chain_now();
+                if (tr) tr[7] = globaltimer_ns();
                 if (rank == 0) {
-                    if (!chain_mbar_wait(rmbar, nred & 1)) atomicExch(p.err, 6);
+                    if (!mbar_wait_bounded<kChainSpin>(rmbar, nred & 1)) atomicExch(p.err, 6);
                     ++nred;
                     for (int t = tid; t < RSB; t += WPC * 32) {
                         float fsum = 0.f;
@@ -306,18 +260,15 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                         const int row = rsb * RSB + t;
                         if (row < o.Mout) {
                             seq_publish(o.ll_out + row, __float_as_uint(fsum), ep_out);
-                            if (o.out_f16) reinterpret_cast<__half *>(o.C)[row] = __float2half_rn(fsum);
-                            else reinterpret_cast<float *>(o.C)[row] = fsum;
-                            for (int q = 0; q < o.npeer; ++q) {      // the all-gather, fused into the epilogue: one store per peer and row
-                                if (o.out_f16) reinterpret_cast<__half *>(o.Cpeer[q])[row] = __float2half_rn(fsum);
-                                else reinterpret_cast<float *>(o.Cpeer[q])[row] = fsum;
-                            }
+                            store_out(o.C, row, fsum, o.out_f16);
+                            for (int q = 0; q < o.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
+                                store_out(o.Cpeer[q], row, fsum, o.out_f16);
                         }
                     }
-                    if (tr) tr[8] = chain_now();
+                    if (tr) tr[8] = globaltimer_ns();
                 }
             }
-            cluster_arrive();                                      // split-phase: waited for before the next op's partials are written
+            cluster_arrive_relaxed();                              // split-phase: waited for before the next op's partials are written
         } else {
             for (int t = tid; t < RSB; t += WPC * 32) {
                 float fsum = 0.f;
@@ -326,7 +277,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                 st_cluster_f32(cl + (size_t)rank * RSB + t, 0, fsum);
             }
             cluster_sync_all();
-            if (tr) tr[7] = chain_now();
+            if (tr) tr[7] = globaltimer_ns();
             if (rank == 0) {
                 if (active)
                     for (int t = tid; t < RSB; t += WPC * 32) {
@@ -335,17 +286,13 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                         for (int k2 = 0; k2 < CS; ++k2) fsum += cl[(size_t)k2 * RSB + t];
                         const int row = rsb * RSB + t;
                         if (row < o.Mout) {
-                            if (o.out_f16) reinterpret_cast<__half *>(o.C)[row] = __float2half_rn(fsum);
-                            else reinterpret_cast<float *>(o.C)[row] = fsum;
-                            for (int q = 0; q < o.npeer; ++q) {
-                                if (o.out_f16) reinterpret_cast<__half *>(o.Cpeer[q])[row] = __float2half_rn(fsum);
-                                else reinterpret_cast<float *>(o.Cpeer[q])[row] = fsum;
-                            }
+                            store_out(o.C, row, fsum, o.out_f16);
+                            for (int q = 0; q < o.npeer; ++q) store_out(o.Cpeer[q], row, fsum, o.out_f16);
                         }
                     }
                 __syncthreads();                                   // the release below is cumulative over the CTA's stores
                 if (tid == 0) asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p.bar), "r"(1u) : "memory");
-                if (tr) tr[8] = chain_now();
+                if (tr) tr[8] = globaltimer_ns();
             }
         }
     }
@@ -360,7 +307,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         }
         p.epochs[blockIdx.x] = epoch0 + 1u;
     }
-    if (flow) cluster_wait_acq();                                  // completes the last split-phase barrier
+    if (flow) cluster_wait();                                      // completes the last split-phase barrier
     cluster_sync_all();                                            // nobody leaves while a peer may still write its shared memory
 }
 

@@ -15,6 +15,14 @@
 // 8-byte constant table indexed by the sign bits.  One DP4A therefore does "negate, scale by
 // the bit-plane weight, add the 4 lookups" = the int16 adder tree + alpha recombination of the
 // reference, exactly, in int32.
+//
+// Shared by every kernel of the project (all headers include this one):
+//   the activation LUT   : lut_abs_sum, lut_scale, lut_ts, lut_odd_entries, lut_q8, lut_stored, lut_addv8, lut_group, lut_bias,
+//                          lut_slice (one chunk's slice in a warp);
+//   the block step       : TMAC_BLOCK_LOOKUPS, TMAC_BLOCK_SCALES (gemv3_kernel and chain_kernel);
+//   PTX wrappers         : smem_u32, mbar_init, mbar_fence_init, fence_proxy_async, mbar_arrive, expect_tx, bulk_load,
+//                          mbar_wait_parity, mbar_wait_bounded<LIMIT>, cluster_arrive_relaxed / cluster_wait, globaltimer_ns;
+//   the output store     : store_out (fp16 or fp32).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -39,9 +47,6 @@ __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
 __device__ __forceinline__ uint32_t hi16(uint32_t x) { return x >> 16; }
 #else
 __device__ __forceinline__ uint32_t hi16(uint32_t x) { return __umulhi(x, 65536u); }
-#endif
-#ifndef TMAC_G3_MINB
-#define TMAC_G3_MINB 4
 #endif
 __device__ __forceinline__ uint4 ldg_stream(const uint4 *p) {
     uint4 r;
@@ -272,6 +277,74 @@ __device__ __forceinline__ float lut_bias(float blk, int first) {
     for (int k = 0; k < WL / 8; ++k) bias = __fadd_rn(bias, __shfl_sync(0xffffffffu, blk, first + 8 * k));
     return bias;
 }
+// LUT slice of one chunk of NAG activation groups, lane = K-group (x0..x3 = its four activations, zero in lanes >= NAG * WL):
+// the lane's stored entries to the warp's table (lanes < NAG * WL), the groups' LUT scales to lsv; returns the sum of their LUT
+// biases.  All 32 lanes must call it.
+template <int WL, int NAG>
+__device__ __forceinline__ float lut_slice(float x0, float x1, float x2, float x3, int lane, unsigned char *tab, float *lsv) {
+    uint32_t lo, hi;
+    float scale, lbsum = 0.f;
+    const float l0 = lut_group<WL>(x0, x1, x2, x3, lo, hi, scale);
+    if (lane < NAG * WL) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
+    const float blk = lut_addv8(l0);
+#pragma unroll
+    for (int a = 0; a < NAG; ++a) {
+        lsv[a] = __shfl_sync(0xffffffffu, scale, a * WL);
+        lbsum += lut_bias<WL>(blk, a * WL);
+    }
+    return lbsum;
+}
+
+// ------------------------------------------------------------------------------------------
+// The arithmetic of one (row super-block, K chunk) block, shared by gemv3_kernel and chain_kernel: the fp32 operation order
+// decides the result, so both run this one code.  The block is the stream layout (tmac_layout.h): QCH quads of 32 lanes x 16
+// code bytes, then RSB weight scales and (zp) RSB zero points of sd bytes each; tab is the warp's LUT slice of the chunk.
+// These two are macros, not functions: the compiler simplifies a callee before it inlines it, and as __forceinline__ functions
+// the step changed the kernels' SASS (gemv3_kernel<2,true,8,4,3,true> 1752 -> 1768 instructions, chain_kernel<2,8,4> another
+// shared-memory load mix).  Expanded in place they compile to the instructions of the code they replaced.
+// ------------------------------------------------------------------------------------------
+// TMAC_BLOCK_LOOKUPS: facc[i] = sum over the chunk's activation groups a of lsv[a] * (lane's row i lookups of a's AGQ quads),
+// Quad<PB, SYM> into iacc, which is left at zero.  AGQ == 0 (integer path, one activation group = the whole row): only iacc
+// accumulates.  Arguments are evaluated more than once.
+#define TMAC_BLOCK_LOOKUPS(PB, SYM, QCH, AGQ, stage, tab, lane, wtx, wty, lsv, iacc, facc)                                        \
+    do {                                                                                                                          \
+        constexpr int RW_ = 8 / (PB), AQ_ = (AGQ) ? (AGQ) : 1;                                                                    \
+        const uint4 *wp_ = reinterpret_cast<const uint4 *>(stage) + (lane);                                                       \
+        _Pragma("unroll") for (int i_ = 0; i_ < RW_; ++i_) (facc)[i_] = 0.f;                                                      \
+        _Pragma("unroll") for (int q_ = 0; q_ < (QCH); ++q_) {                                                                    \
+            const uint4 wq_ = wp_[q_ * 32];                                                                                       \
+            uint32_t t_[(SYM) ? 8 : 16];                                                                                          \
+            if (SYM) {                                                                                                            \
+                const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[2 * q_], b_ = reinterpret_cast<const uint4 *>(tab)[2 * q_ + 1]; \
+                t_[0] = a_.x; t_[1] = a_.y; t_[2] = a_.z; t_[3] = a_.w; t_[4] = b_.x; t_[5] = b_.y; t_[6] = b_.z; t_[7] = b_.w;    \
+            } else {                                                                                                              \
+                _Pragma("unroll") for (int k_ = 0; k_ < 4; ++k_) {                                                                \
+                    const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[4 * q_ + k_];                                           \
+                    t_[4 * k_] = a_.x; t_[4 * k_ + 1] = a_.y; t_[4 * k_ + 2] = a_.z; t_[4 * k_ + 3] = a_.w;                       \
+                }                                                                                                                 \
+            }                                                                                                                     \
+            Quad<PB, SYM>::run(wq_, t_, (iacc), (wtx), (wty));                                                                    \
+            if ((AGQ) && ((q_ + 1) % AQ_) == 0) {                                                                                 \
+                _Pragma("unroll") for (int i_ = 0; i_ < RW_; ++i_) {                                                              \
+                    (facc)[i_] = fmaf((lsv)[q_ / AQ_], (float)(iacc)[i_], (facc)[i_]);                                            \
+                    (iacc)[i_] = 0;                                                                                               \
+                }                                                                                                                 \
+            }                                                                                                                     \
+        }                                                                                                                         \
+    } while (0)
+// TMAC_BLOCK_SCALES: cacc[i] += 0.5*s * (facc[i] + lbsum) (+ z * lbsum) with the weight scale s (scale0 for one_scale tensors)
+// and zero point z of the lane's row i: tbl.cc:435-529 re-associated, lbsum = the LUT biases of the chunk's activation groups.
+#define TMAC_BLOCK_SCALES(PB, QCH, stage, lane, one_scale, scale0, sd, zp, facc, lbsum, cacc)                                     \
+    do {                                                                                                                          \
+        constexpr int RW_ = 8 / (PB), RSB_ = 32 * RW_;                                                                            \
+        const unsigned char *sp_ = (stage) + (size_t)(QCH) * 512;                                                                 \
+        _Pragma("unroll") for (int i_ = 0; i_ < RW_; ++i_) {                                                                      \
+            const float s_ = (one_scale) ? (scale0) : load_scale(sp_, (sd), (lane) * RW_ + i_);                                   \
+            float v_ = fmaf(0.5f * s_, (facc)[i_] + (lbsum), (cacc)[i_]);                                                         \
+            if (zp) v_ = fmaf(load_scale(sp_ + (size_t)RSB_ * (sd), (sd), (lane) * RW_ + i_), (lbsum), v_);                       \
+            (cacc)[i_] = v_;                                                                                                      \
+        }                                                                                                                         \
+    } while (0)
 
 // ==========================================================================================
 // gemv3_kernel -- the production GEMV.
@@ -327,8 +400,8 @@ struct Gemv3Params {
     int npeer;
     void *Cpeer[7];
 };
-#ifdef TMAC_ENABLE_TRACE
 __device__ __forceinline__ long long globaltimer_ns() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+#ifdef TMAC_ENABLE_TRACE
 // slots 0..6: clock64 (SM cycles) since entry; slot 7: globaltimer (ns) at entry.
 #define TMAC_TRACE(slot) do { if (p.trace) p.trace[(size_t)blockIdx.x * 8 + (slot)] = globaltimer_ns(); } while (0)
 #else
@@ -345,12 +418,12 @@ __device__ __forceinline__ uint64_t policy_evict_first() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     return pol;
 }
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc, uint64_t pol) {
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc), "l"(pol) : "memory");
+    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void cp_async16_plain(void *smem_dst, const void *gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
@@ -358,28 +431,32 @@ __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// Split barrier used to establish "every CTA of the cluster is running" before the first
-// distributed-shared-memory access (required by the programming model), without stalling at entry.
+// Split cluster barrier.  gemv3 uses it to establish "every CTA of the cluster is running" before the first distributed-shared-
+// memory access (required by the programming model) without stalling at entry; chain_kernel to guard only the RE-USE of shared-
+// memory buffers, whose readers have consumed their values before they arrive.  Neither carries data, so the arrive needs no
+// release -- which ptxas turns into MEMBAR.ALL.GPU per thread.  (barrier.cluster.wait has only the acquire form.)
 __device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
 __device__ __forceinline__ void st_cluster_f32(float *local_ptr, uint32_t rank, float v) {
-    uint32_t laddr = (uint32_t)__cvta_generic_to_shared(local_ptr), raddr;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(laddr), "r"(rank));
+    uint32_t raddr;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(smem_u32(local_ptr)), "r"(rank));
     asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(raddr), "f"(v) : "memory");
 }
 
-// One bulk (TMA) copy per block instead of a per-lane cp.async loop: 1 instruction from one lane instead of
-// ~4 per 16 bytes on the ALU pipe that the lookup loop saturates; completion on a warp-private mbarrier.
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init1(uint64_t *b) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(b)) : "memory");
+// mbarriers and bulk (TMA) copies.  One bulk copy per block instead of a per-lane cp.async loop: 1 instruction from one lane
+// instead of ~4 per 16 bytes on the ALU pipe that the lookup loop saturates; completion on an mbarrier.
+__device__ __forceinline__ void mbar_init(uint64_t *b, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_fence_init() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// generic-proxy shared-memory accesses before this point are ordered before later bulk copies / wgmma reads (async proxy)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint64_t *b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory"); }
+__device__ __forceinline__ void expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_load(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+    expect_tx(bar, bytes);
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
@@ -387,6 +464,21 @@ __device__ __forceinline__ void mbar_wait_parity(uint64_t *b, uint32_t parity) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}\n"
         ::"r"(smem_u32(b)), "r"(parity) : "memory");
+}
+// Bounded form of the persistent kernels: false if the phase has not completed after LIMIT polls.
+template <int LIMIT> __device__ __forceinline__ bool mbar_wait_bounded(uint64_t *b, uint32_t parity) {
+    uint32_t ok = 0;
+    for (int spins = 0; spins < LIMIT && !ok; ++spins)
+        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
+                     : "=r"(ok) : "r"(smem_u32(b)), "r"(parity) : "memory");
+    return ok != 0;
+}
+
+// One output element C[i], fp16 or fp32.  C by reference and i of the caller's type: the pointer is then read inside the branch
+// and the index widened as at the call site, as in the stores this replaced, and every epilogue compiles as before.
+template <typename I> __device__ __forceinline__ void store_out(void *const &C, I i, float v, int f16) {
+    if (f16) reinterpret_cast<__half *>(C)[i] = __float2half_rn(v);
+    else reinterpret_cast<float *>(C)[i] = v;
 }
 
 constexpr int kG3MaxWarps = 8;
@@ -457,8 +549,9 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 
     // ---- first chunk: HBM -> shared, issued before the dependency wait -------------------------
     if (lane == 0) {
-        mbar_init1(mbar); mbar_init1(mbar + 1);
+        mbar_init(mbar, 1); mbar_init(mbar + 1, 1);
         mbar_fence_init();
+        fence_proxy_async();
         if (c_first < c_end) {
             bulk_load(stage0, rsb_base + (size_t)c_first * p.blk_bytes, (uint32_t)p.blk_bytes, mbar);
             if (p.Wnext)                           // pull the next tensor's blocks of this warp into L2
@@ -563,22 +656,15 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         // ---- LUT slice of this chunk -> warp-private table (lane = group) ---------------------
         float lsv[NAG], lbsum = 0.f;
         if (FUSED) {
-            // lane = K-group of the chunk; W = lanes per activation group
-            constexpr int NG = QCH * 4, W = (AGQ ? AGQ : 1) * 4;
+            constexpr int NG = QCH * 4;            // lane = K-group of the chunk
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
             if (lane < NG) load_group(((size_t)c * NG + lane) * 4, x);
-            uint32_t lo, hi;
-            float scale, l0;
-            if (INT_PATH) lut_stored(x.x, x.y, x.z, x.w, row_ts, lo, hi);
-            else l0 = lut_group<W>(x.x, x.y, x.z, x.w, lo, hi, scale);
-            if (lane < NG) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
-            if (!INT_PATH) {
-                const float blk = lut_addv8(l0);
-#pragma unroll
-                for (int a = 0; a < NAG; ++a) {
-                    lsv[a] = __shfl_sync(0xffffffffu, scale, a * W);
-                    lbsum += lut_bias<W>(blk, a * W);
-                }
+            if (INT_PATH) {
+                uint32_t lo, hi;
+                lut_stored(x.x, x.y, x.z, x.w, row_ts, lo, hi);
+                if (lane < NG) reinterpret_cast<uint2 *>(tab)[lane] = make_uint2(lo, hi);
+            } else {
+                lbsum = lut_slice<(AGQ ? AGQ : 1) * 4, NAG>(x.x, x.y, x.z, x.w, lane, tab, lsv);
             }
         } else {
             if (lane < QCH * 4) {
@@ -595,50 +681,19 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         unsigned char *stage = stage0 + (size_t)buf * p.blk_bytes;
         if (nbuf == 2) {
             if (c + 1 < c_end && lane == 0) {      // request chunk c+1 into the other buffer (consumed at c-1, see the __syncwarp below)
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                fence_proxy_async();
                 bulk_load(stage0 + (size_t)((li + 1) & 1) * p.blk_bytes, rsb_base + (size_t)(c + 1) * p.blk_bytes, (uint32_t)p.blk_bytes, mbar + ((li + 1) & 1));
             }
         } else if (li > 0 && lane == 0) {          // single buffer: the other resident warps cover this warp's load latency
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             bulk_load(stage0, rsb_base + (size_t)c * p.blk_bytes, (uint32_t)p.blk_bytes, mbar);
         }
         mbar_wait_parity(mbar + buf, nbuf == 2 ? ((li >> 1) & 1) : (li & 1));
         __syncwarp();
         if (tid == 0 && c == c_first) TMAC_TRACE(3);
-        const uint4 *wp = reinterpret_cast<const uint4 *>(stage) + lane;
         float facc[RW];
-#pragma unroll
-        for (int i = 0; i < RW; ++i) facc[i] = 0.f;
-#pragma unroll
-        for (int q = 0; q < QCH; ++q) {
-            const uint4 wq = wp[q * 32];
-            uint32_t t[SYM ? 8 : 16];
-            if (SYM) {
-                const uint4 a = reinterpret_cast<const uint4 *>(tab)[2 * q], b2 = reinterpret_cast<const uint4 *>(tab)[2 * q + 1];
-                t[0] = a.x; t[1] = a.y; t[2] = a.z; t[3] = a.w; t[4] = b2.x; t[5] = b2.y; t[6] = b2.z; t[7] = b2.w;
-            } else {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint4 a = reinterpret_cast<const uint4 *>(tab)[4 * q + k];
-                    t[4 * k] = a.x; t[4 * k + 1] = a.y; t[4 * k + 2] = a.z; t[4 * k + 3] = a.w;
-                }
-            }
-            Quad<PB, SYM>::run(wq, t, iacc, wtx, wty);
-            if (!INT_PATH && ((q + 1) % (AGQ ? AGQ : 1)) == 0) {
-#pragma unroll
-                for (int i = 0; i < RW; ++i) { facc[i] = fmaf(lsv[q / (AGQ ? AGQ : 1)], (float)iacc[i], facc[i]); iacc[i] = 0; }
-            }
-        }
-        if (!INT_PATH) {
-            const unsigned char *sp = stage + (size_t)QCH * 512;
-#pragma unroll
-            for (int i = 0; i < RW; ++i) {
-                const float s = p.one_scale ? p.scale0 : load_scale(sp, p.sd, lane * RW + i);
-                float v = fmaf(0.5f * s, facc[i] + lbsum, cacc[i]);
-                if (p.zp) v = fmaf(load_scale(sp + (size_t)RSB * p.sd, p.sd, lane * RW + i), lbsum, v);
-                cacc[i] = v;
-            }
-        }
+        TMAC_BLOCK_LOOKUPS(PB, SYM, QCH, AGQ, stage, tab, lane, wtx, wty, lsv, iacc, facc);
+        if (!INT_PATH) TMAC_BLOCK_SCALES(PB, QCH, stage, lane, p.one_scale, p.scale0, p.sd, p.zp, facc, lbsum, cacc);
         __syncwarp();                              // stage / table are rewritten by a later chunk
     }
     if (tid == 0) TMAC_TRACE(4);
@@ -691,12 +746,9 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             } else
                 out = fsum;
             const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
-            if (p.out_f16) reinterpret_cast<__half *>(Cb)[o] = __float2half_rn(out);
-            else reinterpret_cast<float *>(Cb)[o] = out;
-            for (int q = 0; q < p.npeer; ++q) {      // the all-gather, fused into the epilogue: one store per peer and row
-                if (p.out_f16) reinterpret_cast<__half *>(p.Cpeer[q])[o] = __float2half_rn(out);
-                else reinterpret_cast<float *>(p.Cpeer[q])[o] = out;
-            }
+            store_out(Cb, o, out, p.out_f16);
+            for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
+                store_out(p.Cpeer[q], o, out, p.out_f16);
         }
     }
     if (tid == 0) TMAC_TRACE(7);

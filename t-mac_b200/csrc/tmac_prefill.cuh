@@ -50,7 +50,6 @@ struct PrefillParams {
 constexpr int kPfNT = 128;                       // tokens per CTA pass (MMA N)
 constexpr int kPfStageBytes = 128 * 128;         // one operand tile: 128 rows x 128 contraction bytes
 
-__device__ __forceinline__ uint32_t pf_s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // wgmma shared-memory descriptor, K-major, no swizzle: core matrix = 8 rows x 16 B (128 B) at (kc*G + rn)*128 for K chunk kc,
 // row group rn (G row groups per chunk); leading byte offset = distance between K chunks (G*128), stride byte offset = 128.
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo) {
@@ -86,14 +85,6 @@ __device__ __forceinline__ void wg_mma_s8_n128(uint32_t (&d)[64], uint64_t da, u
                  : "l"(da), "l"(db), "r"(acc));
 }
 
-__device__ __forceinline__ void pf_mbar_init(uint64_t *b, uint32_t c) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(pf_s32(b)), "r"(c)); }
-__device__ __forceinline__ void pf_mbar_arrive(uint64_t *b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(pf_s32(b)) : "memory"); }
-__device__ __forceinline__ void pf_mbar_wait(uint64_t *b, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}\n"
-        ::"r"(pf_s32(b)), "r"(parity) : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------------
 // lut_tile_kernel: QLUT [N][K/4][16] + LUT_Scales/Biases [N][K/64]  ->  per (token tile of 128, activation group) one
 // contiguous 17920-byte record that the GEMM stage receives with ONE bulk copy (TMA):
@@ -125,14 +116,6 @@ constexpr int kPfStages = 4;                     // stages: A tile 16 KB (expand
 constexpr int kPfConsWarps = 8;                  // two consumer warpgroups
 constexpr int kPfProdWarps = 4;                  // one producer warpgroup
 constexpr int kPfThreads2 = (kPfConsWarps + kPfProdWarps) * 32;
-
-__device__ __forceinline__ void pf_bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(pf_s32(dst)), "l"(src), "r"(bytes), "r"(pf_s32(bar)) : "memory");
-}
-__device__ __forceinline__ void pf_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(pf_s32(bar)), "r"(bytes) : "memory");
-}
 
 // PB 4 expansion table: 512 entries, each indexed by one byte of a row's 16-bit code field (two planes, nibble = neg << 3 | j),
 //   [0, 256)    planes 0, 1: +-w0 at byte j0 plus +-w1 at byte j1
@@ -193,8 +176,8 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
         pf_build_xtab4(xtab, p.bits, false, tid, kPfThreads2);
     }
     if (tid == 0) {
-        for (int i = 0; i < kPfStages; ++i) { pf_mbar_init(full + i, kPfProdWarps + 1); pf_mbar_init(empty + i, kPfConsWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int i = 0; i < kPfStages; ++i) { mbar_init(full + i, kPfProdWarps + 1); mbar_init(empty + i, kPfConsWarps); }
+        mbar_fence_init();
     }
     __syncthreads();
     const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
@@ -233,11 +216,10 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
             for (int h = 0; h < 2; ++h) {
                 const int step = 2 * c + h, s = step % kPfStages;
                 if (r == 0) PF_TRACE(0, step, 0);
-                pf_mbar_wait(empty + s, ((step / kPfStages) & 1) ^ 1);     // stage released by the consumers of step - S
+                mbar_wait_parity(empty + s, ((step / kPfStages) & 1) ^ 1);     // stage released by the consumers of step - S
                 if (r == 0) {
                     PF_TRACE(0, step, 1);
-                    pf_expect_tx(full + s, kPfRec);
-                    pf_bulk_g2s(sR + (size_t)s * kPfRec, rec_src + (size_t)step * kPfRec, kPfRec, full + s);
+                    bulk_load(sR + (size_t)s * kPfRec, rec_src + (size_t)step * kPfRec, kPfRec, full + s);
                 }
                 unsigned char *a_dst = sA + (size_t)s * kPfStageBytes;
 #pragma unroll
@@ -265,9 +247,9 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                         make_uint4((uint32_t)v2[0], (uint32_t)(v2[0] >> 32), (uint32_t)v2[1], (uint32_t)(v2[1] >> 32));
                 }
                 if (r == 0) PF_TRACE(0, step, 2);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                fence_proxy_async();
                 __syncwarp();
-                if (lane == 0) pf_mbar_arrive(full + s);
+                if (lane == 0) mbar_arrive(full + s);
                 __syncwarp();
             }
         }
@@ -300,9 +282,9 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                 for (int h = 0; h < 2; ++h) { hs_n[h] = ld_s(c + 1, r0 + 8 * h); zz_n[h] = ld_z(c + 1, r0 + 8 * h); }
             }
             if (tid == 0) PF_TRACE(1, step, 0);
-            pf_mbar_wait(full + s, (step / kPfStages) & 1);
+            mbar_wait_parity(full + s, (step / kPfStages) & 1);
             if (tid == 0) PF_TRACE(1, step, 1);
-            const uint32_t a0 = pf_s32(sA + (size_t)s * kPfStageBytes) + wg * 1024, b0 = pf_s32(sR + (size_t)s * kPfRec);
+            const uint32_t a0 = smem_u32(sA + (size_t)s * kPfStageBytes) + wg * 1024, b0 = smem_u32(sR + (size_t)s * kPfRec);
             wg_fence();
 #pragma unroll
             for (int i = 0; i < 4; ++i) wg_mma_s8_n128(acc, wg_desc(a0 + i * 4096, 2048), wg_desc(b0 + i * 4096, 2048), i > 0 ? 1u : 0u);
@@ -340,7 +322,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                 for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h]; zz[h] = zz_n[h]; }
             }
             __syncwarp();
-            if (lane == 0) pf_mbar_arrive(empty + s);        // A tile and record of this step are dead: the stage may be refilled
+            if (lane == 0) mbar_arrive(empty + s);        // A tile and record of this step are dead: the stage may be refilled
             __syncwarp();
         }
 #pragma unroll
@@ -352,12 +334,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int t = 8 * c8 + tc + e;
-                    if (t < ntok) {
-                        const size_t o = (size_t)(n0 + t) * p.ldc + row;
-                        const float val = accf[4 * c8 + 2 * h + e];
-                        if (p.out_f16) reinterpret_cast<__half *>(p.C)[o] = __float2half_rn(val);
-                        else reinterpret_cast<float *>(p.C)[o] = val;
-                    }
+                    if (t < ntok) store_out(p.C, (size_t)(n0 + t) * p.ldc + row, accf[4 * c8 + 2 * h + e], p.out_f16);
                 }
         }
     }

@@ -154,8 +154,8 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
 
     if constexpr (PB == 4) pf_build_xtab4(xtab, p.bits, true, tid, kP16Threads);
     if (tid == 0) {
-        for (int i = 0; i < kP16NA; ++i) { pf_mbar_init(full + i, kP16ProdWarps + 1); pf_mbar_init(empty + i, kP16ConsWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int i = 0; i < kP16NA; ++i) { mbar_init(full + i, kP16ProdWarps + 1); mbar_init(empty + i, kP16ConsWarps); }
+        mbar_fence_init();
     }
     __syncthreads();
 
@@ -172,17 +172,16 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
         int it = 0;                                  // running step counter over both fragments
         auto stage_in = [&](int f, int u) {          // wait for a free stage, request its B tile; returns the A tile
             const int s = it % kP16NA;
-            pf_mbar_wait(empty + s, ((it / kP16NA) & 1) ^ 1);   // the MMAs that read this stage have completed
+            mbar_wait_parity(empty + s, ((it / kP16NA) & 1) ^ 1);   // the MMAs that read this stage have completed
             if (r == 0) {
-                pf_expect_tx(full + s, kP16SubB);
-                pf_bulk_g2s(sB + (size_t)s * kP16SubB, p.tiles + ((size_t)(ft[f] / p.nrt) * nsteps + u) * kP16BBytes, kP16SubB, full + s);
+                bulk_load(sB + (size_t)s * kP16SubB, p.tiles + ((size_t)(ft[f] / p.nrt) * nsteps + u) * kP16BBytes, kP16SubB, full + s);
             }
             return sA + (size_t)s * kP16SubA;
         };
         auto stage_out = [&]() {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            fence_proxy_async();
             __syncwarp();
-            if (lane == 0) pf_mbar_arrive(full + it % kP16NA);
+            if (lane == 0) mbar_arrive(full + it % kP16NA);
             __syncwarp();
             ++it;
         };
@@ -299,8 +298,8 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
             if (f == nfrag) break;
             for (int u = fs0[f]; u < fs1[f]; ++u, ++it) {
                 const int s = it % kP16NA;
-                pf_mbar_wait(full + s, (it / kP16NA) & 1);
-                const uint32_t a0 = pf_s32(sA + (size_t)s * kP16SubA) + wg * 1024, b0 = pf_s32(sB + (size_t)s * kP16SubB);
+                mbar_wait_parity(full + s, (it / kP16NA) & 1);
+                const uint32_t a0 = smem_u32(sA + (size_t)s * kP16SubA) + wg * 1024, b0 = smem_u32(sB + (size_t)s * kP16SubB);
                 wg_fence();
 #pragma unroll
                 for (int i = 0; i < 8; ++i)         // K = 16 entries = two 16-byte chunks per MMA
@@ -309,7 +308,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                 wg_wait0();
                 wg_fence_acc(acc);
                 __syncwarp();
-                if (lane == 0) pf_mbar_arrive(empty + s);              // both tiles of the stage are free
+                if (lane == 0) mbar_arrive(empty + s);              // both tiles of the stage are free
                 __syncwarp();
             }
             const bool whole = fs0[f] == 0 && fs1[f] == nsteps, last = fs1[f] == nsteps;
@@ -323,12 +322,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int t = 8 * c8 + tc + e;
-                            if (t < ntok && row < p.Mout) {
-                                const size_t o = (size_t)(n0 + t) * p.ldc + row;
-                                const float val = acc[4 * c8 + 2 * h + e];
-                                if (p.out_f16) reinterpret_cast<__half *>(p.C)[o] = __float2half_rn(val);
-                                else reinterpret_cast<float *>(p.C)[o] = val;
-                            }
+                            if (t < ntok && row < p.Mout) store_out(p.C, (size_t)(n0 + t) * p.ldc + row, acc[4 * c8 + 2 * h + e], p.out_f16);
                         }
                 }
                 continue;
@@ -364,11 +358,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                 float sum = 0.f;
                 for (int c2 = c_first; c2 < cta; ++c2) sum += __ldcg(p.scratch + ((size_t)c2 * kP16NT + t) * 128 + er);
                 sum += __ldcg(mine + (size_t)t * 128 + er);
-                if (row < p.Mout) {
-                    const size_t o = (size_t)(n0 + t) * p.ldc + row;
-                    if (p.out_f16) reinterpret_cast<__half *>(p.C)[o] = __float2half_rn(sum);
-                    else reinterpret_cast<float *>(p.C)[o] = sum;
-                }
+                if (row < p.Mout) store_out(p.C, (size_t)(n0 + t) * p.ldc + row, sum, p.out_f16);
             }
             asm volatile("bar.sync 2, 256;" ::: "memory");                 // all partial reads done: the flags can be reused by the next launch
             if (tid == 0) for (int c2 = c_first; c2 < cta; ++c2) asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p.flags + c2), "r"(0) : "memory");

@@ -79,8 +79,6 @@ struct SeqParams {
     long long *trace;                     // optional [nops][grid][16] globaltimer stamps, followed by [nops][grid][NW][16] per-warp clock64 stamps
 };
 
-__device__ __forceinline__ long long seq_timer() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-
 __device__ __forceinline__ void seq_publish(uint2 *slot, uint32_t bits, uint32_t epoch) {
     asm volatile("st.relaxed.gpu.global.v2.u32 [%0], {%1, %2};" ::"l"(slot), "r"(bits), "r"(epoch) : "memory");
 }
@@ -112,13 +110,6 @@ __device__ __forceinline__ uint4 seq_wait(const void *slot, bool active, uint32_
     return v;
 }
 __device__ __forceinline__ void seq_bar(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(kSeqWarps * 32) : "memory"); }
-__device__ __forceinline__ bool seq_mbar_wait(uint64_t *b, uint32_t parity) {
-    uint32_t ok = 0;
-    for (int spins = 0; spins < kSeqSpinLimit && !ok; ++spins)
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(smem_u32(b)), "r"(parity) : "memory");
-    return ok != 0;
-}
 __device__ __forceinline__ int ld_volatile_s32(const int *p) { int v; asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory"); return v; }
 __device__ __forceinline__ void st_volatile_s32(int *p, int v) { asm volatile("st.volatile.shared.s32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory"); }
 
@@ -166,8 +157,9 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
     const uint32_t epoch = p.epochs[cta] + 1u;
 
     if (tid == 0) {
-        for (int s = 0; s < p.nslots; ++s) mbar_init1(full + s);
+        for (int s = 0; s < p.nslots; ++s) mbar_init(full + s, 1);
         mbar_fence_init();
+        fence_proxy_async();
     }
     if (tid <= NW) prog[tid] = 0;                  // prog[NW] = issued
     static_assert(sizeof(SeqOp) <= 160 && sizeof(SeqCta) == 64, "descriptor staging layout");
@@ -191,7 +183,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
             const unsigned char *W = o.W;
             const unsigned long long rs = o.rsb_stride;
             int sb = q.sb_first, c = q.c0;
-            if (p.trace) p.trace[((size_t)op * G + cta) * 16 + 8] = seq_timer();     // producer reaches this op
+            if (p.trace) p.trace[((size_t)op * G + cta) * 16 + 8] = globaltimer_ns();  // producer reaches this op
             for (int b = b0; b < b1; ++b, ++seq) {
                 if (seq >= p.nslots) {                         // slot still holds block seq - nslots: wait until nobody needs it
                     const int need = seq - p.nslots + 1;
@@ -205,13 +197,13 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                         if (++spins > kSeqSpinLimit) { atomicExch(p.err, 1); return; }
                     }
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                fence_proxy_async();
                 bulk_load(ring + (size_t)slot * p.slot_bytes, W + (size_t)sb * rs + (size_t)c * blk, (uint32_t)blk, full + slot);
                 st_volatile_s32(issued, seq + 1);              // the phase parity of `full` is only meaningful once the request is out
                 if (++slot == p.nslots) slot = 0;
                 if (++c == nchunk) { c = 0; ++sb; }
             }
-            if (p.trace) p.trace[((size_t)op * G + cta) * 16 + 9] = seq_timer();     // ... and has requested all of its blocks
+            if (p.trace) p.trace[((size_t)op * G + cta) * 16 + 9] = globaltimer_ns();  // ... and has requested all of its blocks
         }
         return;
     }
@@ -245,8 +237,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
         if (lane == 0) st_volatile_s32(prog + warp, seq_base);
         long long *tr = p.trace ? p.trace + ((size_t)op * G + cta) * 16 : nullptr;
         long long *tw = (p.trace && lane == 0) ? p.trace + (size_t)p.nops * G * 16 + (((size_t)op * G + cta) * NW + warp) * 16 : nullptr;
-        if (tw) { tw[0] = clock64(); tw[12] = seq_timer(); }
-        if (tr && tid == 0) { tr[0] = seq_timer(); tr[10] = 0; }
+        if (tw) { tw[0] = clock64(); tw[12] = globaltimer_ns(); }
+        if (tr && tid == 0) { tr[0] = globaltimer_ns(); tr[10] = 0; }
         if (tr && warp == NW - 1 && lane == 0) tr[11] = 0;
 
         // ---- (A) LUT slices of my chunks: thread = K-group.  Either fetched ready-made (built by the CTAs that finished the
@@ -296,7 +288,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                 }
             }
         }
-        if (tr && tid == 0) tr[1] = seq_timer();      // (stamps right after a bar.sync would show its issue, not its release)
+        if (tr && tid == 0) tr[1] = globaltimer_ns();   // (stamps right after a bar.sync would show its issue, not its release)
         if (tw) tw[1] = clock64();
         seq_bar(1);
         long long ck1 = 0;
@@ -344,10 +336,10 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                     if (tw && ck1) tw[3] = tw0;
                     int spins = 0;
                     while (ld_volatile_s32(issued) <= seq_base + j && ++spins < kSeqSpinLimit) __nanosleep(100);
-                    if (spins >= kSeqSpinLimit || !seq_mbar_wait(full + slot, (uint32_t)par)) atomicExch(p.err, 4);
+                    if (spins >= kSeqSpinLimit || !mbar_wait_bounded<kSeqSpinLimit>(full + slot, (uint32_t)par)) atomicExch(p.err, 4);
                     if (tr && lane == 0 && (warp == 0 || warp == NW - 1)) tr[warp == 0 ? 10 : 11] += clock64() - tw0;   // cycles waiting for weights
                 }
-                if (tr && tid == 0 && u == 0) tr[2] = seq_timer();      // first block of the share is resident
+                if (tr && tid == 0 && u == 0) tr[2] = globaltimer_ns();   // first block of the share is resident
                 if (tw && ck1) { tw[4] = clock64(); ck1 = 0; }           // my first block is resident
                 const unsigned char *stage = ring + (size_t)slot * p.slot_bytes;
                 const uint4 *wp = reinterpret_cast<const uint4 *>(stage) + lane;
@@ -409,7 +401,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                 for (int i = 0; i < RW; ++i) r[i] = cacc[i];
             }
         }
-        if (tr && lane == 0 && (warp == 0 || warp == NW / 2 || warp == NW - 1)) tr[warp == 0 ? 3 : (warp == NW - 1 ? 4 : 5)] = seq_timer();
+        if (tr && lane == 0 && (warp == 0 || warp == NW / 2 || warp == NW - 1)) tr[warp == 0 ? 3 : (warp == NW - 1 ? 4 : 5)] = globaltimer_ns();
         if (tw) tw[5] = clock64();
         if (tid < 56) desc[((op + 1) & 1) * kSeqDescWords + tid] = next_word;
         seq_bar(2);
@@ -422,7 +414,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
             float mine = 0.f;
 #pragma unroll 4
             for (int w = 0; w < NW; ++w) mine += red[((size_t)s * NW + w) * RSB + t];
-            if (tr && item == 0) tr[6] = seq_timer() + (mine == 1.2345e-30f);    // after the barrier released and the sums are in
+            if (tr && item == 0) tr[6] = globaltimer_ns() + (mine == 1.2345e-30f); // after the barrier released and the sums are in
             if (tw && item < NW * 32) tw[6] = clock64() + (mine == 1.2345e-30f);
             if (!ends_here) {                                   // continues in the next CTA (always my last super-block)
                 seq_publish(xchg + (size_t)cta * RSB + t, __float_as_uint(mine), epoch);
@@ -437,10 +429,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
             if (tw && item < NW * 32) tw[7] = clock64() + (fsum == 1.2345e-30f);
             const int row = sb * RSB + t;
             if (row < Mout) {
-                if (Cout) {
-                    if (out_f16) reinterpret_cast<__half *>(Cout)[row] = __float2half_rn(fsum);
-                    else reinterpret_cast<float *>(Cout)[row] = fsum;
-                }
+                if (Cout) store_out(Cout, row, fsum, out_f16);
                 seq_publish(yv + row, __float_as_uint(fsum), epoch);
             }
             if (lut_out) yfin[item] = row < Mout ? fsum : 0.f;
@@ -490,7 +479,7 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                 }
             }
         }
-        if (tr && tid == 0) tr[7] = seq_timer();
+        if (tr && tid == 0) tr[7] = globaltimer_ns();
         if (tw) tw[11] = clock64();
         seq_base += nb;
         slot_base += nb;
