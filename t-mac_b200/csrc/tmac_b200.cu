@@ -417,19 +417,24 @@ int tile_min_n(const StreamLayout &L) {
     return (L.pb == 4 && (L.nrsb + 1) / 2 < 64) ? 128 : 32;
 }
 
+// Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): W2 or W3/W4 streams, chunk 128,
+// act group 64, per-row scales, N >= tile_min_n.
+bool takes_prefill_tile(const StreamLayout &L, int N) {
+    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && L.qch == 8 && L.act_group_size == 64 && !L.one_scale;
+}
+
 // Prefill tile on the tensor cores (wgmma, tmac_prefill.cuh).  Returns 1 if the shape is not covered (caller falls back to the GEMV
 // kernel per activation row), 0 on launch, -1 on error.
 int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls, const float *lb, void *C, int ldc, int out_f16, bool sym) {
     const StreamLayout &L = R.L;
-    if (!g.use_prefill || N < tile_min_n(L) || !sym) return 1;
-    if ((L.pb != 2 && L.pb != 4) || L.qch != 8 || L.act_group_size != 64 || L.one_scale || L.ck != 128) return 1;
+    if (!sym || !takes_prefill_tile(L, N)) return 1;
     const size_t rawsz = (L.blk + 127) & ~(size_t)127;
     // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
     const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
-    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = L.pb == 4 ? 512 * 8 : 0;   // + the PB 4 expansion table
+    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
     if (g.use_prefill16 && N >= 64) {   // fp path: scales folded into fp16 operands, fp32 accumulation over K in registers (tmac_prefill16.cuh)
         const int nmain = L.K / 64, nextra = (L.nchunk + 31) / 32, ntile16 = (N + kP16NT - 1) / kP16NT;
-        const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + xtab + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
+        const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
         if (smem16 <= 227 * 1024) {
             if (g.d_tiles.ensure((size_t)ntile16 * (nmain + nextra) * kP16BBytes)) return fail("out of device memory (LUT tiles)");
             lut_tile16_kernel<<<dim3(nmain + nextra, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, nmain, nextra);
@@ -451,17 +456,16 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
                 }
                 q.scratch = (float *)g.d_pf_scratch.p; q.flags = (int *)g.d_pf_flags.p;
             }
-            const void *fn16 = L.pb == 4 ? (const void *)prefill16_kernel<4> : (const void *)prefill16_kernel<2>;
-            CUDA_OK(cudaFuncSetAttribute(fn16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
-            if (L.pb == 4) prefill16_kernel<4><<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
-            else prefill16_kernel<2><<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
+            const auto fn16 = L.pb == 4 ? prefill16_kernel<4> : prefill16_kernel<2>;
+            CUDA_OK(cudaFuncSetAttribute((const void *)fn16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
+            fn16<<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
             CUDA_OK(cudaGetLastError());
             g.last_launch[0] = 16; g.last_launch[1] = kP16Threads / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = q.streamk; g.last_launch[4] = grid;
             g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;
             return 0;
         }
     }
-    const size_t smem = (size_t)kPfStages * (kPfStageBytes + kPfRec) + rawall + (L.pb == 4 ? 512 : 256) * 8 + (2 * kPfStages + 4) * 8 + 1024;
+    const size_t smem = (size_t)kPfStages * (kPfStageBytes + kPfRec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
     if (smem > 225 * 1024) return 1;
     const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;
     if (g.d_tiles.ensure((size_t)ntile * nag * kPfRec)) return fail("out of device memory (LUT tiles)");
@@ -478,11 +482,9 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
         CUDA_OK(cudaMemsetAsync(g.d_trace.p, 0, 3 * 32 * 4 * sizeof(long long), g.stream()));
         p.dbg = (long long *)g.d_trace.p; g.trace_ctas = 12;   // 96 rows of 4 = 48 rows of 8
     }
-    const void *fn = L.pb == 4 ? (const void *)prefill_kernel<4> : (const void *)prefill_kernel<2>;
-    CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(nrt, ntile);
-    if (L.pb == 4) prefill_kernel<4><<<grid, kPfThreads2, smem, g.stream()>>>(p);
-    else prefill_kernel<2><<<grid, kPfThreads2, smem, g.stream()>>>(p);
+    const auto fn = L.pb == 4 ? prefill_kernel<4> : prefill_kernel<2>;
+    CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    fn<<<dim3(nrt, ntile), kPfThreads2, smem, g.stream()>>>(p);
     CUDA_OK(cudaGetLastError());
     g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = 1; g.last_launch[4] = nrt;
     g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;   // batch < 0 marks the tensor-core prefill tile
@@ -492,8 +494,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
 // Launch qgemm_lut over rows [row_begin,row_end) (relative to the resident tensor): the tensor-core tile for whole-tensor batches,
 // else gemv3_kernel.  All pointers are device pointers; C is [N][ldc] with C[n][row - c_row0].
 int launch_gemv(const Resident &R, int row_begin, int row_end, int N, const int8_t *qlut, const float *ls,
-                const float *lb, void *C, int ldc, int c_row0, int out_f16, bool sym, int32_t *cbits_unused) {
-    (void)cbits_unused;
+                const float *lb, void *C, int ldc, int c_row0, int out_f16, bool sym) {
     if (row_begin == 0 && row_end == R.L.Mout && c_row0 == 0 && ldc == R.L.Mout) {
         const int rc = launch_prefill(R, N, qlut, ls, lb, C, ldc, out_f16, sym);
         if (rc <= 0) return rc;
@@ -1096,7 +1097,7 @@ static int qgemm_impl(Resident &R, int row0, int rows, int N, int dtype, const v
         if (!hit) {
             const size_t full = (size_t)N * L.Mout * es;
             if (hl->res.ensure(full)) return fail("out of pinned memory");
-            if (launch_gemv(R, 0, L.Mout, N, dq, dls, dlb, hl->res.p, L.Mout, 0, dtype == TMAC_B200_F16, sym, nullptr)) return -1;
+            if (launch_gemv(R, 0, L.Mout, N, dq, dls, dlb, hl->res.p, L.Mout, 0, dtype == TMAC_B200_F16, sym)) return -1;
             CUDA_OK(cudaStreamSynchronize(g.stream()));
             hl->res_id = R.id; hl->res_dtype = dtype; hl->N = N;
         }
@@ -1110,7 +1111,7 @@ static int qgemm_impl(Resident &R, int row0, int rows, int N, int dtype, const v
         if (g.d_c.ensure(cb)) return fail("out of device memory");
         dC = g.d_c.p;
     }
-    if (launch_gemv(R, row0, row0 + rows, N, dq, dls, dlb, dC, rows, row0, dtype == TMAC_B200_F16, sym, nullptr)) return -1;
+    if (launch_gemv(R, row0, row0 + rows, N, dq, dls, dlb, dC, rows, row0, dtype == TMAC_B200_F16, sym)) return -1;
     if (!dev_c) {
         if (g.h_out.ensure(cb)) return fail("out of pinned memory");
         CUDA_OK(cudaMemcpyAsync(g.h_out.p, dC, cb, cudaMemcpyDeviceToHost, g.stream()));
@@ -1239,8 +1240,7 @@ int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {
     const int kind_b = ptr_kind(B, &pinB), kind_c = ptr_kind(C, &pinC);
     const bool dev_b = kind_b == 2, dev_c = kind_c == 2;
     const bool int_path = L.one_scale && L.act_group_size == L.K;
-    const bool prefill_shape = g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && L.qch == 8 && L.act_group_size == 64 && !L.one_scale;
-    const bool can_fuse = g.use_fused && (int_path || L.act_group_size <= L.ck) && g.lut_mode != 1 && !prefill_shape;
+    const bool can_fuse = g.use_fused && (int_path || L.act_group_size <= L.ck) && g.lut_mode != 1 && !takes_prefill_tile(L, N);
     auto launch_compute = [&](const void *dB, void *dC) -> int {
         if (can_fuse)   // one launch: the GEMV builds each chunk's LUT slice itself (bit-identical tables)
             return launch_gemv3(R, 0, L.Mout, N, nullptr, nullptr, nullptr, dC, L.Mout, 0, dtype == TMAC_B200_F16, true, nullptr, dB,
@@ -1248,7 +1248,7 @@ int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {
         if (g.d_qlut.ensure(qb) || g.d_ls.ensure(sb) || g.d_lb.ensure(sb)) return fail("out of device memory");
         if (launch_preprocessor(L.K, N, L.act_group_size, dtype, dB, (float *)g.d_ls.p, (float *)g.d_lb.p, (int8_t *)g.d_qlut.p)) return -1;
         return launch_gemv(R, 0, L.Mout, N, (const int8_t *)g.d_qlut.p, (const float *)g.d_ls.p, (const float *)g.d_lb.p, dC, L.Mout, 0,
-                           dtype == TMAC_B200_F16, g.lut_mode != 1, nullptr);
+                           dtype == TMAC_B200_F16, g.lut_mode != 1);
     };
     // The (small) output is stored by the kernel straight into page-locked host memory the device can address -- the
     // caller's own buffer when it is page-locked, else our staging buffer -- instead of a device buffer + D2H copy.

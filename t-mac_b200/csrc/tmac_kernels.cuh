@@ -214,6 +214,17 @@ __device__ __forceinline__ float load_scale(const unsigned char *p, int sd, int 
     return sd == 2 ? __half2float(reinterpret_cast<const __half *>(p)[i]) : reinterpret_cast<const float *>(p)[i];
 }
 
+// The plane codes of lane-row i, K-group k of a lane's quad w4 (its four words, the stream layout of tmac_layout.h): nibble b of
+// the result is the code (j | neg << 3) of plane b; 16 bits for PB 4, 8 for PB 2, 4 for PB 1.  PB 4 keeps each code whole in
+// word k; PB 2 and PB 1 keep the j bits there and the neg bits of a group pair (PB 2) / quad (PB 1) together in one word.
+template <int PB>
+__device__ __forceinline__ uint32_t row_codes(const uint32_t *w4, int k, int i) {
+    static_assert(PB == 1 || PB == 2 || PB == 4, "planes per word");
+    if constexpr (PB == 4) return (w4[k] >> (16 * i)) & 0xffffu;
+    else if constexpr (PB == 2) return ((w4[k] >> (8 * i)) & 0x77u) | (((w4[2 * (k >> 1) + (i >> 1)] >> (16 * (i & 1) + 8 * (k & 1) + 3)) & 0x11u) << 3);
+    else return ((w4[k] >> (4 * i)) & 7u) | (((w4[i >> 1] >> (16 * (i & 1) + 4 * k + 3)) & 1u) << 3);
+}
+
 // ------------------------------------------------------------------------------------------
 // The activation LUT: the operation order of the AVX2 branch of lut_ctor.cc, with explicit round-to-nearest operations so
 // that no FMA contraction can change a rounding.  Every kernel that builds LUT bytes, LUT scales or LUT biases
@@ -757,7 +768,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 // ------------------------------------------------------------------------------------------
 // cbits_kernel (debug / parity gate G2): per-plane int32 sums in the reference plane layout.
 // One thread per (row, plane); straightforward lookups in the full 16-entry table, decoding the
-// stream layout nibble by nibble.  Not a performance path.
+// stream layout with row_codes.  Not a performance path.
 // ------------------------------------------------------------------------------------------
 static __global__ void cbits_kernel(const unsigned char *W, const int8_t *qlut, int32_t *cbits, int Mout, int K, int bits,
                              int pb, int qch, int nchunk, size_t rsb_stride, size_t blk_stride, int N) {
@@ -777,17 +788,14 @@ static __global__ void cbits_kernel(const unsigned char *W, const int8_t *qlut, 
             const uint32_t *w4 = wq + ((size_t)q * 32 + lane) * 4;
             for (int k = 0; k < 4; ++k) {
                 const int g = (c * qch + q) * 4 + k;
-                uint32_t j, neg;
-                if (pb == 4) { const uint32_t nb = (w4[k] >> (4 * (4 * i + b))) & 15u; j = nb & 7u; neg = nb >> 3; }
-                else if (pb == 2) {
-                    j = (w4[k] >> (4 * (2 * i + b))) & 7u;
-                    const int pair = k >> 1, nn = b + 2 * (k & 1);
-                    neg = (w4[2 * pair + i / 2] >> (16 * (i % 2) + 4 * nn + 3)) & 1u;
-                } else {
-                    j = (w4[k] >> (4 * i)) & 7u;
-                    neg = (w4[i / 2] >> (16 * (i % 2) + 4 * k + 3)) & 1u;
+                uint32_t codes;
+                switch (pb) {
+                case 4: codes = row_codes<4>(w4, k, i); break;
+                case 2: codes = row_codes<2>(w4, k, i); break;
+                default: codes = row_codes<1>(w4, k, i); break;
                 }
-                const uint32_t idx = neg ? (8u | (j ^ 7u)) : j;
+                const uint32_t code = (codes >> (4 * b)) & 15u, j = code & 7u;
+                const uint32_t idx = (code & 8u) ? (8u | (j ^ 7u)) : j;
                 sum += lut[(size_t)g * 16 + idx];
             }
         }

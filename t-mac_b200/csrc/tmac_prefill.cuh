@@ -21,6 +21,10 @@
 //                    K-major no-swizzle canonical layout; fence.proxy.async; arrive full[s].  Thread 0 also issues the
 //                    step's LUT record as one bulk copy (TMA) into the same stage.
 //
+// Shared with the fp16 tile (tmac_prefill16.cuh): the producer's row (PF_PRODUCER_ROW), the double-buffered block staging
+// (PF_STAGE_BLOCKS), the code decode (row_codes, tmac_kernels.cuh), the expansion table (pf_build_xtab) and the scale offset
+// in a block (kPfScaleOff).  Each tile keeps its own expansion of a chunk's codes into A entries.
+//
 // Supported: PB == 2 (W2: a 128-row tile is one super-block) and PB == 4 (W3/W4: two 64-row super-blocks, one per consumer
 // warpgroup), chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points), symmetric LUT.  Everything else
 // takes the GEMV kernel once per activation row.
@@ -117,17 +121,20 @@ constexpr int kPfConsWarps = 8;                  // two consumer warpgroups
 constexpr int kPfProdWarps = 4;                  // one producer warpgroup
 constexpr int kPfThreads2 = (kPfConsWarps + kPfProdWarps) * 32;
 
-// PB 4 expansion table: 512 entries, each indexed by one byte of a row's 16-bit code field (two planes, nibble = neg << 3 | j),
+constexpr int kPfScaleOff = 8 * 512;            // a block's scales follow its QCH 8 quads of 512 B of codes
+
+// Expansion table: 128*PB entries, each indexed by one byte of row_codes<PB> (two planes, nibble = neg << 3 | j),
 //   [0, 256)    planes 0, 1: +-w0 at byte j0 plus +-w1 at byte j1
-//   [256, 512)  planes 2, 3: +-w2 at byte j2 plus +-w3 at byte j3
-// w_b = 2*alpha_b from plane_weight_regs: {1, 2, 4, 8}, W3 {1, 2, 4, 0} (its padded fourth plane is code 0 and must add nothing).
-// biased == false: signed bytes, one entry of each half added byte-wise (__vadd4) is S[e].  biased == true: the bytes of the two
-// halves carry +3 and +13 (|w0| + |w1| <= 3, |w2| + |w3| <= 12), so every byte is non-negative and a plain 32-bit add of one entry
-// of each half holds S[e] + 16 in [1, 31] per byte without a carry between bytes.
-__device__ __forceinline__ void pf_build_xtab4(uint64_t *xtab, int bits, bool biased, int tid, int nthreads) {
+//   [256, 512)  PB 4 only, planes 2, 3: +-w2 at byte j2 plus +-w3 at byte j3
+// w_b = 2*alpha_b from plane_weight_regs: W2 {1, 2}, W4 {1, 2, 4, 8}, W3 {1, 2, 4, 0} (its padded fourth plane is code 0 and must
+// add nothing).  biased == false: signed bytes; W2: one entry is S[e], PB 4: one entry of each half added byte-wise (__vadd4) is
+// S[e].  biased == true (PB 4): the bytes of the two halves carry +3 and +13 (|w0| + |w1| <= 3, |w2| + |w3| <= 12), so every byte
+// is non-negative and a plain 32-bit add of one entry of each half holds S[e] + 16 in [1, 31] per byte without a carry between bytes.
+template <int PB>
+__device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool biased, int tid, int nthreads) {
     uint32_t wtx, wty;
     plane_weight_regs(bits, true, &wtx, &wty);
-    for (int e = tid; e < 512; e += nthreads) {
+    for (int e = tid; e < 128 * PB; e += nthreads) {
         const int h = e >> 8, wa = (int)((wtx >> (16 * h)) & 0xff), wb = (int)((wtx >> (16 * h + 8)) & 0xff);
         const int bias = biased ? (h ? 13 : 3) : 0;
         const int ja = e & 7, jb = (e >> 4) & 7, va = (e & 8) ? -wa : wa, vb = (e & 0x80) ? -wb : wb;
@@ -137,6 +144,49 @@ __device__ __forceinline__ void pf_build_xtab4(uint64_t *xtab, int bits, bool bi
         xtab[e] = x;
     }
 }
+
+// The producer warpgroup of both tiles.  These two are macros: written as inline functions (or a struct and a template that
+// takes the expansion as a lambda) the same code is ordered differently by the compiler, and the fp16 tile's consumers spill more.
+//
+// PF_PRODUCER_ROW declares the row of producer thread r < 128 (weight row r of the 128-row tile).  PB 2: the tile is one
+// super-block, stream lane wl = r / 4, row-in-lane wi = r % 4 (RW = 4).  PB 4: super-block sb = r / 64 of the tile, lane
+// wl = (r % 64) / 2, row-in-lane wi = r % 2 (RW = 2).
+#define PF_PRODUCER_ROW(PB, r_)                                                                                              \
+    const int r = (r_), sb = (PB) == 4 ? r >> 6 : 0, wl = (PB) == 4 ? (r & 63) >> 1 : r >> 2, wi = (PB) == 4 ? r & 1 : r & 3
+
+// PF_STAGE_BLOCKS runs the expansion (the variadic argument) once per chunk c of [c_first, c_last], with blk = the thread's
+// super-block's block of chunk c in shared memory (codes, then the scales at kPfScaleOff).  The blocks come from rsb_base (the row
+// tile's first super-block) and sb_base (super-block sb) through raw, a double buffer [2][NSB][rawsz] with chunk c in half c & 1:
+// cp.async fetches chunk c + 1 while chunk c is expanded.  The 128 / NSB threads of a super-block stage its blocks; a super-block
+// that is not live stages nothing.  Named barrier 1 (the 128 producer threads) makes block c visible to every producer and retires
+// block c - 1, whose half then takes chunk c + 1.  The block of c_last may still be read when the loop ends: a producer that stages
+// another run passes barrier 1 before it.  Besides PF_PRODUCER_ROW's names it reads p, live, rsb_base, sb_base, raw, rawsz and NSB
+// of the kernel.
+#define PF_STAGE_BLOCKS(PB, c, blk, c_first, c_last, ...)                                                                    \
+    do {                                                                                                                     \
+        const int pf_c0 = (c_first), pf_c1 = (c_last), n16 = p.blk_bytes >> 4;                                             \
+        auto load_blocks = [&](int c_, unsigned char *dst) {   /* chunk c_ of the tile's super-block(s) -> dst [NSB][rawsz] */ \
+            if constexpr ((PB) == 2) {                                                                                       \
+                for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c_ * p.blk_bytes + i * 16); \
+            } else if (live) {                                                                                               \
+                for (int i = r & 63; i < n16; i += 64)                                                                       \
+                    cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c_ * p.blk_bytes + i * 16);        \
+            }                                                                                                                \
+        };                                                                                                                   \
+        load_blocks(pf_c0, raw + (size_t)(pf_c0 & 1) * NSB * rawsz);                                                        \
+        cp_async_commit();                                                                                                   \
+        for (int c = pf_c0; c <= pf_c1; ++c) {                                                                               \
+            unsigned char *rb = raw + (size_t)(c & 1) * NSB * rawsz;                                                         \
+            cp_async_wait_all();                                                                                             \
+            asm volatile("bar.sync 1, 128;" ::: "memory");             /* block c visible to all producers; block c-1 dead */ \
+            if (c + 1 <= pf_c1) {                                                                                            \
+                load_blocks(c + 1, raw + (size_t)((c + 1) & 1) * NSB * rawsz);                                               \
+                cp_async_commit();                                                                                           \
+            }                                                                                                                \
+            const unsigned char *blk = rb + (size_t)sb * rawsz;                                                              \
+            __VA_ARGS__                                                                                                      \
+        }                                                                                                                    \
+    } while (0)
 
 // grid = (row tiles of 128 rows, ceil(N / 128)), block = 384 threads, 1 CTA per SM.
 //   warps 0..7  : consumers, warpgroup wg = rows 64*wg .. 64*wg+63 of the tile (wgmma accumulator layout)
@@ -153,8 +203,8 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
     unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][kPfRec] B tile + lut scales + lut bias pairs
     unsigned char *raw = sR + kPfStages * kPfRec;                          // [2][NSB][blk_bytes] packed blocks (codes + scales)
     const int rawsz = (p.blk_bytes + 127) & ~127;
-    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // [256] (PB 2) / [512] (PB 4) expansion table
-    uint64_t *bars = xtab + (PB == 4 ? 512 : 256);
+    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // [128 * PB] expansion table
+    uint64_t *bars = xtab + 128 * PB;
     uint64_t *full = bars, *empty = bars + kPfStages;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -162,19 +212,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
     const int ntok = min(kPfNT, p.N - n0);
     const int nag = p.K / 64;
 
-    if constexpr (PB == 2) {
-        for (int e = tid; e < 256; e += kPfThreads2) {
-            // index byte: low nibble = plane 0 (neg<<3 | j), high nibble = plane 1; value = +-1 at byte j0, +-2 at byte j1
-            int v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            v[e & 7] += (e & 8) ? -1 : 1;
-            v[(e >> 4) & 7] += (e & 0x80) ? -2 : 2;
-            uint64_t x = 0;
-            for (int i = 0; i < 8; ++i) x |= (uint64_t)(uint8_t)(int8_t)v[i] << (8 * i);
-            xtab[e] = x;
-        }
-    } else {
-        pf_build_xtab4(xtab, p.bits, false, tid, kPfThreads2);
-    }
+    pf_build_xtab<PB>(xtab, p.bits, false, tid, kPfThreads2);
     if (tid == 0) {
         for (int i = 0; i < kPfStages; ++i) { mbar_init(full + i, kPfProdWarps + 1); mbar_init(empty + i, kPfConsWarps); }
         mbar_fence_init();
@@ -185,35 +223,13 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
 
     if (warp >= kPfConsWarps) {
         // ======================= producers: thread = weight row of the tile =======================
-        const int r = tid - kPfConsWarps * 32;
-        // PB 2: lane / row-in-lane of the stream layout (RW = 4).  PB 4: super-block sb of the tile, lane, row-in-lane (RW = 2);
-        // the 64 threads of a super-block load its blocks.
-        const int sb = PB == 4 ? r >> 6 : 0;
-        const int wl = PB == 4 ? (r & 63) >> 1 : r >> 2, wi = PB == 4 ? r & 1 : r & 3;
+        PF_PRODUCER_ROW(PB, tid - kPfConsWarps * 32);
         const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
-        const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
-        const int n16 = p.blk_bytes >> 4;
         const unsigned char *rec_src = p.lut_tiles + (size_t)tile * nag * kPfRec;
-        auto load_blocks = [&](int c, unsigned char *dst) {   // chunk c of the tile's super-block(s) -> dst [NSB][rawsz]
-            if constexpr (PB == 2) {
-                for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c * p.blk_bytes + i * 16);
-            } else if (live) {
-                for (int i = r & 63; i < n16; i += 64) cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c * p.blk_bytes + i * 16);
-            }
-        };
-        load_blocks(0, raw);
-        cp_async_commit();
-        for (int c = 0; c < p.nchunk; ++c) {
-            unsigned char *rb = raw + (size_t)(c & 1) * NSB * rawsz;
-            cp_async_wait_all();
-            asm volatile("bar.sync 1, 128;" ::: "memory");                 // block c visible to all producers; block c-1 dead
-            if (c + 1 < p.nchunk) {
-                load_blocks(c + 1, raw + (size_t)((c + 1) & 1) * NSB * rawsz);
-                cp_async_commit();
-            }
-            const uint32_t *words = reinterpret_cast<const uint32_t *>(rb + (size_t)sb * rawsz);
-#pragma unroll 1
-            for (int h = 0; h < 2; ++h) {
+        const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
+        PF_STAGE_BLOCKS(PB, c, blk, 0, p.nchunk - 1, {
+            const uint32_t *words = reinterpret_cast<const uint32_t *>(blk);
+            _Pragma("unroll 1") for (int h = 0; h < 2; ++h) {
                 const int step = 2 * c + h, s = step % kPfStages;
                 if (r == 0) PF_TRACE(0, step, 0);
                 mbar_wait_parity(empty + s, ((step / kPfStages) & 1) ^ 1);     // stage released by the consumers of step - S
@@ -222,23 +238,18 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                     bulk_load(sR + (size_t)s * kPfRec, rec_src + (size_t)step * kPfRec, kPfRec, full + s);
                 }
                 unsigned char *a_dst = sA + (size_t)s * kPfStageBytes;
-#pragma unroll
-                for (int kc = 0; kc < 8; ++kc) {
+                _Pragma("unroll") for (int kc = 0; kc < 8; ++kc) {
                     uint64_t v2[2];
-#pragma unroll
-                    for (int u = 0; u < 2; ++u) {
+                    _Pragma("unroll") for (int u = 0; u < 2; ++u) {
                         const int gq = h * 16 + kc * 2 + u;                // group within the chunk (0..31)
                         const int q = gq >> 2, k = gq & 3;
-                        const uint32_t *w4 = words + ((size_t)q * 32 + wl) * 4;
+                        const uint32_t cw = row_codes<PB>(words + ((size_t)q * 32 + wl) * 4, k, wi);
                         if constexpr (PB == 2) {
-                            const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;
-                            const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;
-                            v2[u] = xtab[jb | (ng << 3)];
+                            v2[u] = xtab[cw];
                         } else {
-                            // nibble 4*wi + b of word k = full code of plane b: planes (0, 1) and (2, 3) index the two table halves,
-                            // added byte-wise (|S| <= 15: no byte overflows, no borrow crosses into the next entry)
-                            const uint32_t cw = w4[k] >> (16 * wi);
-                            const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + ((cw >> 8) & 0xffu)];
+                            // planes (0, 1) and (2, 3) index the two table halves, added byte-wise (|S| <= 15: no byte overflows,
+                            // no borrow crosses into the next entry)
+                            const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + (cw >> 8)];
                             const uint32_t s0 = __vadd4((uint32_t)lo, (uint32_t)hi), s1 = __vadd4((uint32_t)(lo >> 32), (uint32_t)(hi >> 32));
                             v2[u] = live ? ((uint64_t)s1 << 32 | s0) : 0ull;
                         }
@@ -252,7 +263,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                 if (lane == 0) mbar_arrive(full + s);
                 __syncwarp();
             }
-        }
+        });
     } else {
         // ======================= consumers: wgmma accumulator fragment of warpgroup wg =======================
         // register j = 4*c8 + 2*h + e holds row 64*wg + 16*(warp%4) + lane/4 + 8*h, token 8*c8 + 2*(lane%4) + e
@@ -267,10 +278,10 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
         const unsigned char *wg_base = rsb_base + (size_t)(PB == 4 ? wg : 0) * p.rsb_stride;
         const bool live = PB == 2 || rt * NSB + wg < p.nrsb;
         auto ld_s = [&](int c, int r) {
-            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + 4096, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + kPfScaleOff, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
         };
         auto ld_z = [&](int c, int r) {
-            return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + 4096 + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+            return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + kPfScaleOff + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
         };
         float hs[2], zz[2], hs_n[2], zz_n[2];
 #pragma unroll

@@ -17,7 +17,9 @@
 //   warpgroup  2    : producers (thread = weight row, the step's 16 K-groups): plane codes -> 8 fp16 entries fp16(k * hs), one 16-byte
 //                     store per group into the K-major canonical A tile; thread 0 also issues the step's 64 KB B tile as one bulk copy (TMA).
 // Supported: W2 (PB 2) and W3/W4 (PB 4: a 128-row tile is two 64-row super-blocks), chunk 128, act group 64, per-row scales
-// (+ zero points), symmetric LUT -- as the int8 tile.
+// (+ zero points), symmetric LUT -- as the int8 tile.  The producers take their row, block staging, code decode, PB 4 table and
+// scale offset from the int8 tile's shared code (tmac_prefill.cuh: PF_PRODUCER_ROW, PF_STAGE_BLOCKS, row_codes, pf_build_xtab,
+// kPfScaleOff); the expansion into fp16 A entries is this tile's own.  Each stream-K fragment is staged as one run.
 #pragma once
 #include "tmac_prefill.cuh"
 
@@ -130,7 +132,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
     unsigned char *sB = sA + kP16NA * kP16SubA;                            // [NB][64 KB]
     unsigned char *raw = sB + kP16NB * kP16SubB;                           // [2][NSB][blk] packed blocks (codes + scales)
     const int rawsz = (p.blk_bytes + 127) & ~127;
-    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // PB 4: [512] expansion table (pf_build_xtab4, biased)
+    uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // PB 4: [512] expansion table (pf_build_xtab, biased)
     uint64_t *bars = xtab + (PB == 4 ? 512 : 0);
     uint64_t *full = bars, *empty = full + kP16NA;
 
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
         x = fs1[0]; fs1[0] = fs1[1]; fs1[1] = x;
     }
 
-    if constexpr (PB == 4) pf_build_xtab4(xtab, p.bits, true, tid, kP16Threads);
+    if constexpr (PB == 4) pf_build_xtab<4>(xtab, p.bits, true, tid, kP16Threads);
     if (tid == 0) {
         for (int i = 0; i < kP16NA; ++i) { mbar_init(full + i, kP16ProdWarps + 1); mbar_init(empty + i, kP16ConsWarps); }
         mbar_fence_init();
@@ -162,13 +164,8 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
     if (warp >= kP16ConsWarps) {
         // ======================= producers: thread = weight row, all 16 K-groups of the step =======================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");           // registers go to the consumers' accumulators
-        const int r = tid - kP16ConsWarps * 32;
-        // PB 2: lane / row-in-lane of the stream layout (RW = 4).  PB 4: super-block sb of the tile, lane, row-in-lane (RW = 2);
-        // the 64 threads of a super-block load its blocks.
-        const int sb = PB == 4 ? r >> 6 : 0;
-        const int wl = PB == 4 ? (r & 63) >> 1 : r >> 2, wi = PB == 4 ? r & 1 : r & 3;
+        PF_PRODUCER_ROW(PB, tid - kP16ConsWarps * 32);
         const int srow = wl * (8 / PB) + wi;         // row within the super-block = scale index
-        const int n16 = p.blk_bytes >> 4;
         int it = 0;                                  // running step counter over both fragments
         auto stage_in = [&](int f, int u) {          // wait for a free stage, request its B tile; returns the A tile
             const int s = it % kP16NA;
@@ -192,50 +189,29 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
             const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
             const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
             const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
-            auto load_blocks = [&](int c, unsigned char *dst) {   // chunk c of the tile's super-block(s) -> dst [NSB][rawsz]
-                if constexpr (PB == 2) {
-                    for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c * p.blk_bytes + i * 16);
-                } else if (live) {
-                    for (int i = r & 63; i < n16; i += 64) cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c * p.blk_bytes + i * 16);
-                }
-            };
             const int s0 = fs0[f], s1m = min(fs1[f], p.nmain);
             if (s0 < s1m) {
                 const int c_first = s0 >> 1, c_last = (s1m - 1) >> 1;
                 asm volatile("bar.sync 1, 128;" ::: "memory");             // the previous fragment's last block is dead
-                load_blocks(c_first, raw + (size_t)(c_first & 1) * NSB * rawsz);
-                cp_async_commit();
-                for (int c = c_first; c <= c_last; ++c) {
-                    unsigned char *rb = raw + (size_t)(c & 1) * NSB * rawsz;
-                    cp_async_wait_all();
-                    asm volatile("bar.sync 1, 128;" ::: "memory");         // block c visible to all producers; block c-1 dead
-                    if (c + 1 <= c_last) {
-                        load_blocks(c + 1, raw + (size_t)((c + 1) & 1) * NSB * rawsz);
-                        cp_async_commit();
-                    }
-                    const uint32_t *words = reinterpret_cast<const uint32_t *>(rb + (size_t)sb * rawsz);
+                PF_STAGE_BLOCKS(PB, c, blk, c_first, c_last, {
+                    const uint32_t *words = reinterpret_cast<const uint32_t *>(blk);
                     // hs = fp16(0.5 * scale).  PB 2: the row's 8 A entries of one K-group are +-hs at entry j0 (plane 0) plus +-2hs at
                     // entry j1 (plane 1), built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the exact k * hs.
-                    const __half hsh = __float2half_rn(live ? 0.5f * load_scale(rb + (size_t)sb * rawsz + 4096, p.sd, srow) : 0.f);
+                    const __half hsh = __float2half_rn(live ? 0.5f * load_scale(blk + kPfScaleOff, p.sd, srow) : 0.f);
                     const uint32_t c1 = __half_as_ushort(hsh), c2 = __half_as_ushort(__hadd(hsh, hsh));
                     const int u0 = (c == c_first) ? (s0 & 1) : 0, u1 = (c == c_last) ? ((s1m - 1) & 1) : 1;   // steps of this chunk
-#pragma unroll 1
-                    for (int u = u0; u <= u1; ++u) {
+                    _Pragma("unroll 1") for (int u = u0; u <= u1; ++u) {
                         unsigned char *a_dst = stage_in(f, 2 * c + u);
-#pragma unroll
-                        for (int gl = 0; gl < 16; ++gl) {                      // group within the step = 16-byte chunk index
+                        _Pragma("unroll") for (int gl = 0; gl < 16; ++gl) {    // group within the step = 16-byte chunk index
                             const int gqc = u * 16 + gl;                       // group within the chunk (0..31)
                             const int q = gqc >> 2, k = gqc & 3;
-                            const uint32_t *w4 = words + ((size_t)q * 32 + wl) * 4;
+                            const uint32_t cw = row_codes<PB>(words + ((size_t)q * 32 + wl) * 4, k, wi);
                             uint32_t o4[4];
                             if constexpr (PB == 2) {
-                                const uint32_t jb = (w4[k] >> (8 * wi)) & 0x77u;                                   // j0 | j1 << 4
-                                const uint32_t ng = (w4[2 * (k >> 1) + (wi >> 1)] >> (16 * (wi & 1) + 8 * (k & 1) + 3)) & 0x11u;   // neg0 | neg1 << 4
-                                const uint32_t j0 = jb & 7u, j1 = jb >> 4;
-                                const uint32_t v0 = (c1 ^ ((ng & 1u) << 15)) << ((j0 & 1u) * 16), v1 = (c2 ^ ((ng & 0x10u) << 11)) << ((j1 & 1u) * 16);
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    const uint32_t a = (j0 >> 1) == (uint32_t)e ? v0 : 0u, b = (j1 >> 1) == (uint32_t)e ? v1 : 0u;
+                                // cw = j0 | neg0 << 3 | j1 << 4 | neg1 << 7
+                                const uint32_t v0 = (c1 ^ ((cw & 8u) << 12)) << ((cw & 1u) * 16), v1 = (c2 ^ ((cw & 0x80u) << 8)) << (((cw >> 4) & 1u) * 16);
+                                _Pragma("unroll") for (int e = 0; e < 4; ++e) {
+                                    const uint32_t a = (cw & 6u) == 2u * e ? v0 : 0u, b = (cw & 0x60u) == 32u * e ? v1 : 0u;
                                     const __half2 x = __hadd2(*reinterpret_cast<const __half2 *>(&a), *reinterpret_cast<const __half2 *>(&b));
                                     o4[e] = *reinterpret_cast<const uint32_t *>(&x);
                                 }
@@ -243,12 +219,10 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                                 // PB 4: the integer k = S[e] (|S| <= 15) of the row's four planes from the two biased table halves: the plain
                                 // 32-bit add holds k + 16 in [1, 31] per byte.  fp16 bits 0x6400 | m are 1024 + m, minus 1040 is
                                 // k exactly; k and hs are exact fp16 values, so the HMUL2 rounds the exact product k * hs once.
-                                const uint32_t cw = w4[k] >> (16 * wi);
-                                const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + ((cw >> 8) & 0xffu)];
+                                const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + (cw >> 8)];
                                 const uint32_t sk[2] = {(uint32_t)lo + (uint32_t)hi, (uint32_t)(lo >> 32) + (uint32_t)(hi >> 32)};
                                 const __half2 hs2 = __halves2half2(hsh, hsh), off = __float2half2_rn(1040.f);
-#pragma unroll
-                                for (int e = 0; e < 4; ++e) {
+                                _Pragma("unroll") for (int e = 0; e < 4; ++e) {
                                     const uint32_t m = __byte_perm(sk[e >> 1], 0x64u, (e & 1) ? 0x4342u : 0x4140u);   // entries 2e, 2e + 1
                                     const __half2 kk = __hsub2(*reinterpret_cast<const __half2 *>(&m), off);
                                     const __half2 x = __hmul2(kk, hs2);
@@ -259,7 +233,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                         }
                         stage_out();
                     }
-                }
+                });
             }
             // bias steps: A columns 4*wg + {0,1,2,3} = {0.5s, 0.5s, z, z} of weight group wg (= chunk index), 2 groups per 16-byte chunk
             for (int step = max(fs0[f], p.nmain); step < fs1[f]; ++step) {
@@ -273,7 +247,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                         const int wg = e * 32 + kc * 2 + u;
                         float hs = 0.f, zz = 0.f;
                         if (live && wg < p.nchunk) {
-                            const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + 4096;
+                            const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + kPfScaleOff;
                             hs = 0.5f * load_scale(sp, p.sd, srow);
                             if (p.zp) zz = load_scale(sp + (size_t)RSB * p.sd, p.sd, srow);
                         }
