@@ -177,6 +177,12 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
         const int nchunk = o.nchunk, bpw = o.bpw, zp = o.zp, sd = o.sd, one_scale = o.one_scale;
         const float scale0 = o.scale0;
         const float *x = o.x;
+        // read once per op, before the waits: every asm volatile below (polls, mbarrier waits, barriers) would otherwise force a
+        // reload of the ChainOp field right where the waited-for data has arrived
+        const uint2 *const ll_in = o.ll_in;
+        uint2 *const ll_out = o.ll_out;
+        void *const C = o.C;
+        const int Mout = o.Mout, out_f16 = o.out_f16, npeer = o.npeer;
         const bool active = rsb < o.nrsb;
         const int c_first = c_slot * bpw, c_end = min(nchunk, c_first + bpw);
         const uint32_t ep_in = epoch0 * (uint32_t)p.nops + (uint32_t)o.in_op + 1u, ep_out = epoch0 * (uint32_t)p.nops + (uint32_t)op + 1u;
@@ -202,8 +208,8 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
             for (int c = c_first; c < c_end; ++c) {
                 // ---- LUT slice of this chunk -> warp-private table (lane = group) ----
                 float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
-                if (flow && o.ll_in) {                             // the producer's rows, as soon as they exist
-                    chain_wait_x(o.ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, b0, b1, b2, b3);
+                if (flow && ll_in) {                               // the producer's rows, as soon as they exist
+                    chain_wait_x(ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, b0, b1, b2, b3);
                     if (lane >= NG) b0 = b1 = b2 = b3 = 0.f;
                 } else if (lane < NG) {
                     const float4 f = __ldcg(reinterpret_cast<const float4 *>(x + ((size_t)c * NG + lane) * 4));   // L2: written by other SMs
@@ -258,11 +264,11 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
 #pragma unroll
                         for (int k2 = 0; k2 < CS; ++k2) fsum += cl[(size_t)k2 * RSB + t];
                         const int row = rsb * RSB + t;
-                        if (row < o.Mout) {
-                            seq_publish(o.ll_out + row, __float_as_uint(fsum), ep_out);
-                            store_out(o.C, row, fsum, o.out_f16);
-                            for (int q = 0; q < o.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
-                                store_out(o.Cpeer[q], row, fsum, o.out_f16);
+                        if (row < Mout) {
+                            seq_publish(ll_out + row, __float_as_uint(fsum), ep_out);
+                            store_out(C, row, fsum, out_f16);
+                            for (int q = 0; q < npeer; ++q)          // the all-gather, fused into the epilogue: one store per peer and row
+                                store_out(o.Cpeer[q], row, fsum, out_f16);
                         }
                     }
                     if (tr) tr[8] = globaltimer_ns();
@@ -285,9 +291,9 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
 #pragma unroll
                         for (int k2 = 0; k2 < CS; ++k2) fsum += cl[(size_t)k2 * RSB + t];
                         const int row = rsb * RSB + t;
-                        if (row < o.Mout) {
-                            store_out(o.C, row, fsum, o.out_f16);
-                            for (int q = 0; q < o.npeer; ++q) store_out(o.Cpeer[q], row, fsum, o.out_f16);
+                        if (row < Mout) {
+                            store_out(C, row, fsum, out_f16);
+                            for (int q = 0; q < npeer; ++q) store_out(o.Cpeer[q], row, fsum, out_f16);
                         }
                     }
                 __syncthreads();                                   // the release below is cumulative over the CTA's stores
