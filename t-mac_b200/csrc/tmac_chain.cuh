@@ -21,13 +21,14 @@
 // bench.py times it on the bench chain (32 x 11008x4096 W2, x[i+1] = first K outputs of op i) beside the launch chain and
 // tmac_seq.cuh; flags bit 0 selects the grid-barrier form this kernel started as, kept for comparison.  Per-phase stamps
 // (ChainParams::trace) are read by tools/seq_bench.py --trace.
-// The LUT slices are built by lut_slice and the blocks run by TMAC_BLOCK_LOOKUPS / TMAC_BLOCK_SCALES (tmac_kernels.cuh), the
-// code gemv3's fused path runs, so LUT bytes, scales and biases are identical to the preprocessor's and a block's fp32
-// operation order is gemv3's; fp32 sums in fixed (warp, then cluster rank) order; the K split differs from the lone launch's,
-// so results equal tmac_b200_gemv's up to fp32 re-association.  Waits are bounded (error flag, mbar_wait_bounded).
+// The LUT slices are built by lut_slice, the code gemv3's fused path runs, and the blocks by TMAC_BLOCK_LOOKUPS /
+// TMAC_BLOCK_SCALES (tmac_kernels.cuh), gemv3's block step, so LUT bytes, scales and biases are identical
+// to the preprocessor's and a block's fp32 operation order is gemv3's; fp32 sums in fixed (warp, then cluster rank) order;
+// the K split differs from the lone launch's, so results equal tmac_b200_gemv's up to fp32 re-association.  Waits are
+// bounded (error flag): mbar_wait_bounded, and wait_words of tmac_seq.cuh for the producer's {value, epoch} words.
 #pragma once
 #include "tmac_kernels.cuh"
-#include "tmac_seq.cuh"     // {value, epoch} words: seq_publish
+#include "tmac_seq.cuh"     // {value, epoch} words: seq_publish, wait_words
 
 namespace tmac_b200 {
 
@@ -72,32 +73,6 @@ __device__ __forceinline__ void st_async_f32(float *local_ptr, uint64_t *local_b
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(local_ptr)), "r"(rank));
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(smem_u32(local_bar)), "r"(rank));
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(__float_as_uint(v)), "r"(rb) : "memory");
-}
-// Four consecutive {value, epoch} words (32 bytes) per active lane.  Every lane loads its words once; if some are stale, the lowest
-// stale lane alone polls its first word (the rest of the warp would only add L2 traffic), then the stale lanes reload both
-// 16-byte halves together: data that is already there costs one L2 round trip, data that arrives while waiting two.
-__device__ __forceinline__ void chain_wait_x(const uint2 *src, bool active, uint32_t epoch, int *err, float &b0, float &b1, float &b2, float &b3) {
-    uint4 v0 = make_uint4(0u, epoch, 0u, epoch), v1 = v0;
-    auto load = [&]() {
-        asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v0.x), "=r"(v0.y), "=r"(v0.z), "=r"(v0.w) : "l"(src) : "memory");
-        asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v1.x), "=r"(v1.y), "=r"(v1.z), "=r"(v1.w) : "l"(src + 2) : "memory");
-    };
-    if (active) load();
-    int spins = 0;
-    for (;;) {
-        const bool stale = active && (v0.y != epoch || v0.w != epoch || v1.y != epoch || v1.w != epoch);
-        const unsigned m = __ballot_sync(0xffffffffu, stale);
-        if (m == 0) break;
-        const int leader = __ffs(m) - 1;
-        if ((int)(threadIdx.x & 31) == leader) {
-            uint32_t e;
-            do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(e) : "l"(reinterpret_cast<const uint32_t *>(src) + 1) : "memory"); } while (e != epoch && ++spins < kChainSpin);
-        }
-        spins = __shfl_sync(0xffffffffu, spins, leader);
-        if (spins >= kChainSpin) { if ((threadIdx.x & 31) == 0) atomicExch(err, 5); v0.x = v0.z = v1.x = v1.z = 0u; break; }
-        if (stale) load();
-    }
-    b0 = __uint_as_float(v0.x); b1 = __uint_as_float(v0.z); b2 = __uint_as_float(v1.x); b3 = __uint_as_float(v1.z);
 }
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned *p) { unsigned v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 
@@ -209,7 +184,7 @@ __global__ void __launch_bounds__(kChainWarps * 32, 5) chain_kernel(const ChainP
                 // ---- LUT slice of this chunk -> warp-private table (lane = group) ----
                 float b0 = 0.f, b1 = 0.f, b2 = 0.f, b3 = 0.f;
                 if (flow && ll_in) {                               // the producer's rows, as soon as they exist
-                    chain_wait_x(ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, b0, b1, b2, b3);
+                    wait_words<kChainSpin>(ll_in + ((size_t)c * NG + lane) * 4, lane < NG, ep_in, p.err, 5, b0, b1, b2, b3);
                     if (lane >= NG) b0 = b1 = b2 = b3 = 0.f;
                 } else if (lane < NG) {
                     const float4 f = __ldcg(reinterpret_cast<const float4 *>(x + ((size_t)c * NG + lane) * 4));   // L2: written by other SMs

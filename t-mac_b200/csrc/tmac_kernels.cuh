@@ -19,7 +19,8 @@
 // Shared by every kernel of the project (all headers include this one):
 //   the activation LUT   : lut_abs_sum, lut_scale, lut_ts, lut_odd_entries, lut_q8, lut_stored, lut_addv8, lut_group, lut_bias,
 //                          lut_slice (one chunk's slice in a warp);
-//   the block step       : TMAC_BLOCK_LOOKUPS, TMAC_BLOCK_SCALES (gemv3_kernel and chain_kernel);
+//   the block step       : TMAC_QUAD_LOOKUP, TMAC_GROUP_FOLD (gemv3_kernel, chain_kernel, seq_kernel), TMAC_BLOCK_LOOKUPS
+//                          (written with those two), TMAC_BLOCK_SCALES (gemv3_kernel and chain_kernel);
 //   PTX wrappers         : smem_u32, mbar_init, mbar_fence_init, fence_proxy_async, mbar_arrive, expect_tx, bulk_load,
 //                          mbar_wait_parity, mbar_wait_bounded<LIMIT>, cluster_arrive_relaxed / cluster_wait, globaltimer_ns;
 //   the output store     : store_out (fp16 or fp32).
@@ -307,40 +308,50 @@ __device__ __forceinline__ float lut_slice(float x0, float x1, float x2, float x
 }
 
 // ------------------------------------------------------------------------------------------
-// The arithmetic of one (row super-block, K chunk) block, shared by gemv3_kernel and chain_kernel: the fp32 operation order
-// decides the result, so both run this one code.  The block is the stream layout (tmac_layout.h): QCH quads of 32 lanes x 16
-// code bytes, then RSB weight scales and (zp) RSB zero points of sd bytes each; tab is the warp's LUT slice of the chunk.
-// These two are macros, not functions: the compiler simplifies a callee before it inlines it, and as __forceinline__ functions
-// the step changed the kernels' SASS (gemv3_kernel<2,true,8,4,3,true> 1752 -> 1768 instructions, chain_kernel<2,8,4> another
-// shared-memory load mix).  Expanded in place they compile to the instructions of the code they replaced.
+// The arithmetic of one (row super-block, K chunk) block, shared by gemv3_kernel and chain_kernel, whose lookups seq_kernel runs
+// too: the fp32 operation order decides the result, so they run this one code.  The block is the stream layout (tmac_layout.h):
+// QCH quads of 32 lanes x 16 code bytes, then RSB weight scales and (zp) RSB zero points of sd bytes each; tab is the warp's LUT
+// slice of the chunk.  These are macros, not functions: the compiler simplifies a callee before it inlines it, and as
+// __forceinline__ functions the step changed the kernels' SASS (gemv3_kernel<2,true,8,4,3,true> 1752 -> 1768 instructions,
+// chain_kernel<2,8,4> another shared-memory load mix).  Expanded in place they compile to the instructions of the code they
+// replaced.
 // ------------------------------------------------------------------------------------------
+// TMAC_QUAD_LOOKUP: quad q of the block -- the lane's code word at wp[q * 32] (wp = the block's first uint4 + lane), the quad's
+// table entries -- through Quad<PB, SYM> into iacc.
+#define TMAC_QUAD_LOOKUP(PB, SYM, wp, tab, q, wtx, wty, iacc)                                                                     \
+    do {                                                                                                                          \
+        const uint4 wq_ = (wp)[(q) * 32];                                                                                         \
+        uint32_t t_[(SYM) ? 8 : 16];                                                                                              \
+        if (SYM) {                                                                                                                \
+            const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[2 * (q)], b_ = reinterpret_cast<const uint4 *>(tab)[2 * (q) + 1]; \
+            t_[0] = a_.x; t_[1] = a_.y; t_[2] = a_.z; t_[3] = a_.w; t_[4] = b_.x; t_[5] = b_.y; t_[6] = b_.z; t_[7] = b_.w;        \
+        } else {                                                                                                                  \
+            _Pragma("unroll") for (int k_ = 0; k_ < 4; ++k_) {                                                                    \
+                const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[4 * (q) + k_];                                              \
+                t_[4 * k_] = a_.x; t_[4 * k_ + 1] = a_.y; t_[4 * k_ + 2] = a_.z; t_[4 * k_ + 3] = a_.w;                           \
+            }                                                                                                                     \
+        }                                                                                                                         \
+        Quad<PB, SYM>::run(wq_, t_, (iacc), (wtx), (wty));                                                                        \
+    } while (0)
+// TMAC_GROUP_FOLD: the end of an activation group, facc[i] += ls * iacc[i] with the group's LUT scale ls; iacc is left at zero.
+#define TMAC_GROUP_FOLD(PB, ls, iacc, facc)                                                                                       \
+    do {                                                                                                                          \
+        _Pragma("unroll") for (int i_ = 0; i_ < 8 / (PB); ++i_) {                                                                 \
+            (facc)[i_] = fmaf((ls), (float)(iacc)[i_], (facc)[i_]);                                                               \
+            (iacc)[i_] = 0;                                                                                                       \
+        }                                                                                                                         \
+    } while (0)
 // TMAC_BLOCK_LOOKUPS: facc[i] = sum over the chunk's activation groups a of lsv[a] * (lane's row i lookups of a's AGQ quads),
 // Quad<PB, SYM> into iacc, which is left at zero.  AGQ == 0 (integer path, one activation group = the whole row): only iacc
 // accumulates.  Arguments are evaluated more than once.
 #define TMAC_BLOCK_LOOKUPS(PB, SYM, QCH, AGQ, stage, tab, lane, wtx, wty, lsv, iacc, facc)                                        \
     do {                                                                                                                          \
-        constexpr int RW_ = 8 / (PB), AQ_ = (AGQ) ? (AGQ) : 1;                                                                    \
+        constexpr int AQ_ = (AGQ) ? (AGQ) : 1;                                                                                    \
         const uint4 *wp_ = reinterpret_cast<const uint4 *>(stage) + (lane);                                                       \
-        _Pragma("unroll") for (int i_ = 0; i_ < RW_; ++i_) (facc)[i_] = 0.f;                                                      \
+        _Pragma("unroll") for (int i_ = 0; i_ < 8 / (PB); ++i_) (facc)[i_] = 0.f;                                                 \
         _Pragma("unroll") for (int q_ = 0; q_ < (QCH); ++q_) {                                                                    \
-            const uint4 wq_ = wp_[q_ * 32];                                                                                       \
-            uint32_t t_[(SYM) ? 8 : 16];                                                                                          \
-            if (SYM) {                                                                                                            \
-                const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[2 * q_], b_ = reinterpret_cast<const uint4 *>(tab)[2 * q_ + 1]; \
-                t_[0] = a_.x; t_[1] = a_.y; t_[2] = a_.z; t_[3] = a_.w; t_[4] = b_.x; t_[5] = b_.y; t_[6] = b_.z; t_[7] = b_.w;    \
-            } else {                                                                                                              \
-                _Pragma("unroll") for (int k_ = 0; k_ < 4; ++k_) {                                                                \
-                    const uint4 a_ = reinterpret_cast<const uint4 *>(tab)[4 * q_ + k_];                                           \
-                    t_[4 * k_] = a_.x; t_[4 * k_ + 1] = a_.y; t_[4 * k_ + 2] = a_.z; t_[4 * k_ + 3] = a_.w;                       \
-                }                                                                                                                 \
-            }                                                                                                                     \
-            Quad<PB, SYM>::run(wq_, t_, (iacc), (wtx), (wty));                                                                    \
-            if ((AGQ) && ((q_ + 1) % AQ_) == 0) {                                                                                 \
-                _Pragma("unroll") for (int i_ = 0; i_ < RW_; ++i_) {                                                              \
-                    (facc)[i_] = fmaf((lsv)[q_ / AQ_], (float)(iacc)[i_], (facc)[i_]);                                            \
-                    (iacc)[i_] = 0;                                                                                               \
-                }                                                                                                                 \
-            }                                                                                                                     \
+            TMAC_QUAD_LOOKUP(PB, SYM, wp_, tab, q_, wtx, wty, iacc);                                                              \
+            if ((AGQ) && ((q_ + 1) % AQ_) == 0) TMAC_GROUP_FOLD(PB, (lsv)[q_ / AQ_], iacc, facc);                                 \
         }                                                                                                                         \
     } while (0)
 // TMAC_BLOCK_SCALES: cacc[i] += 0.5*s * (facc[i] + lbsum) (+ z * lbsum) with the weight scale s (scale0 for one_scale tensors)

@@ -13,10 +13,10 @@
 //     ~2 GEMVs ahead of the arithmetic, across the data dependencies, because weights do not depend on activations;
 //   * 20 consumer warps per CTA do, per op: (A) build the LUT slices of the CTA's K chunks from the op's input
 //     vector (lut_group, lut_addv8 and lut_bias of tmac_kernels.cuh, the LUT functions preprocessor_kernel uses
-//     -> bit-identical tables), (B) the PRMT + DP4A lookups (Quad<>::run, as gemv3) over an arithmetic "stream-K"
-//     share of the op's blocks -- CTA c owns blocks [T*c/G, T*(c+1)/G), a warp owns a contiguous run of
-//     activation-group units inside them --, (C) reduce
-//     the warps through shared memory in fixed order and finish the rows;
+//     -> bit-identical tables), (B) the lookups of gemv3 and chain_kernel (TMAC_QUAD_LOOKUP and TMAC_GROUP_FOLD of
+//     tmac_kernels.cuh) over an arithmetic "stream-K" share of the op's blocks -- CTA c owns blocks
+//     [T*c/G, T*(c+1)/G), a warp owns a contiguous run of activation-group units inside them, so a warp's run can
+//     start and end inside a block --, (C) reduce the warps through shared memory in fixed order and finish the rows;
 //   * rows whose K range is split between CTAs are finished by the LAST CTA that touches them: the earlier ones
 //     publish their partial sums through 8-byte {value, epoch} slots in global memory (one store, one polling load
 //     per row; no fence, no atomic; ascending CTA order -> deterministic);
@@ -82,32 +82,39 @@ struct SeqParams {
 __device__ __forceinline__ void seq_publish(uint2 *slot, uint32_t bits, uint32_t epoch) {
     asm volatile("st.relaxed.gpu.global.v2.u32 [%0], {%1, %2};" ::"l"(slot), "r"(bits), "r"(epoch) : "memory");
 }
-// Waiting for {value, epoch} words.  Polling is WARP-cooperative: every lane loads its word once; while some are stale only the
-// lowest stale lane polls (one 32-byte sector per L2 round trip), then the stale lanes reload.  (All 640 threads of all CTAs
-// polling their own words costs ~5 KB of L2 bandwidth per cycle -- as much as the L2 can deliver -- and starves the very
-// stores they wait for.)  `active` lanes take part; all 32 lanes must call.
-template <int NWORDS>   // 2: one {value, epoch} word (8 bytes), 4: two adjacent words (16 bytes)
-__device__ __forceinline__ uint4 seq_wait(const void *slot, bool active, uint32_t epoch, int *err, int code) {
-    uint4 v = make_uint4(0u, epoch, 0u, epoch);
+// Waiting for N = 1, 2 or 4 consecutive {value, epoch} words at src per active lane; val = their values (0 in inactive lanes and
+// after LIMIT polls: error `code`), separate references because an array or a returned vector changes chain_kernel's SASS.  While
+// some are stale only the lowest stale lane polls the epoch of its first word (all 640 threads of all CTAs polling would take
+// ~5 KB of L2 bandwidth per cycle and starve the very stores they wait for), then the stale lanes reload all their words.  All
+// 32 lanes must call.
+template <int LIMIT, typename... F>
+__device__ __forceinline__ void wait_words(const uint2 *src, bool active, uint32_t epoch, int *err, int code, F &...val) {
+    constexpr int N = sizeof...(F);
+    static_assert(N == 1 || N == 2 || N == 4, "words per lane");
+    uint4 v0 = make_uint4(0u, epoch, 0u, epoch), v1 = v0;      // words 0, 1 | 2, 3 (absent words read as current)
     auto load = [&]() {
-        if (NWORDS == 2) asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(slot) : "memory");
-        else asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(slot) : "memory");
+        if constexpr (N == 1) asm volatile("ld.relaxed.gpu.global.v2.u32 {%0, %1}, [%2];" : "=r"(v0.x), "=r"(v0.y) : "l"(src) : "memory");
+        else asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v0.x), "=r"(v0.y), "=r"(v0.z), "=r"(v0.w) : "l"(src) : "memory");
+        if constexpr (N == 4) asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v1.x), "=r"(v1.y), "=r"(v1.z), "=r"(v1.w) : "l"(src + 2) : "memory");
     };
     if (active) load();
     int spins = 0;
     for (;;) {
-        const bool stale = active && (v.y != epoch || v.w != epoch);
+        const bool stale = active && (v0.y != epoch || v0.w != epoch || v1.y != epoch || v1.w != epoch);
         const unsigned m = __ballot_sync(0xffffffffu, stale);
         if (m == 0) break;
         const int leader = __ffs(m) - 1;
         if ((int)(threadIdx.x & 31) == leader) {
-            do { load(); } while ((v.y != epoch || v.w != epoch) && ++spins < kSeqSpinLimit);
+            uint32_t e;
+            do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(e) : "l"(reinterpret_cast<const uint32_t *>(src) + 1) : "memory"); } while (e != epoch && ++spins < LIMIT);
         }
         spins = __shfl_sync(0xffffffffu, spins, leader);
-        if (spins >= kSeqSpinLimit) { if ((threadIdx.x & 31) == 0) atomicExch(err, code); v.x = v.z = 0; break; }
-        if (stale && (int)(threadIdx.x & 31) != leader) load();
+        if (spins >= LIMIT) { if ((threadIdx.x & 31) == 0) atomicExch(err, code); v0.x = v0.z = v1.x = v1.z = 0u; break; }
+        if (stale) load();
     }
-    return v;
+    const float w[4] = {__uint_as_float(v0.x), __uint_as_float(v0.z), __uint_as_float(v1.x), __uint_as_float(v1.z)};
+    int i = 0;
+    ((val = w[i++]), ...);
 }
 __device__ __forceinline__ void seq_bar(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(kSeqWarps * 32) : "memory"); }
 __device__ __forceinline__ int ld_volatile_s32(const int *p) { int v; asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory"); return v; }
@@ -129,6 +136,26 @@ template <int N> __device__ __forceinline__ void load_half_vec(const unsigned ch
     for (int i = 0; i < N / 2; ++i) {
         const float2 f = __half22float2(*reinterpret_cast<const __half2 *>(&w[i]));
         out[2 * i] = f.x; out[2 * i + 1] = f.y;
+    }
+}
+
+// The LUT record of a K-group (lane = K-group, x0..x3 = its activations, WL lanes per activation group): the stored entries
+// lo | hi and the group's LUT scale; returns the group's LUT bias.  All 32 lanes must call it.
+template <int WL>
+__device__ __forceinline__ float lut_record(float x0, float x1, float x2, float x3, int lane, uint32_t &lo, uint32_t &hi, float &scale) {
+    return lut_bias<WL>(lut_addv8(lut_group<WL>(x0, x1, x2, x3, lo, hi, scale)), lane & ~(WL - 1));
+}
+// LUT hand-over: the record of K-group g of an op's output from its four rows x, published as {lo, epoch, hi, epoch} to
+// lut_out[g] and, by the activation group's first lane, {scale, epoch, bias, epoch} to ag_out[g / WL] (`valid` lanes only).
+// All 32 lanes must call it.
+template <int WL>
+__device__ __forceinline__ void publish_lut_record(float4 x, int lane, bool valid, size_t g, uint4 *lut_out, uint4 *ag_out, uint32_t epoch) {
+    uint32_t lo, hi;
+    float scale;
+    const float bias = lut_record<WL>(x.x, x.y, x.z, x.w, lane, lo, hi, scale);
+    if (valid) {
+        seq_publish16(lut_out + g, lo, hi, epoch);
+        if ((lane & (WL - 1)) == 0) seq_publish16(ag_out + g / WL, __float_as_uint(scale), __float_as_uint(bias), epoch);
     }
 }
 
@@ -255,13 +282,14 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                 int c = c0 + ci; if (c >= nchunk) c -= nchunk;
                 float *d = lsb + (size_t)ci * (2 * NAG);
                 if (li) {
-                    const uint4 r = seq_wait<4>(li + (size_t)c * NG + gl, valid, epoch, p.err, 5);
+                    float lo, hi, scale, bias;
+                    wait_words<kSeqSpinLimit>(reinterpret_cast<const uint2 *>(li + (size_t)c * NG + gl), valid, epoch, p.err, 5, lo, hi);
                     const bool first = valid && (gl % WL) == 0;
-                    const uint4 a = seq_wait<4>(ai + (size_t)c * NAG + gl / WL, first, epoch, p.err, 5);
-                    if (valid) reinterpret_cast<uint2 *>(tabs + (size_t)ci * TAB)[gl] = make_uint2(r.x, r.z);
+                    wait_words<kSeqSpinLimit>(reinterpret_cast<const uint2 *>(ai + (size_t)c * NAG + gl / WL), first, epoch, p.err, 5, scale, bias);
+                    if (valid) reinterpret_cast<uint2 *>(tabs + (size_t)ci * TAB)[gl] = make_uint2(__float_as_uint(lo), __float_as_uint(hi));
                     if (first) {
-                        d[gl / WL] = __uint_as_float(a.x);
-                        d[NAG + gl / WL] = __uint_as_float(a.z);
+                        d[gl / WL] = scale;
+                        d[NAG + gl / WL] = bias;
                     }
                     continue;
                 }
@@ -274,13 +302,12 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                             x0 = f.x; x1 = f.y; x2 = f.z; x3 = f.w;
                         }
                     } else {
-                        const uint4 v0 = seq_wait<4>(xl + k0, valid, epoch, p.err, 3), v1 = seq_wait<4>(xl + k0 + 2, valid, epoch, p.err, 3);
-                        x0 = __uint_as_float(v0.x); x1 = __uint_as_float(v0.z); x2 = __uint_as_float(v1.x); x3 = __uint_as_float(v1.z);
+                        wait_words<kSeqSpinLimit>(xl + k0, valid, epoch, p.err, 3, x0, x1, x2, x3);
                     }
                 }
                 uint32_t lo, hi;
                 float scale;
-                const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(x0, x1, x2, x3, lo, hi, scale)), lane & ~(WL - 1));
+                const float bias = lut_record<WL>(x0, x1, x2, x3, lane, lo, hi, scale);
                 if (valid) reinterpret_cast<uint2 *>(tabs + (size_t)ci * TAB)[gl] = make_uint2(lo, hi);
                 if (valid && (gl % WL) == 0) {
                     d[gl / WL] = scale;
@@ -346,22 +373,16 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                 float facc[RW];
 #pragma unroll
                 for (int i = 0; i < RW; ++i) facc[i] = 0.f;
-                float lbp = 0.f;
+                float lbp = 0.f;                                // LUT biases of the activation groups [a0, a1)
                 for (int a = a0; a < a1; ++a) {
 #pragma unroll
-                    for (int qq = 0; qq < AGQ; ++qq) {
-                        const int q = a * AGQ + qq;
-                        const uint4 wq = wp[q * 32];
-                        const uint4 ta = reinterpret_cast<const uint4 *>(tab)[2 * q], tb = reinterpret_cast<const uint4 *>(tab)[2 * q + 1];
-                        const uint32_t t[8] = {ta.x, ta.y, ta.z, ta.w, tb.x, tb.y, tb.z, tb.w};
-                        Quad<PB, true>::run(wq, t, iacc, wtx, wty);
-                    }
-                    const float lsv = ls[a];
-#pragma unroll
-                    for (int i = 0; i < RW; ++i) { facc[i] = fmaf(lsv, (float)iacc[i], facc[i]); iacc[i] = 0; }
+                    for (int qq = 0; qq < AGQ; ++qq) TMAC_QUAD_LOOKUP(PB, true, wp, tab, a * AGQ + qq, wtx, wty, iacc);
+                    TMAC_GROUP_FOLD(PB, ls[a], iacc, facc);
                     lbp += ls[NAG + a];
                 }
                 {
+                    // TMAC_BLOCK_SCALES's arithmetic with lbsum = lbp, but the fp16 scales read with one vector load per lane:
+                    // the macro's per-row load_scale made this kernel ~5% slower on the 32 x 11008x4096 W2 chain (H100 SXM, 700 W)
                     const unsigned char *sp = stage + (size_t)QCH * 512;
                     float sv[RW], zv[RW];
                     if (one_scale) {
@@ -422,8 +443,11 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
             }
             float fsum = 0.f;
             if (s == 0) {                                       // started in earlier CTAs: their partial sums, ascending K order
-                for (int k2 = fc; k2 < cta; ++k2)               // (RSB is a multiple of 32: the whole warp is in this branch)
-                    fsum += __uint_as_float(seq_wait<2>(xchg + (size_t)k2 * RSB + t, true, epoch, p.err, 2).x);
+                for (int k2 = fc; k2 < cta; ++k2) {             // (RSB is a multiple of 32: the whole warp is in this branch)
+                    float part;
+                    wait_words<kSeqSpinLimit>(xchg + (size_t)k2 * RSB + t, true, epoch, p.err, 2, part);
+                    fsum += part;
+                }
             }
             fsum += mine;
             if (tw && item < NW * 32) tw[7] = clock64() + (fsum == 1.2345e-30f);
@@ -451,15 +475,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                         const bool valid = t < GPS;
                         const float4 f = valid ? reinterpret_cast<const float4 *>(yfin)[s * GPS + t] : make_float4(0.f, 0.f, 0.f, 0.f);
                         if (tw) tw[9] = clock64() + (f.x == 1.2345e-30f);
-                        uint32_t lo, hi;
-                        float scale;
-                        const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(f.x, f.y, f.z, f.w, lo, hi, scale)), lane & ~(WL - 1));
-                        if (tw) tw[10] = clock64() + (lo == 0x12345678u);
-                        if (valid) {
-                            const size_t g = (size_t)(sb_first + s) * GPS + t;
-                            seq_publish16(lut_out + g, lo, hi, epoch);
-                            if ((t % WL) == 0) seq_publish16(ag_out + g / WL, __float_as_uint(scale), __float_as_uint(bias), epoch);
-                        }
+                        publish_lut_record<WL>(f, lane, valid, (size_t)(sb_first + s) * GPS + t, lut_out, ag_out, epoch);
+                        if (tw) tw[10] = clock64();
                     }
                 }
             } else {
@@ -468,14 +485,8 @@ __global__ void __launch_bounds__(kSeqThreads, 1) seq_kernel(const SeqParams p, 
                     const int t = t0 + lane;
                     const bool valid = t < nfin * GPS;
                     const float4 f = valid ? reinterpret_cast<const float4 *>(yfin)[t] : make_float4(0.f, 0.f, 0.f, 0.f);
-                    uint32_t lo, hi;
-                    float scale;
-                    const float bias = lut_bias<WL>(lut_addv8(lut_group<WL>(f.x, f.y, f.z, f.w, lo, hi, scale)), lane & ~(WL - 1));
-                    if (valid) {
-                        const size_t g = (size_t)sb_first * GPS + t;    // finished super-blocks are my first nfin ones
-                        seq_publish16(lut_out + g, lo, hi, epoch);
-                        if ((t % WL) == 0) seq_publish16(ag_out + g / WL, __float_as_uint(scale), __float_as_uint(bias), epoch);
-                    }
+                    // finished super-blocks are my first nfin ones
+                    publish_lut_record<WL>(f, lane, valid, (size_t)sb_first * GPS + t, lut_out, ag_out, epoch);
                 }
             }
         }
