@@ -412,15 +412,21 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
 // Smallest N that takes a prefill tile (unless set with the prefill_min_n knob).  W2: 32.  W3/W4: 32 as well, but a tensor of fewer
 // than 64 row tiles of 128 rows (the 4096-row Llama-2 projections: 32) fills a quarter of the SMs with one token tile, and there the
 // tiles overtake the W4 GEMV only between N = 64 and 128 (H100 SXM at 400 W, DESIGN.md 3.3): 128.
+// The integer path (one scale): 128 below 64 row tiles, 64 from there.  A tile then sums the whole K alone, so a tensor of few row
+// tiles runs long serial tiles: on BitNet-3B's 3200-row projections (25 row tiles) the GEMV wins at N = 64 and loses at 128, on the
+// 8640-row one (68 row tiles) the tile wins from N = 64 against both GEMV call forms (H100 SXM at 700 W, DESIGN.md 3.3).
 int tile_min_n(const StreamLayout &L) {
     if (g.prefill_min_n > 0) return g.prefill_min_n;
+    if (L.one_scale) return (L.nrsb * L.rsb + 127) / 128 < 64 ? 128 : 64;
     return (L.pb == 4 && (L.nrsb + 1) / 2 < 64) ? 128 : 32;
 }
 
-// Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): W2 or W3/W4 streams, chunk 128,
-// act group 64, per-row scales, N >= tile_min_n.
+// Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): W2 or W3/W4 streams, N >= tile_min_n,
+// and either the fp path (chunk 128, act group 64, per-row scales) or the integer path (one scale, act group K, chunk 128 or 64).
 bool takes_prefill_tile(const StreamLayout &L, int N) {
-    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && L.qch == 8 && L.act_group_size == 64 && !L.one_scale;
+    const bool int_path = L.one_scale && L.act_group_size == L.K;
+    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) &&
+           ((L.qch == 8 && L.act_group_size == 64 && !L.one_scale) || (int_path && (L.qch == 8 || L.qch == 4)));
 }
 
 // Prefill tile on the tensor cores (wgmma, tmac_prefill.cuh).  Returns 1 if the shape is not covered (caller falls back to the GEMV
@@ -428,11 +434,14 @@ bool takes_prefill_tile(const StreamLayout &L, int N) {
 int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls, const float *lb, void *C, int ldc, int out_f16, bool sym) {
     const StreamLayout &L = R.L;
     if (!sym || !takes_prefill_tile(L, N)) return 1;
+    const bool int_path = L.one_scale;   // takes_prefill_tile admits one-scale tensors on the integer path only
     const size_t rawsz = (L.blk + 127) & ~(size_t)127;
     // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
     const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
     const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
-    if (g.use_prefill16 && N >= 64) {   // fp path: scales folded into fp16 operands, fp32 accumulation over K in registers (tmac_prefill16.cuh)
+    // fp path: scales folded into fp16 operands, fp32 accumulation over K in registers (tmac_prefill16.cuh).  Not exact, so the
+    // integer path never takes it.
+    if (g.use_prefill16 && N >= 64 && !int_path) {
         const int nmain = L.K / 64, nextra = (L.nchunk + 31) / 32, ntile16 = (N + kP16NT - 1) / kP16NT;
         const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
         if (smem16 <= 227 * 1024) {
@@ -465,24 +474,27 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
             return 0;
         }
     }
-    const size_t smem = (size_t)kPfStages * (kPfStageBytes + kPfRec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
+    const size_t rec = pf_rec_bytes(int_path);
+    const size_t smem = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
     if (smem > 225 * 1024) return 1;
     const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;
-    if (g.d_tiles.ensure((size_t)ntile * nag * kPfRec)) return fail("out of device memory (LUT tiles)");
-    lut_tile_kernel<<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
+    if (g.d_tiles.ensure((size_t)ntile * nag * rec)) return fail("out of device memory (LUT tiles)");
+    if (int_path) lut_tile_kernel<true><<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, nullptr, nullptr, (unsigned char *)g.d_tiles.p, N, L.K);
+    else lut_tile_kernel<false><<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
     CUDA_OK(cudaGetLastError());
     PrefillParams p{};
     p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C;
     p.lut_tiles = (const unsigned char *)g.d_tiles.p;
     p.N = N; p.K = L.K; p.Mout = L.Mout; p.ldc = ldc; p.out_f16 = out_f16;
     p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride;
-    p.nrsb = L.nrsb; p.bits = L.bits;
+    p.nrsb = L.nrsb; p.bits = L.bits; p.qch = L.qch; p.scale0 = L.scale0;
     if (g.trace) {
         if (g.d_trace.ensure(8192)) return fail("out of device memory (trace)");
         CUDA_OK(cudaMemsetAsync(g.d_trace.p, 0, 3 * 32 * 4 * sizeof(long long), g.stream()));
         p.dbg = (long long *)g.d_trace.p; g.trace_ctas = 12;   // 96 rows of 4 = 48 rows of 8
     }
-    const auto fn = L.pb == 4 ? prefill_kernel<4> : prefill_kernel<2>;
+    const auto fn = int_path ? (L.pb == 4 ? prefill_kernel<4, true> : prefill_kernel<2, true>)
+                             : (L.pb == 4 ? prefill_kernel<4, false> : prefill_kernel<2, false>);
     CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fn<<<dim3(nrt, ntile), kPfThreads2, smem, g.stream()>>>(p);
     CUDA_OK(cudaGetLastError());

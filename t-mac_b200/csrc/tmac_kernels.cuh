@@ -503,6 +503,17 @@ template <typename I> __device__ __forceinline__ void store_out(void *const &C, 
     else reinterpret_cast<float *>(C)[i] = v;
 }
 
+// Integer-path (BitNet) output of one row and token from its exact integer sum isum = sum_b 2*alpha_b*CBits_b, the token's LUT
+// scale ls and bias lb and the tensor's one weight scale:
+// C = ((sum_b alpha_b*CBits_b) * LUT_Scales[0] + LUT_Biases[0]*alpha_0) * Scales[0] (python/t_mac/ops/qgemm.py:160,171-174),
+// every operation rounded on its own (no contraction into an fma), in the reference's order.
+__device__ __forceinline__ float int_path_out(int isum, float ls, float lb, float scale0) {
+    const float cb = __fmul_rn((float)isum, 0.5f);
+    const float t1 = __fmul_rn(cb, ls);
+    const float t2 = __fmul_rn(lb, 0.5f);
+    return __fmul_rn(__fadd_rn(t1, t2), scale0);
+}
+
 constexpr int kG3MaxWarps = 8;
 
 // MINB = minimum resident CTAs per SM the register allocation is tuned for: 3 (85 registers, more ILP;
@@ -758,14 +769,9 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         const int row = (p.rsb0 + rsb) * RSB + t;
         if (row >= p.row_begin && row < p.row_end) {
             float out;
-            if (INT_PATH) {
-                // C = ((sum_b alpha_b*CBits_b) * LUT_Scales[0] + LUT_Biases[0]*alpha_0) * Scales[0]
-                // (python/t_mac/ops/qgemm.py:160,171-174); isum = sum_b 2*alpha_b*CBits_b exactly.
-                const float cb = __fmul_rn((float)isum, 0.5f);
-                const float t1 = __fmul_rn(cb, FUSED ? row_scale : __ldg(lsg));
-                const float t2 = __fmul_rn(FUSED ? iscr[(p.K >> 5) + kG3MaxWarps] : __ldg(lbg), 0.5f);
-                out = __fmul_rn(__fadd_rn(t1, t2), p.scale0);
-            } else
+            if (INT_PATH)
+                out = int_path_out(isum, FUSED ? row_scale : __ldg(lsg), FUSED ? iscr[(p.K >> 5) + kG3MaxWarps] : __ldg(lbg), p.scale0);
+            else
                 out = fsum;
             const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
             store_out(Cb, o, out, p.out_f16);

@@ -25,9 +25,16 @@
 // (PF_STAGE_BLOCKS), the code decode (row_codes, tmac_kernels.cuh), the expansion table (pf_build_xtab) and the scale offset
 // in a block (kPfScaleOff).  Each tile keeps its own expansion of a chunk's codes into A entries.
 //
+// Integer path (INT_PATH, BitNet: one weight scale, one activation group per row): the int32 accumulator sums over the whole K
+// with no fold, and one epilogue per output applies the token's LUT scale and bias and the tensor's scale in the GEMV's order
+// (int_path_out).  The int32 sum is the GEMV's integer (|S| <= 15, |T8| <= 127: no overflow at any K a row can have), converted to
+// fp32 the same way, so the output is bit-identical to the GEMV and to the reference.  Its LUT records are the table entries only.
+//
 // Supported: PB == 2 (W2: a 128-row tile is one super-block) and PB == 4 (W3/W4: two 64-row super-blocks, one per consumer
-// warpgroup), chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points), symmetric LUT.  Everything else
-// takes the GEMV kernel once per activation row.
+// warpgroup), with a symmetric LUT and either
+//   fp path: chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points), or
+//   integer path: one scale, act group = K, chunk = 128 K (QCH 8) or 64 K (QCH 4).
+// Everything else takes the GEMV kernel once per activation row.
 #pragma once
 #include "tmac_kernels.cuh"
 
@@ -36,7 +43,7 @@ namespace tmac_b200 {
 struct PrefillParams {
     const unsigned char *W;        // stream layout of the tensor (first super-block)
     const int8_t *qlut;            // [N][K/4][16]
-    const float *lut_scales, *lut_biases;   // [N][K/64]
+    const float *lut_scales, *lut_biases;   // [N][K/64]; integer path: [N][1]
     void *C;                       // [N][ldc]
     int N, K, Mout, ldc, out_f16;
     int nchunk, zp, sd, blk_bytes;
@@ -44,6 +51,8 @@ struct PrefillParams {
     const unsigned char *lut_tiles; // output of lut_tile_kernel: [token tile][step][kPfRec]
     long long *dbg;                // optional trace [role][step][4] (TMAC_ENABLE_TRACE builds)
     int nrsb, bits;                // row super-blocks of the tensor (PB 4: the last row tile may hold only one), bit width
+    int qch;                       // quads of 16 K per chunk: 8, or 4 (integer path only)
+    float scale0;                  // integer path: the tensor's one weight scale
 };
 #ifdef TMAC_ENABLE_TRACE
 #define PF_TRACE(role, step, k) do { if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && (step) < 32) p.dbg[((role) * 32 + (step)) * 4 + (k)] = clock64(); } while (0)
@@ -97,12 +106,18 @@ __device__ __forceinline__ void wg_mma_s8_n128(uint32_t (&d)[64], uint64_t da, u
 //     [  512 B]  lut_scale[token][step]
 //     [ 1024 B]  (lut_bias[token][2c], lut_bias[token][2c+1]) of the step's chunk c = step/2
 // Tokens >= N are zero.  grid = (steps, token tiles), block = 128 (thread = token).
+// INT_PATH: the record is the 16384 bytes of table entries alone (the consumers read the token's one LUT scale and bias of
+// [N][1] in their epilogue); ls and lb are not read.
 // ---------------------------------------------------------------------------------------------------
-constexpr int kPfRec = 16384 + 512 + 1024;
+constexpr int kPfTab = 16384;
+constexpr int kPfRec = kPfTab + 512 + 1024;
+__host__ __device__ constexpr int pf_rec_bytes(bool int_path) { return int_path ? kPfTab : kPfRec; }
+template <bool INT_PATH>
 __global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K) {
+    constexpr int REC = pf_rec_bytes(INT_PATH);
     const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * 128 + t;
     const int nag = K / 64;
-    unsigned char *rec = out + ((size_t)tile * nag + step) * kPfRec;
+    unsigned char *rec = out + ((size_t)tile * nag + step) * REC;
     const uint2 *src = reinterpret_cast<const uint2 *>(qlut) + ((size_t)n * (K / 4) + (size_t)step * 16) * 2;
 #pragma unroll
     for (int kc = 0; kc < 8; ++kc) {
@@ -110,6 +125,7 @@ __global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const
         if (n < N) { lo = __ldg(src + kc * 4); hi = __ldg(src + kc * 4 + 2); }
         *reinterpret_cast<uint4 *>(rec + ((size_t)(kc * 16 + (t >> 3)) * 128 + (t & 7) * 16)) = make_uint4(lo.x, lo.y, hi.x, hi.y);
     }
+    if constexpr (INT_PATH) return;
     float l = 0.f; float2 b2 = make_float2(0.f, 0.f);
     if (n < N) { l = ls[(size_t)n * nag + step]; b2 = make_float2(lb[(size_t)n * nag + (step & ~1)], lb[(size_t)n * nag + (step | 1)]); }
     reinterpret_cast<float *>(rec + 16384)[t] = l;
@@ -193,15 +209,17 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 //   warps 8..11 : producers, thread = weight row; thread 0 also issues the record copy of each step
 // PB 2 (W2): a row tile is one 128-row super-block.  PB 4 (W3/W4): two 64-row super-blocks 2*tile + wg, one per consumer
 // warpgroup; when nrsb is odd the last tile's second super-block does not exist and its A rows are zero.
-template <int PB>
+// INT_PATH: the integer path (see the header); a step is 64 K, QCH / 4 of them per chunk.
+template <int PB, bool INT_PATH>
 __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
+    constexpr int REC = pf_rec_bytes(INT_PATH);
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [S][16 KB]
-    unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][kPfRec] B tile + lut scales + lut bias pairs
-    unsigned char *raw = sR + kPfStages * kPfRec;                          // [2][NSB][blk_bytes] packed blocks (codes + scales)
+    unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][REC] B tile (+ lut scales + lut bias pairs)
+    unsigned char *raw = sR + kPfStages * REC;                             // [2][NSB][blk_bytes] packed blocks (codes + scales)
     const int rawsz = (p.blk_bytes + 127) & ~127;
     uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // [128 * PB] expansion table
     uint64_t *bars = xtab + 128 * PB;
@@ -219,23 +237,24 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
     }
     __syncthreads();
     const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
-    const int nsteps = 2 * p.nchunk;                 // activation groups (two per chunk)
+    const int spc = INT_PATH ? p.qch >> 2 : 2;       // steps (64 K) per chunk
+    const int nsteps = spc * p.nchunk;               // fp path: activation groups (two per chunk)
 
     if (warp >= kPfConsWarps) {
         // ======================= producers: thread = weight row of the tile =======================
         PF_PRODUCER_ROW(PB, tid - kPfConsWarps * 32);
         const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
-        const unsigned char *rec_src = p.lut_tiles + (size_t)tile * nag * kPfRec;
+        const unsigned char *rec_src = p.lut_tiles + (size_t)tile * nag * REC;
         const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
         PF_STAGE_BLOCKS(PB, c, blk, 0, p.nchunk - 1, {
             const uint32_t *words = reinterpret_cast<const uint32_t *>(blk);
-            _Pragma("unroll 1") for (int h = 0; h < 2; ++h) {
-                const int step = 2 * c + h, s = step % kPfStages;
+            _Pragma("unroll 1") for (int h = 0; h < spc; ++h) {
+                const int step = spc * c + h, s = step % kPfStages;
                 if (r == 0) PF_TRACE(0, step, 0);
                 mbar_wait_parity(empty + s, ((step / kPfStages) & 1) ^ 1);     // stage released by the consumers of step - S
                 if (r == 0) {
                     PF_TRACE(0, step, 1);
-                    bulk_load(sR + (size_t)s * kPfRec, rec_src + (size_t)step * kPfRec, kPfRec, full + s);
+                    bulk_load(sR + (size_t)s * REC, rec_src + (size_t)step * REC, REC, full + s);
                 }
                 unsigned char *a_dst = sA + (size_t)s * kPfStageBytes;
                 _Pragma("unroll") for (int kc = 0; kc < 8; ++kc) {
@@ -284,53 +303,59 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
             return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + kPfScaleOff + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
         };
         float hs[2], zz[2], hs_n[2], zz_n[2];
+        if constexpr (!INT_PATH) {               // the integer path's blocks carry no scales
 #pragma unroll
-        for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h] = ld_s(0, r0 + 8 * h); zz[h] = zz_n[h] = ld_z(0, r0 + 8 * h); }
+            for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h] = ld_s(0, r0 + 8 * h); zz[h] = zz_n[h] = ld_z(0, r0 + 8 * h); }
+        }
         for (int step = 0; step < nsteps; ++step) {
             const int c = step >> 1, s = step % kPfStages;
-            if (!(step & 1) && c + 1 < p.nchunk) {
+            if (!INT_PATH && !(step & 1) && c + 1 < p.nchunk) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h) { hs_n[h] = ld_s(c + 1, r0 + 8 * h); zz_n[h] = ld_z(c + 1, r0 + 8 * h); }
             }
             if (tid == 0) PF_TRACE(1, step, 0);
             mbar_wait_parity(full + s, (step / kPfStages) & 1);
             if (tid == 0) PF_TRACE(1, step, 1);
-            const uint32_t a0 = smem_u32(sA + (size_t)s * kPfStageBytes) + wg * 1024, b0 = smem_u32(sR + (size_t)s * kPfRec);
+            const uint32_t a0 = smem_u32(sA + (size_t)s * kPfStageBytes) + wg * 1024, b0 = smem_u32(sR + (size_t)s * REC);
             wg_fence();
+            // fp path: each step's int32 tile is folded below, the next step overwrites it; integer path: one int32 sum over K
 #pragma unroll
-            for (int i = 0; i < 4; ++i) wg_mma_s8_n128(acc, wg_desc(a0 + i * 4096, 2048), wg_desc(b0 + i * 4096, 2048), i > 0 ? 1u : 0u);
+            for (int i = 0; i < 4; ++i)
+                wg_mma_s8_n128(acc, wg_desc(a0 + i * 4096, 2048), wg_desc(b0 + i * 4096, 2048), (i > 0 || (INT_PATH && step > 0)) ? 1u : 0u);
             wg_commit();
             wg_wait0();
             wg_fence_acc(acc);
             if (tid == 0) PF_TRACE(1, step, 2);
-            const unsigned char *rec = sR + (size_t)s * kPfRec;
-            const float2 *ls2 = reinterpret_cast<const float2 *>(rec + 16384);                 // (ls[t], ls[t+1]) pairs
-#pragma unroll
-            for (int c8 = 0; c8 < 16; ++c8) {
-                const float2 l = ls2[(8 * c8 + tc) >> 1];
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int j = 4 * c8 + 2 * h;
-                    accf[j] = fmaf(hs[h] * l.x, (float)(int)acc[j], accf[j]);
-                    accf[j + 1] = fmaf(hs[h] * l.y, (float)(int)acc[j + 1], accf[j + 1]);
-                }
-            }
-            if (step & 1) {
-                // LUT-bias / zero-point term of the chunk: (0.5*s + z)[row] * (lb[2c] + lb[2c+1])[token]
-                const float4 *lb4 = reinterpret_cast<const float4 *>(rec + 16384 + 512);  // two tokens: (lb0, lb1), (lb0, lb1)
+            if constexpr (!INT_PATH) {
+                const unsigned char *rec = sR + (size_t)s * REC;
+                const float2 *ls2 = reinterpret_cast<const float2 *>(rec + 16384);                 // (ls[t], ls[t+1]) pairs
 #pragma unroll
                 for (int c8 = 0; c8 < 16; ++c8) {
-                    const float4 l = lb4[(8 * c8 + tc) >> 1];
+                    const float2 l = ls2[(8 * c8 + tc) >> 1];
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int j = 4 * c8 + 2 * h;
-                        const float wz = hs[h] + zz[h];
-                        accf[j] = fmaf(wz, l.x + l.y, accf[j]);
-                        accf[j + 1] = fmaf(wz, l.z + l.w, accf[j + 1]);
+                        accf[j] = fmaf(hs[h] * l.x, (float)(int)acc[j], accf[j]);
+                        accf[j + 1] = fmaf(hs[h] * l.y, (float)(int)acc[j + 1], accf[j + 1]);
                     }
                 }
+                if (step & 1) {
+                    // LUT-bias / zero-point term of the chunk: (0.5*s + z)[row] * (lb[2c] + lb[2c+1])[token]
+                    const float4 *lb4 = reinterpret_cast<const float4 *>(rec + 16384 + 512);  // two tokens: (lb0, lb1), (lb0, lb1)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h]; zz[h] = zz_n[h]; }
+                    for (int c8 = 0; c8 < 16; ++c8) {
+                        const float4 l = lb4[(8 * c8 + tc) >> 1];
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int j = 4 * c8 + 2 * h;
+                            const float wz = hs[h] + zz[h];
+                            accf[j] = fmaf(wz, l.x + l.y, accf[j]);
+                            accf[j + 1] = fmaf(wz, l.z + l.w, accf[j + 1]);
+                        }
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h]; zz[h] = zz_n[h]; }
+                }
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(empty + s);        // A tile and record of this step are dead: the stage may be refilled
@@ -344,8 +369,12 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
             for (int c8 = 0; c8 < 16; ++c8)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    const int t = 8 * c8 + tc + e;
-                    if (t < ntok) store_out(p.C, (size_t)(n0 + t) * p.ldc + row, accf[4 * c8 + 2 * h + e], p.out_f16);
+                    const int t = 8 * c8 + tc + e, j = 4 * c8 + 2 * h + e;
+                    // integer path: the token's one LUT scale and bias ([N][1]) and the tensor's scale, in the GEMV's order
+                    if (t < ntok)
+                        store_out(p.C, (size_t)(n0 + t) * p.ldc + row,
+                                  INT_PATH ? int_path_out((int)acc[j], __ldg(p.lut_scales + n0 + t), __ldg(p.lut_biases + n0 + t), p.scale0) : accf[j],
+                                  p.out_f16);
                 }
         }
     }
