@@ -119,7 +119,7 @@ struct Context {
     int seq_grid = 0;                    // decode sequences: grid override (tests: CTA-boundary placements); 0 = one CTA per SM
     int use_prefill16 = 1;               // fp16-operand prefill tile for N >= 64 (tmac_prefill16.cuh); 0 = the exact int8 tile for every N >= tile_min_n
     int pf_streamk = 0;                  // stream-K over all SMs when a prefill call has fewer tiles than SMs (measured slower: B delivery from L2 is the bound)
-    int use_prefill = 1, prefill_min_n = 0;    // N >= prefill_min_n: the wgmma tiles (W2, W3/W4 g128 act64); 0 = by shape (tile_min_n)
+    int use_prefill = 1, prefill_min_n = 0;    // N >= prefill_min_n: the wgmma tiles (W2, W3/W4, takes_prefill_tile); 0 = by shape (tile_min_n)
     int npeer = 0; void *peer_out[7] = {};   // one-shot: peer output vectors of the next N = 1 launch (tmac_b200_peer_outputs)
     int64_t next_hint = 0;               // one-shot: tensor whose blocks the next launch prefetches into L2
     std::map<int64_t, Resident> res;
@@ -415,18 +415,47 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
 // The integer path (one scale): 128 below 64 row tiles, 64 from there.  A tile then sums the whole K alone, so a tensor of few row
 // tiles runs long serial tiles: on BitNet-3B's 3200-row projections (25 row tiles) the GEMV wins at N = 64 and loses at 128, on the
 // 8640-row one (68 row tiles) the tile wins from N = 64 against both GEMV call forms (H100 SXM at 700 W, DESIGN.md 3.3).
+// The other fp groupings follow the same rule, with one exception: a 32-K chunk (ggml Q4_0, GPTQ g32) makes the W3/W4 GEMV slower,
+// and on the 4096-row Llama-2 projections (32 row tiles) the tiles win from N = 64 against both call forms, so W3/W4 g32 tensors of
+// 32 to 63 row tiles take them from 64 (H100 SXM at 700 W, DESIGN.md 3.3).  Fewer row tiles keep 128 (not measured).
 int tile_min_n(const StreamLayout &L) {
     if (g.prefill_min_n > 0) return g.prefill_min_n;
     if (L.one_scale) return (L.nrsb * L.rsb + 127) / 128 < 64 ? 128 : 64;
-    return (L.pb == 4 && (L.nrsb + 1) / 2 < 64) ? 128 : 32;
+    const int nrt = (L.nrsb + 1) / 2;
+    if (L.pb == 4 && nrt < 64) return (L.ck == 32 && nrt >= 32) ? 64 : 128;
+    return 32;
 }
 
 // Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): W2 or W3/W4 streams, N >= tile_min_n,
-// and either the fp path (chunk 128, act group 64, per-row scales) or the integer path (one scale, act group K, chunk 128 or 64).
+// and either the fp path (per-row scales, K % 128 == 0, chunk 128, 64 or 32 K; the layout keeps the act group, 128, 64 or 32 K,
+// inside the chunk) or the integer path (one scale, act group K, chunk 128 or 64).
 bool takes_prefill_tile(const StreamLayout &L, int N) {
     const bool int_path = L.one_scale && L.act_group_size == L.K;
-    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) &&
-           ((L.qch == 8 && L.act_group_size == 64 && !L.one_scale) || (int_path && (L.qch == 8 || L.qch == 4)));
+    const bool fp_path = !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0;
+    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && (fp_path || (int_path && (L.qch == 8 || L.qch == 4)));
+}
+
+// The fp path's kernels of one grouping (QCH quads per chunk, AGQ quads per activation group): int8 tile, its LUT records,
+// fp16 tile, its B tiles.
+struct PfKernels {
+    void (*tile)(const PrefillParams);
+    void (*lut)(const int8_t *, const float *, const float *, unsigned char *, int, int);
+    void (*tile16)(const Prefill16Params);
+    void (*lut16)(const int8_t *, const float *, const float *, unsigned char *, int, int, int, int);
+};
+template <int PB, int QCH, int AGQ> PfKernels pf_kernels() {
+    return {prefill_kernel<PB, false, QCH, AGQ>, lut_tile_kernel<false, QCH, AGQ>, prefill16_kernel<PB, QCH, AGQ>, lut_tile16_kernel<QCH, AGQ>};
+}
+template <int PB> PfKernels pick_pf_qa(int qch, int agq) {
+    switch (qch * 16 + agq) {
+        case 8 * 16 + 8: return pf_kernels<PB, 8, 8>();
+        case 8 * 16 + 4: return pf_kernels<PB, 8, 4>();
+        case 8 * 16 + 2: return pf_kernels<PB, 8, 2>();
+        case 4 * 16 + 4: return pf_kernels<PB, 4, 4>();
+        case 4 * 16 + 2: return pf_kernels<PB, 4, 2>();
+        case 2 * 16 + 2: return pf_kernels<PB, 2, 2>();
+    }
+    return {};
 }
 
 // Prefill tile on the tensor cores (wgmma, tmac_prefill.cuh).  Returns 1 if the shape is not covered (caller falls back to the GEMV
@@ -435,7 +464,14 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
     const StreamLayout &L = R.L;
     if (!sym || !takes_prefill_tile(L, N)) return 1;
     const bool int_path = L.one_scale;   // takes_prefill_tile admits one-scale tensors on the integer path only
-    const size_t rawsz = (L.blk + 127) & ~(size_t)127;
+    const int agq = L.act_group_size / 16;
+    PfKernels fk{};
+    if (!int_path) {
+        fk = L.pb == 4 ? pick_pf_qa<4>(L.qch, agq) : pick_pf_qa<2>(L.qch, agq);
+        if (!fk.tile) return fail("prefill: no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
+    }
+    // the producers stage a 128-K window of 128 / ck chunk blocks (integer path: one chunk)
+    const size_t rawsz = ((int_path ? 1 : 8 / L.qch) * L.blk + 127) & ~(size_t)127;
     // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
     const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
     const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
@@ -446,7 +482,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
         const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
         if (smem16 <= 227 * 1024) {
             if (g.d_tiles.ensure((size_t)ntile16 * (nmain + nextra) * kP16BBytes)) return fail("out of device memory (LUT tiles)");
-            lut_tile16_kernel<<<dim3(nmain + nextra, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, nmain, nextra);
+            fk.lut16<<<dim3(nmain + nextra, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, nmain, nextra);
             CUDA_OK(cudaGetLastError());
             Prefill16Params q{};
             q.W = R.d; q.C = C; q.N = N; q.K = L.K; q.Mout = L.Mout; q.ldc = ldc; q.out_f16 = out_f16;
@@ -465,7 +501,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
                 }
                 q.scratch = (float *)g.d_pf_scratch.p; q.flags = (int *)g.d_pf_flags.p;
             }
-            const auto fn16 = L.pb == 4 ? prefill16_kernel<4> : prefill16_kernel<2>;
+            const auto fn16 = fk.tile16;
             CUDA_OK(cudaFuncSetAttribute((const void *)fn16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
             fn16<<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
             CUDA_OK(cudaGetLastError());
@@ -474,13 +510,13 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
             return 0;
         }
     }
-    const size_t rec = pf_rec_bytes(int_path);
+    const size_t rec = pf_rec_bytes(int_path, L.qch, agq);
     const size_t smem = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
     if (smem > 225 * 1024) return 1;
-    const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;
+    const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;   // records: one per 64-K step
     if (g.d_tiles.ensure((size_t)ntile * nag * rec)) return fail("out of device memory (LUT tiles)");
     if (int_path) lut_tile_kernel<true><<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, nullptr, nullptr, (unsigned char *)g.d_tiles.p, N, L.K);
-    else lut_tile_kernel<false><<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
+    else fk.lut<<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
     CUDA_OK(cudaGetLastError());
     PrefillParams p{};
     p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C;
@@ -493,8 +529,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
         CUDA_OK(cudaMemsetAsync(g.d_trace.p, 0, 3 * 32 * 4 * sizeof(long long), g.stream()));
         p.dbg = (long long *)g.d_trace.p; g.trace_ctas = 12;   // 96 rows of 4 = 48 rows of 8
     }
-    const auto fn = int_path ? (L.pb == 4 ? prefill_kernel<4, true> : prefill_kernel<2, true>)
-                             : (L.pb == 4 ? prefill_kernel<4, false> : prefill_kernel<2, false>);
+    const auto fn = int_path ? (L.pb == 4 ? prefill_kernel<4, true> : prefill_kernel<2, true>) : fk.tile;
     CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fn<<<dim3(nrt, ntile), kPfThreads2, smem, g.stream()>>>(p);
     CUDA_OK(cudaGetLastError());

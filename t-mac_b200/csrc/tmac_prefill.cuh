@@ -10,20 +10,21 @@
 // i.e. an exact dense int8 contraction of length 8 per K-group:  I[m][n] = S[m][:] . T8[n][:]  -- a true
 // int8 GEMM with int32 accumulation, bit-identical to the integer sums of the GEMV path.  It runs as
 // wgmma.mma_async m64n128k32.s32.s8.s8 (two consumer warpgroups = 128 weight rows, N = 128 tokens), accumulator in
-// registers.  Per activation group (64 K positions = 128 contraction bytes = 4 MMAs per warpgroup) the int32 tile is
-// folded into fp32 registers with lut_scale[n][ag] * 0.5*scale[m][wg]; the LUT-bias / zero-point terms are a
-// rank-(K/group_size) correction added once per chunk.
+// registers.  A step is 64 K positions = 128 contraction bytes = 4 MMAs per warpgroup.  Once per activation group (ags 32: after
+// MMAs {0, 1} and {2, 3} of a step; ags 64: after the step; ags 128: after every second step) the int32 tile is folded into fp32
+// registers with lut_scale[n][ag] * 0.5*scale[m][wg] -- the layout keeps an activation group inside one weight chunk, so the fold
+// has one weight scale; the LUT-bias / zero-point terms are a rank-(K/group_size) correction added once per chunk.
 //
 //   warpgroups 0, 1  consumers: 4 wgmma per step on rows 64*wg .. 64*wg+63, int32 -> fp32 fold, final store.
-//   warpgroup  2     producers: cp.async the (row super-block, chunk) block(s), expand the packed codes of "their"
+//   warpgroup  2     producers: cp.async the (row super-block, 128-K window) blocks, expand the packed codes of "their"
 //                    weight row into S (one 64-bit one-hot-signed vector per (row, group), through a 256-entry (W2) or
 //                    512-entry (W3/W4: two planes per lookup, two lookups added byte-wise) shared-memory table) in the
 //                    K-major no-swizzle canonical layout; fence.proxy.async; arrive full[s].  Thread 0 also issues the
 //                    step's LUT record as one bulk copy (TMA) into the same stage.
 //
 // Shared with the fp16 tile (tmac_prefill16.cuh): the producer's row (PF_PRODUCER_ROW), the double-buffered block staging
-// (PF_STAGE_BLOCKS), the code decode (row_codes, tmac_kernels.cuh), the expansion table (pf_build_xtab) and the scale offset
-// in a block (kPfScaleOff).  Each tile keeps its own expansion of a chunk's codes into A entries.
+// (PF_STAGE_BLOCKS), the code decode (row_codes, tmac_kernels.cuh), the expansion table (pf_build_xtab), the grouping constants
+// (PfGroups) and the scale offset in a block (pf_scale_off).  Each tile keeps its own expansion of a chunk's codes into A entries.
 //
 // Integer path (INT_PATH, BitNet: one weight scale, one activation group per row): the int32 accumulator sums over the whole K
 // with no fold, and one epilogue per output applies the token's LUT scale and bias and the tensor's scale in the GEMV's order
@@ -32,8 +33,11 @@
 //
 // Supported: PB == 2 (W2: a 128-row tile is one super-block) and PB == 4 (W3/W4: two 64-row super-blocks, one per consumer
 // warpgroup), with a symmetric LUT and either
-//   fp path: chunk = 128 K (QCH 8), act group 64 (AGQ 4), per-row scales (+ zero points), or
-//   integer path: one scale, act group = K, chunk = 128 K (QCH 8) or 64 K (QCH 4).
+//   fp path: K % 128 == 0, per-row scales (+ zero points), chunk ck = 128, 64 or 32 K (template QCH 8, 4, 2) and act group
+//            ags = 128, 64 or 32 K (template AGQ 8, 4, 2) with ags <= ck: (128, 128), (128, 64), (128, 32), (64, 64), (64, 32),
+//            (32, 32) -- the last is ggml Q4_0 and GPTQ g32.  The producers stage a 128-K window (128 / ck consecutive chunk
+//            blocks, one contiguous run of the stream layout) per two steps, whatever the chunk; or
+//   integer path: one scale, act group = K, chunk = 128 K or 64 K (p.qch at run time; QCH and AGQ are not used).
 // Everything else takes the GEMV kernel once per activation row.
 #pragma once
 #include "tmac_kernels.cuh"
@@ -43,12 +47,12 @@ namespace tmac_b200 {
 struct PrefillParams {
     const unsigned char *W;        // stream layout of the tensor (first super-block)
     const int8_t *qlut;            // [N][K/4][16]
-    const float *lut_scales, *lut_biases;   // [N][K/64]; integer path: [N][1]
+    const float *lut_scales, *lut_biases;   // [N][K/ags]; integer path: [N][1]
     void *C;                       // [N][ldc]
     int N, K, Mout, ldc, out_f16;
     int nchunk, zp, sd, blk_bytes;
     size_t rsb_stride;
-    const unsigned char *lut_tiles; // output of lut_tile_kernel: [token tile][step][kPfRec]
+    const unsigned char *lut_tiles; // output of lut_tile_kernel: [token tile][step][pf_rec_bytes]
     long long *dbg;                // optional trace [role][step][4] (TMAC_ENABLE_TRACE builds)
     int nrsb, bits;                // row super-blocks of the tensor (PB 4: the last row tile may hold only one), bit width
     int qch;                       // quads of 16 K per chunk: 8, or 4 (integer path only)
@@ -98,26 +102,43 @@ __device__ __forceinline__ void wg_mma_s8_n128(uint32_t (&d)[64], uint64_t da, u
                  : "l"(da), "l"(db), "r"(acc));
 }
 
+// The fp path's grouping: QCH quads of 16 K per weight chunk, AGQ quads per activation group (AGQ <= QCH, both 8, 4 or 2).  A
+// step is 64 K; a window, the producers' staging unit, is 128 K = WB chunk blocks (two steps).
+template <int QCH, int AGQ> struct PfGroups {
+    static_assert((QCH == 8 || QCH == 4 || QCH == 2) && (AGQ == 8 || AGQ == 4 || AGQ == 2) && QCH % AGQ == 0, "prefill grouping");
+    static constexpr int WB = 8 / QCH;                   // chunk blocks per window
+    static constexpr int SPC = QCH == 8 ? 2 : 1;         // steps per chunk set: the NCS chunks whose scales a consumer holds
+    static constexpr int NCS = QCH == 2 ? 2 : 1;         // chunks per chunk set (a step never straddles two sets)
+    static constexpr int APC = QCH / AGQ;                // activation groups per chunk
+    static constexpr int NLS = AGQ == 2 ? 2 : 1;         // LUT scales per token in a step's record: the step's activation groups
+    static constexpr int NLB = NCS * APC;                // LUT biases per token in a step's record: those of the step's chunk set
+};
+__host__ __device__ constexpr int pf_scale_off(int qch) { return qch * 512; }   // a block's scales follow its QCH quads of codes
+
 // ---------------------------------------------------------------------------------------------------
-// lut_tile_kernel: QLUT [N][K/4][16] + LUT_Scales/Biases [N][K/64]  ->  per (token tile of 128, activation group) one
-// contiguous 17920-byte record that the GEMM stage receives with ONE bulk copy (TMA):
-//     [16384 B]  the 8 stored LUT entries of the 16 groups of the step for 128 tokens, already in the K-major
-//                canonical order: chunk kc (groups 2kc, 2kc+1), token t at ((kc*16 + t/8)*128 + (t%8)*16)
-//     [  512 B]  lut_scale[token][step]
-//     [ 1024 B]  (lut_bias[token][2c], lut_bias[token][2c+1]) of the step's chunk c = step/2
+// lut_tile_kernel: QLUT [N][K/4][16] + LUT_Scales/Biases [N][K/ags]  ->  per (token tile of 128, 64-K step) one contiguous
+// record that the GEMM stage receives with ONE bulk copy (TMA):
+//     [16384 B]      the 8 stored LUT entries of the 16 groups of the step for 128 tokens, already in the K-major
+//                    canonical order: chunk kc (groups 2kc, 2kc+1), token t at ((kc*16 + t/8)*128 + (t%8)*16)
+//     [NLS * 512 B]  per token the LUT scales of the step's activation groups (ags 128: the group that holds the step)
+//     [NLB * 512 B]  per token the LUT biases of the activation groups of the step's chunk set (ck 128: chunk step/2)
+// (ck 128, ags 64: 17920 bytes: lut_scale[t][step], then (lut_bias[t][2c], lut_bias[t][2c+1]) of chunk c = step/2.)
 // Tokens >= N are zero.  grid = (steps, token tiles), block = 128 (thread = token).
 // INT_PATH: the record is the 16384 bytes of table entries alone (the consumers read the token's one LUT scale and bias of
 // [N][1] in their epilogue); ls and lb are not read.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kPfTab = 16384;
-constexpr int kPfRec = kPfTab + 512 + 1024;
-__host__ __device__ constexpr int pf_rec_bytes(bool int_path) { return int_path ? kPfTab : kPfRec; }
-template <bool INT_PATH>
+__host__ __device__ constexpr int pf_rec_bytes(bool int_path, int qch = 8, int agq = 4) {
+    return int_path ? kPfTab : kPfTab + 512 * ((agq == 2 ? 2 : 1) + (qch == 2 ? 2 : 1) * (qch / agq));   // PfGroups NLS + NLB
+}
+template <bool INT_PATH, int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K) {
-    constexpr int REC = pf_rec_bytes(INT_PATH);
+    using G = PfGroups<QCH, AGQ>;
+    constexpr int REC = pf_rec_bytes(INT_PATH, QCH, AGQ);
+    static_assert(INT_PATH || REC == kPfTab + 512 * (G::NLS + G::NLB), "record size");
     const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * 128 + t;
-    const int nag = K / 64;
-    unsigned char *rec = out + ((size_t)tile * nag + step) * REC;
+    const int nsteps = K / 64;
+    unsigned char *rec = out + ((size_t)tile * nsteps + step) * REC;
     const uint2 *src = reinterpret_cast<const uint2 *>(qlut) + ((size_t)n * (K / 4) + (size_t)step * 16) * 2;
 #pragma unroll
     for (int kc = 0; kc < 8; ++kc) {
@@ -126,18 +147,34 @@ __global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const
         *reinterpret_cast<uint4 *>(rec + ((size_t)(kc * 16 + (t >> 3)) * 128 + (t & 7) * 16)) = make_uint4(lo.x, lo.y, hi.x, hi.y);
     }
     if constexpr (INT_PATH) return;
-    float l = 0.f; float2 b2 = make_float2(0.f, 0.f);
-    if (n < N) { l = ls[(size_t)n * nag + step]; b2 = make_float2(lb[(size_t)n * nag + (step & ~1)], lb[(size_t)n * nag + (step | 1)]); }
-    reinterpret_cast<float *>(rec + 16384)[t] = l;
-    reinterpret_cast<float2 *>(rec + 16384 + 512)[t] = b2;
+    const int nag = K / (16 * AGQ);                                      // activation groups per row
+    const int ag0 = step * 4 / AGQ;                                      // the step's first activation group
+    const int lb0 = (QCH == 8 ? step >> 1 : step * G::NCS) * G::APC;     // first activation group of the step's chunk set
+    float *lsd = reinterpret_cast<float *>(rec + 16384) + t * G::NLS, *lbd = reinterpret_cast<float *>(rec + 16384 + 512 * G::NLS) + t * G::NLB;
+#pragma unroll
+    for (int i = 0; i < G::NLS; ++i) lsd[i] = n < N ? ls[(size_t)n * nag + ag0 + i] : 0.f;
+#pragma unroll
+    for (int i = 0; i < G::NLB; ++i) lbd[i] = n < N ? lb[(size_t)n * nag + lb0 + i] : 0.f;
+}
+
+// NV consecutive floats of shared memory (NV = 2, 4 or 8, aligned to their size) as vector loads
+template <int NV> __device__ __forceinline__ void pf_ld_floats(const float *src, float (&v)[NV]) {
+    if constexpr (NV == 2) {
+        const float2 a = *reinterpret_cast<const float2 *>(src);
+        v[0] = a.x; v[1] = a.y;
+    } else {
+#pragma unroll
+        for (int i = 0; i < NV / 4; ++i) {
+            const float4 a = reinterpret_cast<const float4 *>(src)[i];
+            v[4 * i] = a.x; v[4 * i + 1] = a.y; v[4 * i + 2] = a.z; v[4 * i + 3] = a.w;
+        }
+    }
 }
 
 constexpr int kPfStages = 4;                     // stages: A tile 16 KB (expanded by the producers) + record 17.5 KB (TMA)
 constexpr int kPfConsWarps = 8;                  // two consumer warpgroups
 constexpr int kPfProdWarps = 4;                  // one producer warpgroup
 constexpr int kPfThreads2 = (kPfConsWarps + kPfProdWarps) * 32;
-
-constexpr int kPfScaleOff = 8 * 512;            // a block's scales follow its QCH 8 quads of 512 B of codes
 
 // Expansion table: 128*PB entries, each indexed by one byte of row_codes<PB> (two planes, nibble = neg << 3 | j),
 //   [0, 256)    planes 0, 1: +-w0 at byte j0 plus +-w1 at byte j1
@@ -170,23 +207,25 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 #define PF_PRODUCER_ROW(PB, r_)                                                                                              \
     const int r = (r_), sb = (PB) == 4 ? r >> 6 : 0, wl = (PB) == 4 ? (r & 63) >> 1 : r >> 2, wi = (PB) == 4 ? r & 1 : r & 3
 
-// PF_STAGE_BLOCKS runs the expansion (the variadic argument) once per chunk c of [c_first, c_last], with blk = the thread's
-// super-block's block of chunk c in shared memory (codes, then the scales at kPfScaleOff).  The blocks come from rsb_base (the row
-// tile's first super-block) and sb_base (super-block sb) through raw, a double buffer [2][NSB][rawsz] with chunk c in half c & 1:
-// cp.async fetches chunk c + 1 while chunk c is expanded.  The 128 / NSB threads of a super-block stage its blocks; a super-block
-// that is not live stages nothing.  Named barrier 1 (the 128 producer threads) makes block c visible to every producer and retires
-// block c - 1, whose half then takes chunk c + 1.  The block of c_last may still be read when the loop ends: a producer that stages
-// another run passes barrier 1 before it.  Besides PF_PRODUCER_ROW's names it reads p, live, rsb_base, sb_base, raw, rawsz and NSB
-// of the kernel.
-#define PF_STAGE_BLOCKS(PB, c, blk, c_first, c_last, ...)                                                                    \
+// PF_STAGE_BLOCKS runs the expansion (the variadic argument) once per staging unit c of [c_first, c_last] -- WB consecutive chunk
+// blocks, which are contiguous in the stream layout: a 128-K window on the fp path, one chunk on the integer path -- with blk = the
+// thread's super-block's first block of unit c in shared memory (each block: codes, then the scales at pf_scale_off(QCH)).  The
+// blocks come from rsb_base (the row tile's first super-block) and sb_base (super-block sb) through raw, a double buffer
+// [2][NSB][rawsz] with unit c in half c & 1: cp.async fetches unit c + 1 while unit c is expanded.  The 128 / NSB threads of a
+// super-block stage its blocks; a super-block that is not live stages nothing.  Named barrier 1 (the 128 producer threads) makes
+// unit c visible to every producer and retires unit c - 1, whose half then takes unit c + 1.  The blocks of c_last may still be
+// read when the loop ends: a producer that stages another run passes barrier 1 before it.  Besides PF_PRODUCER_ROW's names it reads
+// p, live, rsb_base, sb_base, raw, rawsz and NSB of the kernel.
+#define PF_STAGE_BLOCKS(PB, WB, c, blk, c_first, c_last, ...)                                                                \
     do {                                                                                                                     \
-        const int pf_c0 = (c_first), pf_c1 = (c_last), n16 = p.blk_bytes >> 4;                                             \
-        auto load_blocks = [&](int c_, unsigned char *dst) {   /* chunk c_ of the tile's super-block(s) -> dst [NSB][rawsz] */ \
+        const int pf_c0 = (c_first), pf_c1 = (c_last), n16 = ((WB) * p.blk_bytes) >> 4;                                     \
+        auto load_blocks = [&](int c_, unsigned char *dst) {   /* unit c_ of the tile's super-block(s) -> dst [NSB][rawsz] */ \
+            const size_t src0 = (size_t)c_ * (WB) * p.blk_bytes;                                                             \
             if constexpr ((PB) == 2) {                                                                                       \
-                for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + (size_t)c_ * p.blk_bytes + i * 16); \
+                for (int i = r; i < n16; i += 128) cp_async16_plain(dst + i * 16, rsb_base + src0 + i * 16);                 \
             } else if (live) {                                                                                               \
                 for (int i = r & 63; i < n16; i += 64)                                                                       \
-                    cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + (size_t)c_ * p.blk_bytes + i * 16);        \
+                    cp_async16_plain(dst + (size_t)sb * rawsz + i * 16, sb_base + src0 + i * 16);                            \
             }                                                                                                                \
         };                                                                                                                   \
         load_blocks(pf_c0, raw + (size_t)(pf_c0 & 1) * NSB * rawsz);                                                        \
@@ -209,18 +248,21 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 //   warps 8..11 : producers, thread = weight row; thread 0 also issues the record copy of each step
 // PB 2 (W2): a row tile is one 128-row super-block.  PB 4 (W3/W4): two 64-row super-blocks 2*tile + wg, one per consumer
 // warpgroup; when nrsb is odd the last tile's second super-block does not exist and its A rows are zero.
-// INT_PATH: the integer path (see the header); a step is 64 K, QCH / 4 of them per chunk.
-template <int PB, bool INT_PATH>
+// fp path: a step is 64 K, two per 128-K window.  INT_PATH: the integer path (see the header); a step is 64 K, p.qch / 4 of them
+// per chunk, and the staging unit is one chunk.
+template <int PB, bool INT_PATH, int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    using G = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
-    constexpr int REC = pf_rec_bytes(INT_PATH);
+    constexpr int REC = pf_rec_bytes(INT_PATH, QCH, AGQ);
+    constexpr int WB = INT_PATH ? 1 : G::WB;                               // chunk blocks per staging unit
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [S][16 KB]
-    unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][REC] B tile (+ lut scales + lut bias pairs)
-    unsigned char *raw = sR + kPfStages * REC;                             // [2][NSB][blk_bytes] packed blocks (codes + scales)
-    const int rawsz = (p.blk_bytes + 127) & ~127;
+    unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][REC] B tile (+ lut scales + lut biases)
+    unsigned char *raw = sR + kPfStages * REC;                             // [2][NSB][WB * blk_bytes] packed blocks (codes + scales)
+    const int rawsz = (WB * p.blk_bytes + 127) & ~127;
     uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // [128 * PB] expansion table
     uint64_t *bars = xtab + 128 * PB;
     uint64_t *full = bars, *empty = bars + kPfStages;
@@ -237,8 +279,9 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
     }
     __syncthreads();
     const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
-    const int spc = INT_PATH ? p.qch >> 2 : 2;       // steps (64 K) per chunk
-    const int nsteps = spc * p.nchunk;               // fp path: activation groups (two per chunk)
+    const int spc = INT_PATH ? p.qch >> 2 : 2;       // steps (64 K) per staging unit
+    const int nunits = p.nchunk / WB;                // fp path: 128-K windows; integer path: chunks
+    const int nsteps = spc * nunits;
 
     if (warp >= kPfConsWarps) {
         // ======================= producers: thread = weight row of the tile =======================
@@ -246,7 +289,7 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
         const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
         const unsigned char *rec_src = p.lut_tiles + (size_t)tile * nag * REC;
         const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
-        PF_STAGE_BLOCKS(PB, c, blk, 0, p.nchunk - 1, {
+        PF_STAGE_BLOCKS(PB, WB, c, blk, 0, nunits - 1, {
             const uint32_t *words = reinterpret_cast<const uint32_t *>(blk);
             _Pragma("unroll 1") for (int h = 0; h < spc; ++h) {
                 const int step = spc * c + h, s = step % kPfStages;
@@ -260,9 +303,11 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                 _Pragma("unroll") for (int kc = 0; kc < 8; ++kc) {
                     uint64_t v2[2];
                     _Pragma("unroll") for (int u = 0; u < 2; ++u) {
-                        const int gq = h * 16 + kc * 2 + u;                // group within the chunk (0..31)
-                        const int q = gq >> 2, k = gq & 3;
-                        const uint32_t cw = row_codes<PB>(words + ((size_t)q * 32 + wl) * 4, k, wi);
+                        const int gq = h * 16 + kc * 2 + u;                // group within the unit (0..31)
+                        // its block in the window and its quad / word there
+                        const int b = WB == 1 ? 0 : gq / (4 * QCH), gb = WB == 1 ? gq : gq % (4 * QCH);
+                        const int q = gb >> 2, k = gb & 3;
+                        const uint32_t cw = row_codes<PB>(words + (size_t)b * (p.blk_bytes >> 2) + ((size_t)q * 32 + wl) * 4, k, wi);
                         if constexpr (PB == 2) {
                             v2[u] = xtab[cw];
                         } else {
@@ -297,64 +342,102 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
         const unsigned char *wg_base = rsb_base + (size_t)(PB == 4 ? wg : 0) * p.rsb_stride;
         const bool live = PB == 2 || rt * NSB + wg < p.nrsb;
         auto ld_s = [&](int c, int r) {
-            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + kPfScaleOff, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + pf_scale_off(QCH), p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
         };
         auto ld_z = [&](int c, int r) {
-            return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + kPfScaleOff + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+            return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + pf_scale_off(QCH) + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
         };
-        float hs[2], zz[2], hs_n[2], zz_n[2];
+        // the scales of the chunk set (G::NCS chunks) of the step and of the next set
+        float hs[G::NCS][2], zz[G::NCS][2], hs_n[G::NCS][2], zz_n[G::NCS][2];
         if constexpr (!INT_PATH) {               // the integer path's blocks carry no scales
 #pragma unroll
-            for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h] = ld_s(0, r0 + 8 * h); zz[h] = zz_n[h] = ld_z(0, r0 + 8 * h); }
-        }
-        for (int step = 0; step < nsteps; ++step) {
-            const int c = step >> 1, s = step % kPfStages;
-            if (!INT_PATH && !(step & 1) && c + 1 < p.nchunk) {
+            for (int i = 0; i < G::NCS; ++i)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) { hs_n[h] = ld_s(c + 1, r0 + 8 * h); zz_n[h] = ld_z(c + 1, r0 + 8 * h); }
+                for (int h = 0; h < 2; ++h) { hs[i][h] = hs_n[i][h] = ld_s(i, r0 + 8 * h); zz[i][h] = zz_n[i][h] = ld_z(i, r0 + 8 * h); }
+        }
+        // MMAs {0..3} of a step in NF runs of 4 / NF; the fp path folds after each run (ags 32: two activation groups per step)
+        constexpr int NF = (!INT_PATH && AGQ == 2) ? 2 : 1, MPF = 4 / NF;
+        // ags 128: the two steps of a window run as one unrolled pair (su), so which one folds is known at compile time
+        constexpr int SU = (!INT_PATH && AGQ == 8) ? 2 : 1;
+        for (int step0 = 0; step0 < nsteps; step0 += SU)
+#pragma unroll
+        for (int su = 0; su < SU; ++su) {
+            const int step = step0 + su;
+            const bool set_first = SU == 2 ? su == 0 : step % G::SPC == 0, set_last = SU == 2 ? su == 1 : step % G::SPC == G::SPC - 1;
+            const int cs = step / G::SPC, s = step % kPfStages;
+            if (!INT_PATH && set_first && (cs + 1) * G::NCS < p.nchunk) {
+#pragma unroll
+                for (int i = 0; i < G::NCS; ++i)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) { hs_n[i][h] = ld_s((cs + 1) * G::NCS + i, r0 + 8 * h); zz_n[i][h] = ld_z((cs + 1) * G::NCS + i, r0 + 8 * h); }
             }
             if (tid == 0) PF_TRACE(1, step, 0);
             mbar_wait_parity(full + s, (step / kPfStages) & 1);
             if (tid == 0) PF_TRACE(1, step, 1);
             const uint32_t a0 = smem_u32(sA + (size_t)s * kPfStageBytes) + wg * 1024, b0 = smem_u32(sR + (size_t)s * REC);
-            wg_fence();
-            // fp path: each step's int32 tile is folded below, the next step overwrites it; integer path: one int32 sum over K
+            const unsigned char *rec = sR + (size_t)s * REC;
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
-                wg_mma_s8_n128(acc, wg_desc(a0 + i * 4096, 2048), wg_desc(b0 + i * 4096, 2048), (i > 0 || (INT_PATH && step > 0)) ? 1u : 0u);
-            wg_commit();
-            wg_wait0();
-            wg_fence_acc(acc);
-            if (tid == 0) PF_TRACE(1, step, 2);
-            if constexpr (!INT_PATH) {
-                const unsigned char *rec = sR + (size_t)s * REC;
-                const float2 *ls2 = reinterpret_cast<const float2 *>(rec + 16384);                 // (ls[t], ls[t+1]) pairs
+            for (int f = 0; f < NF; ++f) {
+                wg_fence();
+                // fp path: each run's int32 tile is folded below and the next run overwrites it, except that ags 128 carries it
+                // into the step's odd partner; integer path: one int32 sum over K
 #pragma unroll
-                for (int c8 = 0; c8 < 16; ++c8) {
-                    const float2 l = ls2[(8 * c8 + tc) >> 1];
+                for (int i = 0; i < MPF; ++i) {
+                    const int m = f * MPF + i;
+                    wg_mma_s8_n128(acc, wg_desc(a0 + m * 4096, 2048), wg_desc(b0 + m * 4096, 2048),
+                                   (i > 0 || (INT_PATH && step > 0) || (SU == 2 && su == 1)) ? 1u : 0u);
+                }
+                wg_commit();
+                wg_wait0();
+                wg_fence_acc(acc);
+                if (tid == 0 && f == NF - 1) PF_TRACE(1, step, 2);
+                if constexpr (!INT_PATH) {
+                    if (SU == 1 || su == 1) {
+                        // the activation group ends here: accf += 0.5*s[row] * ls[token] * acc, s of the group's chunk
+                        const float *lsp = reinterpret_cast<const float *>(rec + 16384);
+                        const int ci = G::NCS == 2 ? f : 0;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int j = 4 * c8 + 2 * h;
-                        accf[j] = fmaf(hs[h] * l.x, (float)(int)acc[j], accf[j]);
-                        accf[j + 1] = fmaf(hs[h] * l.y, (float)(int)acc[j + 1], accf[j + 1]);
+                        for (int c8 = 0; c8 < 16; ++c8) {
+                            float lv[2 * G::NLS];                                  // tokens t, t + 1: their NLS LUT scales each
+                            pf_ld_floats(lsp + ((8 * c8 + tc) >> 1) * 2 * G::NLS, lv);
+                            const float lx = lv[G::NLS == 2 ? f : 0], ly = lv[G::NLS + (G::NLS == 2 ? f : 0)];
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int j = 4 * c8 + 2 * h;
+                                accf[j] = fmaf(hs[ci][h] * lx, (float)(int)acc[j], accf[j]);
+                                accf[j + 1] = fmaf(hs[ci][h] * ly, (float)(int)acc[j + 1], accf[j + 1]);
+                            }
+                        }
                     }
                 }
-                if (step & 1) {
-                    // LUT-bias / zero-point term of the chunk: (0.5*s + z)[row] * (lb[2c] + lb[2c+1])[token]
-                    const float4 *lb4 = reinterpret_cast<const float4 *>(rec + 16384 + 512);  // two tokens: (lb0, lb1), (lb0, lb1)
+            }
+            if constexpr (!INT_PATH) {
+                if (set_last) {
+                    // the chunk set ends here: LUT-bias / zero-point term of each chunk, (0.5*s + z)[row] * (sum of the chunk's
+                    // activation groups' lb)[token]
+                    const float *lbp = reinterpret_cast<const float *>(rec + 16384 + 512 * G::NLS);
 #pragma unroll
                     for (int c8 = 0; c8 < 16; ++c8) {
-                        const float4 l = lb4[(8 * c8 + tc) >> 1];
+                        float lv[2 * G::NLB];                                      // tokens t, t + 1: their NLB LUT biases each
+                        pf_ld_floats(lbp + ((8 * c8 + tc) >> 1) * 2 * G::NLB, lv);
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
                             const int j = 4 * c8 + 2 * h;
-                            const float wz = hs[h] + zz[h];
-                            accf[j] = fmaf(wz, l.x + l.y, accf[j]);
-                            accf[j + 1] = fmaf(wz, l.z + l.w, accf[j + 1]);
+#pragma unroll
+                            for (int i = 0; i < G::NCS; ++i) {
+                                float bx = lv[i * G::APC], by = lv[G::NLB + i * G::APC];
+#pragma unroll
+                                for (int a = 1; a < G::APC; ++a) { bx += lv[i * G::APC + a]; by += lv[G::NLB + i * G::APC + a]; }
+                                const float wz = hs[i][h] + zz[i][h];
+                                accf[j] = fmaf(wz, bx, accf[j]);
+                                accf[j + 1] = fmaf(wz, by, accf[j + 1]);
+                            }
                         }
                     }
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) { hs[h] = hs_n[h]; zz[h] = zz_n[h]; }
+                    for (int i = 0; i < G::NCS; ++i)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) { hs[i][h] = hs_n[i][h]; zz[i][h] = zz_n[i][h]; }
                 }
             }
             __syncwarp();

@@ -2,7 +2,7 @@
 // whole K in registers (wgmma), stream-K over the SMs when there are fewer tiles than SMs.
 //
 //   C[m][n] = sum_{g,e} (0.5*scale[m][wg(g)] * S[m][g][e]) * (lut_scale[n][ag(g)] * T8[n][g][e])            (main term)
-//           + sum_wg (0.5*scale[m][wg] + zero[m][wg]) * (lut_bias[n][2wg] + lut_bias[n][2wg+1])            (bias term)
+//           + sum_wg (0.5*scale[m][wg] + zero[m][wg]) * LB[n][wg],  LB[n][wg] = sum_{ag in chunk wg} lut_bias[n][ag]   (bias term)
 //
 // The int8 tile (tmac_prefill.cuh) keeps the reference's integer sums exact but has to rescale the accumulator after every
 // activation group.  Here both factors ride in the operands: A = fp16(0.5*s*S) is expanded by the producers from the packed
@@ -12,14 +12,16 @@
 // keeps the result inside north_star's 1e-3 of the CPU kernel (tools/sim_fp16_prefill.py: 1.4e-4 W2, 2.2-2.7e-4 W3/W4) -- NOT inside
 // the 2e-5 the exact paths hold, so this tile has its own tolerance and never serves the int32 (BitNet) path.
 //
-// Tile: 128 weight rows x 256 tokens per CTA, wgmma.mma_async m64n256k16.f32.f16.f16, 8 MMAs per warpgroup per activation group.
+// Tile: 128 weight rows x 256 tokens per CTA, wgmma.mma_async m64n256k16.f32.f16.f16, 8 MMAs per warpgroup per 64-K step.
 //   warpgroups 0, 1 : consumers (rows 64*wg .. 64*wg+63, 128 fp32 accumulators per thread), then the epilogue.
-//   warpgroup  2    : producers (thread = weight row, the step's 16 K-groups): plane codes -> 8 fp16 entries fp16(k * hs), one 16-byte
-//                     store per group into the K-major canonical A tile; thread 0 also issues the step's 64 KB B tile as one bulk copy (TMA).
-// Supported: W2 (PB 2) and W3/W4 (PB 4: a 128-row tile is two 64-row super-blocks), chunk 128, act group 64, per-row scales
-// (+ zero points), symmetric LUT -- as the int8 tile.  The producers take their row, block staging, code decode, PB 4 table and
-// scale offset from the int8 tile's shared code (tmac_prefill.cuh: PF_PRODUCER_ROW, PF_STAGE_BLOCKS, row_codes, pf_build_xtab,
-// kPfScaleOff); the expansion into fp16 A entries is this tile's own.  Each stream-K fragment is staged as one run.
+//   warpgroup  2    : producers (thread = weight row, the step's 16 K-groups): plane codes -> 8 fp16 entries fp16(k * hs), hs of the
+//                     group's own chunk, one 16-byte store per group into the K-major canonical A tile; thread 0 also issues the
+//                     step's 64 KB B tile as one bulk copy (TMA).
+// Supported: W2 (PB 2) and W3/W4 (PB 4: a 128-row tile is two 64-row super-blocks), K % 128 == 0, the int8 tile's fp-path
+// groupings (chunk ck = 128, 64 or 32 K: QCH 8, 4, 2; act group ags = 128, 64 or 32 K <= ck: AGQ 8, 4, 2), per-row scales
+// (+ zero points), symmetric LUT.  The producers take their row, 128-K window staging, code decode, PB 4 table, grouping constants
+// and scale offset from the int8 tile's shared code (tmac_prefill.cuh: PF_PRODUCER_ROW, PF_STAGE_BLOCKS, row_codes, pf_build_xtab,
+// PfGroups, pf_scale_off); the expansion into fp16 A entries is this tile's own.  Each stream-K fragment is staged as one run.
 #pragma once
 #include "tmac_prefill.cuh"
 
@@ -38,7 +40,7 @@ struct Prefill16Params {
     void *C;
     int N, K, Mout, ldc, out_f16;
     int nchunk, zp, sd, blk_bytes;
-    int nmain, nextra;                               // activation-group steps, bias steps (128 columns = 32 weight groups each)
+    int nmain, nextra;                               // 64-K steps, bias steps (128 columns = 32 weight groups each)
     size_t rsb_stride;
     const unsigned char *tiles;                      // lut_tile16_kernel output: [token tile][nmain + nextra][kP16BBytes]
     int nrsb, ntiles, streamk;                       // row super-blocks, tiles = nrt * token tiles, stream-K split (see the kernel)
@@ -63,18 +65,25 @@ __device__ __forceinline__ void wg_mma_f16_n256(float (&d)[128], uint64_t da, ui
 }
 
 // B tiles.  grid = (nmain + nextra, token tiles of 256), block = 256 (thread = token).
-//   step < nmain : entries (lut_scale[n][step] * T8[n][16*step + g][e]) as fp16, token t, group g at ((g*32 + t/8)*128 + (t%8)*16)
-//   bias steps   : column 4*wg + {0,1,2,3} = {LBhi, LBlo, LBhi, LBlo}, LB = lut_bias[n][2wg] + lut_bias[n][2wg+1]; 8 columns per chunk
+//   step < nmain : entries (lut_scale[n][ag(16*step + g)] * T8[n][16*step + g][e]) as fp16, token t, group g at
+//                  ((g*32 + t/8)*128 + (t%8)*16), ag(g) = the activation group of K-group g
+//   bias steps   : column 4*wg + {0,1,2,3} = {LBhi, LBlo, LBhi, LBlo}, LB = the sum of lut_bias[n][ag] over the activation groups
+//                  ag of chunk wg in order (ck 128, ags 64: lut_bias[n][2wg] + lut_bias[n][2wg+1]); 8 columns per chunk
+template <int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K,
                                                          int nmain, int nextra) {
+    using G = PfGroups<QCH, AGQ>;
     const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * kP16NT + t;
-    const int nag = K / 64, nwg = K / 128;
+    const int nag = K / (16 * AGQ), nwg = K / (16 * QCH);
     unsigned char *rec = out + ((size_t)tile * (nmain + nextra) + step) * kP16BBytes;
     if (step < nmain) {
-        const float l = (n < N) ? ls[(size_t)n * nag + step] : 0.f;
+        float ll[G::NLS];                            // the LUT scales of the step's activation groups
+#pragma unroll
+        for (int i = 0; i < G::NLS; ++i) ll[i] = (n < N) ? ls[(size_t)n * nag + step * 4 / AGQ + i] : 0.f;
         const uint2 *src = reinterpret_cast<const uint2 *>(qlut) + ((size_t)n * (K / 4) + (size_t)step * 16) * 2;
 #pragma unroll
         for (int g = 0; g < 16; ++g) {
+            const float l = ll[g * G::NLS / 16];
             uint2 q = make_uint2(0, 0);
             if (n < N) q = __ldg(src + g * 2);       // the 8 stored entries of the group
             uint32_t o[4];
@@ -97,7 +106,11 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
             for (int u = 0; u < 2; ++u) {
                 const int wg = e * 32 + kc * 2 + u;
                 float LB = 0.f;
-                if (n < N && wg < nwg) LB = lb[(size_t)n * nag + 2 * wg] + lb[(size_t)n * nag + 2 * wg + 1];
+                if (n < N && wg < nwg) {
+                    LB = lb[(size_t)n * nag + G::APC * wg];
+#pragma unroll
+                    for (int a = 1; a < G::APC; ++a) LB += lb[(size_t)n * nag + G::APC * wg + a];
+                }
                 const __half hi = __float2half_rn(LB);
                 const __half lo = __float2half_rn(LB - __half2float(hi));
                 const __half2 h = __halves2half2(hi, lo);
@@ -122,16 +135,17 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
 // Row tile = 128 rows.  PB 2 (W2): one super-block.  PB 4 (W3/W4): super-blocks 2*rt and 2*rt + 1 (64 rows each), producer
 // threads 0..63 / 64..127 and consumer warpgroups 0 / 1; when nrsb is odd the last tile's second super-block does not exist and
 // its A rows are zero.
-template <int PB>
+template <int PB, int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill16Params p) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    using PG = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [NA][32 KB]
     unsigned char *sB = sA + kP16NA * kP16SubA;                            // [NB][64 KB]
-    unsigned char *raw = sB + kP16NB * kP16SubB;                           // [2][NSB][blk] packed blocks (codes + scales)
-    const int rawsz = (p.blk_bytes + 127) & ~127;
+    unsigned char *raw = sB + kP16NB * kP16SubB;                           // [2][NSB][WB * blk] packed 128-K windows (codes + scales)
+    const int rawsz = (PG::WB * p.blk_bytes + 127) & ~127;
     uint64_t *xtab = reinterpret_cast<uint64_t *>(raw + 2 * NSB * rawsz);  // PB 4: [512] expansion table (pf_build_xtab, biased)
     uint64_t *bars = xtab + (PB == 4 ? 512 : 0);
     uint64_t *full = bars, *empty = full + kP16NA;
@@ -193,23 +207,39 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
             if (s0 < s1m) {
                 const int c_first = s0 >> 1, c_last = (s1m - 1) >> 1;
                 asm volatile("bar.sync 1, 128;" ::: "memory");             // the previous fragment's last block is dead
-                PF_STAGE_BLOCKS(PB, c, blk, c_first, c_last, {
+                PF_STAGE_BLOCKS(PB, PG::WB, c, blk, c_first, c_last, {
                     const uint32_t *words = reinterpret_cast<const uint32_t *>(blk);
-                    // hs = fp16(0.5 * scale).  PB 2: the row's 8 A entries of one K-group are +-hs at entry j0 (plane 0) plus +-2hs at
-                    // entry j1 (plane 1), built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the exact k * hs.
-                    const __half hsh = __float2half_rn(live ? 0.5f * load_scale(blk + kPfScaleOff, p.sd, srow) : 0.f);
-                    const uint32_t c1 = __half_as_ushort(hsh), c2 = __half_as_ushort(__hadd(hsh, hsh));
-                    const int u0 = (c == c_first) ? (s0 & 1) : 0, u1 = (c == c_last) ? ((s1m - 1) & 1) : 1;   // steps of this chunk
+                    // hs = fp16(0.5 * scale) of block b's chunk.  PB 2: the row's 8 A entries of one K-group are +-hs at entry j0
+                    // (plane 0) plus +-2hs at entry j1 (plane 1), built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the
+                    // exact k * hs.  A step holds the groups of NCS chunks: their hs, c1 = hs, c2 = 2hs (ck 128: once per window).
+                    auto hs_of = [&](int b) {
+                        return __float2half_rn(live ? 0.5f * load_scale(blk + (size_t)b * p.blk_bytes + pf_scale_off(QCH), p.sd, srow) : 0.f);
+                    };
+                    __half hsv[PG::NCS];
+                    uint32_t c1[PG::NCS], c2[PG::NCS];
+                    if constexpr (QCH == 8) {
+                        hsv[0] = hs_of(0);
+                        c1[0] = __half_as_ushort(hsv[0]); c2[0] = __half_as_ushort(__hadd(hsv[0], hsv[0]));
+                    }
+                    const int u0 = (c == c_first) ? (s0 & 1) : 0, u1 = (c == c_last) ? ((s1m - 1) & 1) : 1;   // steps of this window
                     _Pragma("unroll 1") for (int u = u0; u <= u1; ++u) {
+                        if constexpr (QCH != 8) {
+                            _Pragma("unroll") for (int i = 0; i < PG::NCS; ++i) {
+                                hsv[i] = hs_of(u * PG::NCS + i);
+                                c1[i] = __half_as_ushort(hsv[i]); c2[i] = __half_as_ushort(__hadd(hsv[i], hsv[i]));
+                            }
+                        }
                         unsigned char *a_dst = stage_in(f, 2 * c + u);
                         _Pragma("unroll") for (int gl = 0; gl < 16; ++gl) {    // group within the step = 16-byte chunk index
-                            const int gqc = u * 16 + gl;                       // group within the chunk (0..31)
-                            const int q = gqc >> 2, k = gqc & 3;
-                            const uint32_t cw = row_codes<PB>(words + ((size_t)q * 32 + wl) * 4, k, wi);
+                            const int gqc = u * 16 + gl;                       // group within the window (0..31)
+                            // its block in the window (= its chunk in the step: ci) and its quad / word there
+                            const int ci = gl * PG::NCS / 16, b = PG::WB == 1 ? 0 : gqc / (4 * QCH), gb = PG::WB == 1 ? gqc : gqc % (4 * QCH);
+                            const int q = gb >> 2, k = gb & 3;
+                            const uint32_t cw = row_codes<PB>(words + (size_t)b * (p.blk_bytes >> 2) + ((size_t)q * 32 + wl) * 4, k, wi);
                             uint32_t o4[4];
                             if constexpr (PB == 2) {
                                 // cw = j0 | neg0 << 3 | j1 << 4 | neg1 << 7
-                                const uint32_t v0 = (c1 ^ ((cw & 8u) << 12)) << ((cw & 1u) * 16), v1 = (c2 ^ ((cw & 0x80u) << 8)) << (((cw >> 4) & 1u) * 16);
+                                const uint32_t v0 = (c1[ci] ^ ((cw & 8u) << 12)) << ((cw & 1u) * 16), v1 = (c2[ci] ^ ((cw & 0x80u) << 8)) << (((cw >> 4) & 1u) * 16);
                                 _Pragma("unroll") for (int e = 0; e < 4; ++e) {
                                     const uint32_t a = (cw & 6u) == 2u * e ? v0 : 0u, b = (cw & 0x60u) == 32u * e ? v1 : 0u;
                                     const __half2 x = __hadd2(*reinterpret_cast<const __half2 *>(&a), *reinterpret_cast<const __half2 *>(&b));
@@ -221,7 +251,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                                 // k exactly; k and hs are exact fp16 values, so the HMUL2 rounds the exact product k * hs once.
                                 const uint64_t lo = xtab[cw & 0xffu], hi = xtab[256 + (cw >> 8)];
                                 const uint32_t sk[2] = {(uint32_t)lo + (uint32_t)hi, (uint32_t)(lo >> 32) + (uint32_t)(hi >> 32)};
-                                const __half2 hs2 = __halves2half2(hsh, hsh), off = __float2half2_rn(1040.f);
+                                const __half2 hs2 = __halves2half2(hsv[ci], hsv[ci]), off = __float2half2_rn(1040.f);
                                 _Pragma("unroll") for (int e = 0; e < 4; ++e) {
                                     const uint32_t m = __byte_perm(sk[e >> 1], 0x64u, (e & 1) ? 0x4342u : 0x4140u);   // entries 2e, 2e + 1
                                     const __half2 kk = __hsub2(*reinterpret_cast<const __half2 *>(&m), off);
@@ -247,7 +277,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                         const int wg = e * 32 + kc * 2 + u;
                         float hs = 0.f, zz = 0.f;
                         if (live && wg < p.nchunk) {
-                            const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + kPfScaleOff;
+                            const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + pf_scale_off(QCH);
                             hs = 0.5f * load_scale(sp, p.sd, srow);
                             if (p.zp) zz = load_scale(sp + (size_t)RSB * p.sd, p.sd, srow);
                         }

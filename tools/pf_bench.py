@@ -11,6 +11,7 @@ The tile's minimum N is set to the smallest N of the run, so that the tile is ti
     python tools/pf_bench.py --bits 3 --shapes 11008x4096
     python tools/pf_bench.py --bitnet                 # W2 integer path (one scale, act group = K): BitNet-3B 3200x3200, 8640x3200,
                                                       # 3200x8640, N = 16 .. 512
+    python tools/pf_bench.py --bits 4 --group 32 --act-group 32 --sym   # ggml Q4_0's grouping (W4 g32, act group 32)
 
 Rates: dense-equivalent = 2*N*M*K / time; MMA = the tile's tensor-core work (padded to whole 128-row x token tiles, contraction
 2K entries + the fp16 tile's bias columns) / time, against the H100 SXM data-sheet peaks (dense): 989 TFLOP/s fp16, 1979 TOP/s int8.
@@ -33,6 +34,8 @@ ap.add_argument("--ns", default=None, help="comma-separated N; default: 32..512 
 ap.add_argument("--reps", type=int, default=20)
 ap.add_argument("--sym", action="store_true", help="no zero points")
 ap.add_argument("--bitnet", action="store_true", help="W2 integer path: one weight scale, one activation group per row (BitNet)")
+ap.add_argument("--group", type=int, default=128, help="weight group size (the stream layout's chunk is min(group, 128))")
+ap.add_argument("--act-group", type=int, default=64, help="activation group size (<= the chunk)")
 a = ap.parse_args()
 if a.bitnet:
     a.bits, a.sym = 2, True
@@ -62,11 +65,13 @@ def time_us(fn):
 try:
     for M, K in shapes:
         w, sc, z = bench.synth(9, mout=M, k=K, bits=a.bits, zp=not a.sym, one_scale=a.bitnet)
-        ags = K if a.bitnet else 64
-        cfg = tb.make_kcfg(M, K, a.bits, T.default_bm(M * a.bits, a.bits), 16, 128, ags, not a.sym, a.bitnet)
+        ags = K if a.bitnet else a.act_group
+        kfactor = 16 if a.bitnet else ags // 4                   # the reference's tile: kfactor * 4 K positions per activation group
+        cfg = tb.make_kcfg(M, K, a.bits, T.default_bm(M * a.bits, a.bits), kfactor, a.group, ags, not a.sym, a.bitnet)
         wt = tb.upload_plain(cfg, w, sc, z)
         nag = K // ags
-        print("W%d %s %d x %d" % (a.bits, "bitnet (one scale, act group K)" if a.bitnet else "sym" if a.sym else "zp", M, K))
+        print("W%d %s %d x %d" % (a.bits, "bitnet (one scale, act group K)" if a.bitnet else
+                                  "g%d a%d %s" % (a.group, ags, "sym" if a.sym else "zp"), M, K))
         for N in ns:
             x = torch.randn((N, K), device="cuda"); o = torch.zeros((N, M), device="cuda")
             q = torch.zeros((N, K // 4, 16), dtype=torch.int8, device="cuda"); ls = torch.zeros((N, nag), device="cuda"); lb = torch.zeros_like(ls)
@@ -81,8 +86,8 @@ try:
                 dense = 2.0 * N * M * K / us / 1e6
                 if ll["batch"] >= 0:
                     kind, mma = "GEMV", ""
-                elif ll["cluster"] == 16:    # fp16 tile: 256-token tiles, K/64 + ceil(K/128/32) steps of 128 entries
-                    work = 2.0 * ((N + 255) // 256 * 256) * ((M + 127) // 128 * 128) * 128 * (K // 64 + (K // 128 + 31) // 32)
+                elif ll["cluster"] == 16:    # fp16 tile: 256-token tiles, K/64 + ceil(chunks/32) steps of 128 entries
+                    work = 2.0 * ((N + 255) // 256 * 256) * ((M + 127) // 128 * 128) * 128 * (K // 64 + (K // min(a.group, 128) + 31) // 32)
                     kind, mma = "fp16 tile", "  MMA %6.1f TFLOP/s (%4.1f%% of 989)" % (work / us / 1e6, 100.0 * work / us / 1e6 / 989)
                 else:                        # int8 tile: 128-token tiles, contraction 2K bytes
                     work = 2.0 * ((N + 127) // 128 * 128) * ((M + 127) // 128 * 128) * (2 * K)

@@ -4,6 +4,7 @@ fp32, with the LUT-bias / zero-point terms kept exact?  W2 and the 4-plane layou
 and at the Llama-2 / Qwen2 K of 11008 and 18944.  Uses the oracle (TEST INFRASTRUCTURE) as the truth.
 
     python tools/sim_fp16_prefill.py         # 8 tokens, seed 3: max|dC|/max|C| 1.4e-4 (W2) .. 2.7e-4 (W4 512 x 4096 sym); bar 1e-3
+                                             # the other groupings: 1.3e-4 .. 3.1e-4
 """
 import os
 import sys
@@ -15,10 +16,15 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import tmac_oracle as T   # noqa: E402
 
 o = T.load_oracle()
-CASES = [(512, 4096, 2, True), (512, 4096, 4, True), (512, 4096, 4, False), (384, 4096, 3, True), (256, 11008, 4, False),
-         (256, 18944, 4, True), (384, 11008, 3, True)]
-for Mout, Kc, bits, zp in CASES:
-    cfg = T.Config(Mout, Kc, bits, zero_point=zp).resolved()
+# (Mout, K, bits, zero points, group size, act group size): g128 / a64, then the other groupings the tiles take
+CASES = [(512, 4096, 2, True, 128, 64), (512, 4096, 4, True, 128, 64), (512, 4096, 4, False, 128, 64), (384, 4096, 3, True, 128, 64),
+         (256, 11008, 4, False, 128, 64), (256, 18944, 4, True, 128, 64), (384, 11008, 3, True, 128, 64),
+         (512, 4096, 4, False, 32, 32), (256, 11008, 4, False, 32, 32), (384, 4096, 3, True, 32, 32), (512, 4096, 2, True, 64, 64),
+         (512, 4096, 2, True, 64, 32), (512, 4096, 4, True, 128, 32), (512, 4096, 4, True, 128, 128), (512, 4096, 2, True, 128, 128),
+         (256, 11008, 4, True, 128, 128)]
+for Mout, Kc, bits, zp, gs_, ags_ in CASES:
+    # the reference's kfactor is ags / 4 (16 for ags 64); with kfactor 16 at ags 128 its packing describes another problem
+    cfg = T.Config(Mout, Kc, bits, kfactor=ags_ // 4, group_size=gs_, act_group_size=ags_, zero_point=zp).resolved()
     N = 8
     w, sc, z, x = T.make_problem(cfg, seed=3, N=N)
     A, S_ = T.pack_reference_layout(w, sc, z, cfg)
@@ -40,5 +46,5 @@ for Mout, Kc, bits, zp in CASES:
     LB = lb.reshape(N, K // gs, gs // ags).sum(-1)
     rest = LB.astype(np.float64) @ (0.5 * sc + (z if zp else 0.0)).astype(np.float64).T
     C = (Bop @ Aop.T).astype(np.float64) + rest
-    print("W%d %4d x %5d %-3s fp16 operands, fp32 accumulate: max|dC|/max|C| = %.2e   nmse %.2e"
-          % (bits, M, K, "zp" if zp else "sym", np.abs(C - Cref).max() / np.abs(Cref).max(), T.nmse(Cref, C.astype(np.float32))))
+    print("W%d g%-3d a%-3d %4d x %5d %-3s fp16 operands, fp32 accumulate: max|dC|/max|C| = %.2e   nmse %.2e"
+          % (bits, gs, ags, M, K, "zp" if zp else "sym", np.abs(C - Cref).max() / np.abs(Cref).max(), T.nmse(Cref, C.astype(np.float32))))
