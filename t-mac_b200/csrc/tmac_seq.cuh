@@ -87,9 +87,10 @@ __device__ __forceinline__ void seq_publish(uint2 *slot, uint32_t bits, uint32_t
 }
 // Waiting for N = 1, 2 or 4 consecutive {value, epoch} words at src per active lane; val = their values (0 in inactive lanes and
 // after LIMIT polls: error `code`), separate references because an array or a returned vector changes chain_kernel's SASS.  While
-// some are stale only the lowest stale lane polls the epoch of its first word (all 640 threads of all CTAs polling would take
-// ~5 KB of L2 bandwidth per cycle and starve the very stores they wait for), then the stale lanes reload all their words.  All
-// 32 lanes must call.
+// some are stale, every stale lane reloads all its words, so the round trip that sees the last epoch also brings the values.
+// (Polling one lane's first epoch and then reloading costs a second L2 round trip per wait after the data has landed: on an H100
+// that made the dependent bench chain 0.18 us per GEMV slower, and seq_kernel 0.67; the extra poll traffic did not show.)  All 32
+// lanes must call.
 template <int LIMIT, typename... F>
 __device__ __forceinline__ void wait_words(const uint2 *src, bool active, uint32_t epoch, int *err, int code, F &...val) {
     constexpr int N = sizeof...(F);
@@ -104,15 +105,8 @@ __device__ __forceinline__ void wait_words(const uint2 *src, bool active, uint32
     int spins = 0;
     for (;;) {
         const bool stale = active && (v0.y != epoch || v0.w != epoch || v1.y != epoch || v1.w != epoch);
-        const unsigned m = __ballot_sync(0xffffffffu, stale);
-        if (m == 0) break;
-        const int leader = __ffs(m) - 1;
-        if ((int)(threadIdx.x & 31) == leader) {
-            uint32_t e;
-            do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(e) : "l"(reinterpret_cast<const uint32_t *>(src) + 1) : "memory"); } while (e != epoch && ++spins < LIMIT);
-        }
-        spins = __shfl_sync(0xffffffffu, spins, leader);
-        if (spins >= LIMIT) { if ((threadIdx.x & 31) == 0) atomicExch(err, code); v0.x = v0.z = v1.x = v1.z = 0u; break; }
+        if (__ballot_sync(0xffffffffu, stale) == 0) break;
+        if (++spins >= LIMIT) { if ((threadIdx.x & 31) == 0) atomicExch(err, code); v0.x = v0.z = v1.x = v1.z = 0u; break; }
         if (stale) load();
     }
     const float w[4] = {__uint_as_float(v0.x), __uint_as_float(v0.z), __uint_as_float(v1.x), __uint_as_float(v1.z)};

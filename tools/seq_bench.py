@@ -66,18 +66,25 @@ def chain_trace(seq):
     if args.dump:
         np.save(args.dump, raw)
     t = raw.astype(np.float64) / 1e3
-    names = ["top->barrier seen", "syncthreads", "input wait + LUT slice", "block wait", "lookups", "red sync", "CTA sums + send (barrier form: cluster sync)", "leader: partials landed, sum, publish"]
     ops = slice(2, None)
     def fmt(a):
         return "%.2f/%.2f/%.2f" % (np.median(a), np.percentile(a, 90), a.max())
     flow = bool(t[ops, :, 1].max() == 0)          # data-flow mode: no barrier stamps
-    for k, nme in enumerate(names):
-        if flow and k < 2:
-            continue
-        a = t[ops, :, k + 1] - t[ops, :, k]
-        if k == 7:
-            a = a[:, ::8]
+    phases = [(2, 3, "input wait + LUT slice"), (3, 4, "block wait"), (4, 5, "lookups"),
+              (5, 6, "buffer guard + red sync" if flow else "red sync"),
+              (6, 7, "CTA sums + send" if flow else "CTA sums + cluster sync"),
+              (7, 8, "leader: partials landed, sum, publish" if flow else "leader: sum, publish")]
+    if not flow:
+        phases = [(0, 1, "top->barrier seen"), (1, 2, "syncthreads")] + phases
+    leaders = t[:, ::4, 8] > 0                    # (op, cluster) with published rows: stamp 8 is the leader's
+    for k0, k1, nme in phases:
+        a = t[ops, :, k1] - t[ops, :, k0]
+        if k1 == 8:
+            a = a[:, ::4][leaders[ops]]
         print("    %-30s median/p90/max us: %s" % (nme, fmt(a)))
+    # stamp 6 follows the CTA barrier after its 4 warps' lookups: the cluster's latest one starts the tail of the reduction
+    last = t[:, :, 6].reshape(t.shape[0], -1, 4).max(axis=2)
+    print("    last CTA barrier of the cluster -> rows published median/p90/max us: %s" % fmt((t[:, ::4, 8] - last)[ops][leaders[ops]]))
     end = np.where(t[:, :, 8] > 0, t[:, :, 8], t[:, :, 7])
     per = np.diff(end.max(axis=1))
     if flow:
