@@ -16,7 +16,8 @@
 //     activations -- so the stream overlaps the ALU-bound phase and is out of the way of the latency-critical words (requesting
 //     earlier, across the hand-over, puts 12.7 MB of bulk traffic in front of the words everybody waits for).  With nstage =
 //     bpw + 1 every block is requested one full op before it is consumed; the host picks the deepest ring that keeps every
-//     cluster resident;
+//     cluster resident.  The copies carry an L2 evict_first policy: a block is read once per launch, and its lines should leave
+//     L2 before the {value, epoch} words, inputs and outputs that the ops after it read;
 //   * CTA placement is fixed for the whole chain (344 CTAs of 128 threads for 11008 rows, all resident).
 // bench.py times it on the bench chain (32 x 11008x4096 W2, x[i+1] = first K outputs of op i) beside the launch chain and
 // tmac_seq.cuh; flags bit 0 selects the grid-barrier form this kernel started as, kept for comparison.  Per-phase stamps
@@ -164,7 +165,8 @@ __global__ void __launch_bounds__(kChainWarps * 32, QD ? 3 : 5) chain_kernel(con
         if (!nw) return;
         if (lane == 0) {
             fence_proxy_async();
-            bulk_load(stage0 + (size_t)rs * p.max_blk, nw + (size_t)rsb * nstride + (size_t)nc * nbytes, (uint32_t)nbytes, mbar + rs);
+            bulk_load_hint(stage0 + (size_t)rs * p.max_blk, nw + (size_t)rsb * nstride + (size_t)nc * nbytes, (uint32_t)nbytes, mbar + rs,
+                           policy_evict_first());
         }
         if (++rs == NS) rs = 0;
         advance();

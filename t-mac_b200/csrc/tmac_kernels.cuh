@@ -24,7 +24,7 @@
 //                          its weight part (QuadWord, quad_decode -> QuadCodes) and table part (Quad<PB, SYM>::lookup,
 //                          TMAC_QUAD_TABLE), which chain_kernel runs apart (TMAC_BLOCK_LOOKUPS_AHEAD);
 //   PTX wrappers         : smem_u32, mbar_init, mbar_fence_init, fence_proxy_async, mbar_arrive, expect_tx, bulk_load,
-//                          mbar_wait_parity, mbar_wait_bounded<LIMIT>, cluster_arrive_relaxed / cluster_wait, globaltimer_ns;
+//                          bulk_load_hint, mbar_wait_parity, mbar_wait_bounded<LIMIT>, cluster_arrive_relaxed / cluster_wait, globaltimer_ns;
 //   the output store     : store_out (fp16 or fp32).
 #pragma once
 #include <cuda_fp16.h>
@@ -542,6 +542,12 @@ __device__ __forceinline__ void bulk_load(void *smem_dst, const void *gsrc, uint
     expect_tx(bar, bytes);
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// bulk_load with an L2 eviction policy for the copied lines (policy_evict_first: data read once)
+__device__ __forceinline__ void bulk_load_hint(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar, uint64_t pol) {
+    expect_tx(bar, bytes);
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void mbar_wait_parity(uint64_t *b, uint32_t parity) {
     asm volatile(

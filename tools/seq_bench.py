@@ -1,7 +1,10 @@
 """Time the decode sequence kernel on the bench workload (32 distinct 11008x4096 W2 g128 zp tensors):
 independent inputs vs a true dependency chain (x_{i+1} = first K outputs of op i); optional per-op timeline.
 
-    python tools/seq_bench.py [--trace] [--layers 32] [--reps 20]
+    python tools/seq_bench.py [--trace] [--layers 32] [--reps 20] [--distinct N]
+
+--distinct N: the ops cycle over N distinct resident tensors (op i runs tensor i % N).  At N = 2 the chain's weights (25 MB)
+stay in the H100's 50 MB L2, so the chain runs without the HBM weight stream: the bound that the stream sets on the op period.
 """
 import argparse
 import os
@@ -19,6 +22,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--trace", action="store_true")
 ap.add_argument("--layers", type=int, default=32)
 ap.add_argument("--reps", type=int, default=20)
+ap.add_argument("--distinct", type=int, default=0, help="distinct tensors the ops cycle over (0 = one per op)")
 ap.add_argument("--bits", type=int, default=2)
 ap.add_argument("--mout", type=int, default=bench.MOUT)
 ap.add_argument("--k", type=int, default=bench.K)
@@ -40,7 +44,9 @@ w, sc, z = bench.synth(100, args.mout, args.k, args.bits, 128, True, False)
 bm = 256 if (args.mout * args.bits) % 256 == 0 else 128
 cfg = tb.make_kcfg(args.mout, args.k, args.bits, bm, 16, 128, 64, True, False)
 base = tb.upload_plain(cfg, w, sc, z)
-layers = [base] + [tb.clone(base) for _ in range(L - 1)]
+nd = args.distinct if args.distinct > 0 else L
+tensors = [base] + [tb.clone(base) for _ in range(min(nd, L) - 1)]
+layers = [tensors[i % len(tensors)] for i in range(L)]
 x = torch.randn((L, args.k), device="cuda").half().float()
 out = torch.zeros((L, args.mout), device="cuda")
 abytes = bench.algorithmic_bytes(args.mout, args.k, args.bits, 128, True)
