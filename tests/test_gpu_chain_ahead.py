@@ -6,136 +6,65 @@ Decode-ahead moves only work that reads the weight block; the integer lookups ar
 output must be bit for bit the same.  A sequence whose clusters need more than 3 CTAs per SM cannot run the decode-ahead
 instantiation (bounded to 3 CTAs per SM for its registers): its build takes the other one, and it must still be the chain.
 kfactor = act_group_size / 4 everywhere: the oracle (like the reference) is only right then."""
-import contextlib
-
 import numpy as np
 import pytest
 
 import tmac_b200 as tb
-import tmac_oracle as T
-from seq_util import kc, oracle_gemv
+from seq_util import TIGHT_TOL, glu, inputs, mk, oracle_gemv, run_form, same_bits, step, stream
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-TIGHT_TOL = 2e-5        # max |got - oracle| / max |oracle|
-CHAIN_RING = -4         # info()["ring_slots"] of a sequence served by the resident chain kernel (-kChainCS)
 
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
-    torch.cuda.set_stream(torch.cuda.default_stream())
-
-
-class Op:
-    def __init__(self, Mout, K, bits, g=128, ags=64, zp=True, seed=0):
-        self.cfg = cfg = T.Config(Mout, K, bits, kfactor=ags // 4, group_size=g, act_group_size=ags, zero_point=zp).resolved()
-        w, sc, z, _ = T.make_problem(cfg, seed=seed)
-        self.A, self.S = T.pack_reference_layout(w, sc, z, cfg)
-        self.wt = tb.upload_reference_layout(kc(cfg), self.A, self.S)
-
-
-@pytest.fixture
-def mk(stream):
-    made = []
-
-    def make(*a, **k):
-        made.append(Op(*a, **k))
-        return made[-1]
-    yield make
-    for o in made:
-        o.wt.free()
-
-
-@contextlib.contextmanager
-def chain_form(ahead):
+def run(steps, ext, ahead):
+    """Builds the sequence as the resident chain, with (ahead = 1) or without decode-ahead, and launches it twice; returns
+    (info, outputs)."""
     try:
-        tb.debug_set("seq_impl", 1); tb.debug_set("chain_flags", 0); tb.debug_set("chain_ahead", ahead)
-        yield
+        tb.debug_set("chain_ahead", ahead)
+        return run_form("flow", steps, ext, launches=2)
     finally:
-        tb.debug_set("seq_impl", 2); tb.debug_set("chain_ahead", 1)
+        tb.debug_set("chain_ahead", 1)
 
 
-def run(steps, x, ahead, launches=2):
-    """steps[i] = (op, src): src None = the external input x, an int = that earlier step's outputs from row 0, a pair (g, u) = the
-    GLU input silu(g) * u of two earlier steps.  Builds the sequence as the resident chain; returns (info, outputs)."""
-    with chain_form(ahead):
-        seq = tb.Sequence()
-        try:
-            outs = []
-            for o, src in steps:
-                out = torch.full((o.cfg.Mout,), float("nan"), device="cuda")
-                if src is None:
-                    seq.add(o.wt, x=x, out=out)
-                elif isinstance(src, tuple):
-                    seq.add_glu(o.wt, src[0], 0, src[1], 0, out=out)
-                else:
-                    seq.add(o.wt, in_op=src, in_offset=0, out=out)
-                outs.append(out)
-            seq.build()
-            info = seq.info()
-            assert info["ring_slots"] == CHAIN_RING, info
-            for _ in range(launches):
-                seq.launch()
-            seq.status()
-            return info, [o.cpu().numpy() for o in outs]
-        finally:
-            seq.free()
-
-
-def same_both_ways(steps, x):
+def same_both_ways(steps, ext):
     """The chain with and without decode-ahead: same ring, bit-identical outputs.  Returns the outputs."""
-    info_a, got_a = run(steps, x, 1)
-    info_p, got_p = run(steps, x, 0)
+    info_a, got_a = run(steps, ext, 1)
+    info_p, got_p = run(steps, ext, 0)
     assert info_a == info_p
     for i, (a, p) in enumerate(zip(got_a, got_p)):
         assert np.isfinite(a).all(), "op %d" % i
-        assert np.array_equal(a.view(np.uint32), p.view(np.uint32)), "op %d differs with decode-ahead" % i
+        assert same_bits(a, p), "op %d differs with decode-ahead" % i
     return got_a
 
 
-def check(oracle, steps, x0, got, ops=None):
-    for i, (o, src) in enumerate(steps):
+def check(oracle, steps, xs, got, ops=None):
+    for i, (o, src, off, *_) in enumerate(steps):
         if ops is not None and i not in ops:
             continue
-        x = x0 if src is None else got[src][:o.cfg.K].astype(np.float32)
+        x = xs[src] if isinstance(src, str) else got[src][off:off + o.cfg.K].astype(np.float32)
         ref = oracle_gemv(oracle, o.cfg, o.A, o.S, x)
         err = np.abs(got[i] - ref).max() / np.abs(ref).max()
         assert err <= TIGHT_TOL, "op %d (%dx%d W%d): rel err %.3g" % (i, o.cfg.Mout, o.cfg.K, o.cfg.bits, err)
 
 
-def ext_input(n, seed):
-    x = np.random.default_rng(seed).standard_normal(n).astype(np.float16).astype(np.float32)
-    return x, torch.from_numpy(x).cuda()
-
-
 def test_bench_chain(oracle, mk):
     """The bench shape (11008x4096 W2 g128 zp, 2 blocks per warp), 8 dependent ops (the bench runs 32 of them)."""
-    base = mk(11008, 4096, 2, seed=1)
-    steps = [(base, None)]
+    base = mk(11008, 4096, 2, zp=True, seed=1)
+    steps = [step(base, "x")]
     for i in range(1, 8):
-        steps.append((mk(11008, 4096, 2, seed=1 + i), i - 1))
-    x, dx = ext_input(4096, 1)
-    got = same_both_ways(steps, dx)
-    check(oracle, steps, x, got, ops=(0, 1, 7))
+        steps.append(step(mk(11008, 4096, 2, zp=True, seed=1 + i), i - 1))
+    xs, ext = inputs(np.random.default_rng(1), x=4096)
+    got = same_both_ways(steps, ext)
+    check(oracle, steps, xs, got, ops=(0, 1, 7))
 
 
 def test_glu_chain(oracle, mk):
     """A SwiGLU FFN: gate and up, then down reading silu(gate) * up (the GLU instantiation)."""
-    steps = [(mk(2048, 1024, 2, seed=11), None), (mk(2048, 1024, 2, seed=12), None), (mk(1024, 2048, 2, seed=13), (0, 1))]
-    x, dx = ext_input(1024, 2)
-    got = same_both_ways(steps, dx)
-    check(oracle, steps, x, got, ops=(0, 1))
+    steps = [step(mk(2048, 1024, 2, zp=True, seed=11), "x"), step(mk(2048, 1024, 2, zp=True, seed=12), "x"),
+             step(mk(1024, 2048, 2, zp=True, seed=13), glu(0, 0, 1, 0))]
+    xs, ext = inputs(np.random.default_rng(2), x=1024)
+    got = same_both_ways(steps, ext)
+    check(oracle, steps, xs, got, ops=(0, 1))
 
 
 @pytest.mark.parametrize("bits,g,ags", [(2, 128, 64), (4, 128, 128), (1, 64, 32), (3, 32, 32)])
@@ -145,10 +74,11 @@ def test_one_two_and_six_blocks_per_warp(oracle, mk, bits, g, ags):
     op has 172 clusters (688 CTAs, 6 per SM on 132 SMs): both builds take the instantiation without decode-ahead, which must keep
     fitting 6 CTAs per SM."""
     kw = dict(g=g, ags=ags, zp=bits in (2, 3))
-    steps = [(mk(11008, 2048, bits, seed=21, **kw), None), (mk(4096, 11008, bits, seed=22, **kw), 0), (mk(512, 4096, bits, seed=23, **kw), 1)]
-    x, dx = ext_input(2048, bits)
-    got = same_both_ways(steps, dx)
-    check(oracle, steps, x, got)
+    steps = [step(mk(11008, 2048, bits, seed=21, **kw), "x"), step(mk(4096, 11008, bits, seed=22, **kw), 0),
+             step(mk(512, 4096, bits, seed=23, **kw), 1)]
+    xs, ext = inputs(np.random.default_rng(bits), x=2048)
+    got = same_both_ways(steps, ext)
+    check(oracle, steps, xs, got)
 
 
 def test_sequence_too_large_for_three_ctas_per_sm(oracle, mk, stream):
@@ -156,7 +86,7 @@ def test_sequence_too_large_for_three_ctas_per_sm(oracle, mk, stream):
     back to the instantiation without decode-ahead and the sequence is still the resident chain, correct and the same bits."""
     if 3 * torch.cuda.get_device_properties(0).multi_processor_count >= 592:
         pytest.skip("592 CTAs fit at 3 per SM on this device")
-    steps = [(mk(18944, 2048, 2, seed=31), None), (mk(512, 2048, 2, seed=32), 0)]
-    x, dx = ext_input(2048, 3)
-    got = same_both_ways(steps, dx)
-    check(oracle, steps, x, got)
+    steps = [step(mk(18944, 2048, 2, zp=True, seed=31), "x"), step(mk(512, 2048, 2, zp=True, seed=32), 0)]
+    xs, ext = inputs(np.random.default_rng(3), x=2048)
+    got = same_both_ways(steps, ext)
+    check(oracle, steps, xs, got)

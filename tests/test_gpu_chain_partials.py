@@ -4,7 +4,8 @@ long enough for that state to wrap many times in one launch; both chain forms mu
 import numpy as np
 import pytest
 
-from test_gpu_chain import check, inputs, mk, run_form, same_bits, stream  # noqa: F401 (fixtures)
+from seq_util import inputs, mk, run_form, same_bits, step, stream  # noqa: F401 (fixtures)
+from test_gpu_chain import check
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -24,7 +25,7 @@ def test_alternating_row_counts(oracle, mk):
     kw = dict(zp=True)
     a, b = mk(1024, 512, 2, seed=91, **kw), mk(512, 512, 2, seed=92, **kw)
     order = [a, b, a, b, b, a, b, a, a, b]
-    steps = [(o, "x0" if i == 0 else i - 1, 0) for i, o in enumerate(order)]
+    steps = [step(o, "x0" if i == 0 else i - 1) for i, o in enumerate(order)]
     xs, ext = inputs(np.random.default_rng(12), x0=512)
     both_forms(oracle, steps, xs, ext)
 
@@ -33,6 +34,6 @@ def test_long_sequence_in_one_launch(oracle, mk):
     """72 ops in one launch: every other op reads its predecessor, the rest a fresh input, so values stay in range."""
     kw = dict(zp=True)
     a, b = mk(512, 256, 2, seed=93, **kw), mk(256, 512, 2, seed=94, **kw)
-    steps = [(b, "x0", 0) if i % 2 == 0 else (a, i - 1, 0) for i in range(72)]
+    steps = [step(b, "x0") if i % 2 == 0 else step(a, i - 1) for i in range(72)]
     xs, ext = inputs(np.random.default_rng(13), x0=512)
     both_forms(oracle, steps, xs, ext)

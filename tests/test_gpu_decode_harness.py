@@ -2,27 +2,12 @@
 through the library must match the same layer with dense dequantised fp32 weights (torch matmul) within the reference's own
 gate for this path, NMSE <= 5e-4 (python/t_mac/ops/qgemm.py:277-282) -- the remaining difference is the int8 LUT quantisation
 noise the CPU kernel has too.  Also: the CUDA-graphed token step of a small model replays to the same output as the eager step."""
-import numpy as np
 import pytest
 
-import tmac_b200 as tb
+from seq_util import stream
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
 
 
 @pytest.mark.parametrize("bits,zp", [(2, True), (4, False)], ids=["w2zp", "w4"])

@@ -18,7 +18,7 @@ import pytest
 import tmac_b200 as tb
 import tmac_oracle as T
 from act_rows import KINDS, KINDS16, rows, rows16
-from seq_util import kc
+from seq_util import CHAIN_RING, kc, same_bits
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -26,7 +26,6 @@ pytestmark = pytest.mark.gpu
 TIGHT_TOL = 2e-5        # fp path: max |got - oracle| / max |oracle|, per activation row
 P16_TOL = 5e-4          # the fp16-operand prefill tile (test_gpu_parity.py)
 DENSE_NMSE = 5e-4       # against the float64 dense dequantised GEMV
-CHAIN_RING = -4         # info()["ring_slots"] of a sequence served by the resident chain kernel (-kChainCS)
 
 
 @pytest.fixture(scope="module")
@@ -57,11 +56,6 @@ def raw(a):
     """The bytes of a numpy array or tensor as unsigned integers of its element size."""
     a = np.ascontiguousarray(a.cpu().numpy() if hasattr(a, "cpu") else a)
     return a.view({1: np.uint8, 2: np.uint16, 4: np.uint32}[a.dtype.itemsize])
-
-
-def same_bits(a, b):
-    a, b = raw(a), raw(b)
-    return a.shape == b.shape and np.array_equal(a, b)
 
 
 def assert_rows_close(got, ref, tol, what):

@@ -11,69 +11,10 @@ import pytest
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
-from seq_util import kc
+from seq_util import A_CASES, A_IDS, EPS, kc, mk, norm_weight, rms_input, same_bits, stream
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
-
-EPS = 1e-5
-
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
-    torch.cuda.set_stream(torch.cuda.default_stream())
-
-
-class Op:
-    """One uploaded tensor in the reference layout."""
-
-    def __init__(self, Mout, K, bits, g=128, ags=64, zp=False, seed=0):
-        self.cfg = cfg = T.Config(Mout, K, bits, kfactor=ags // 4, group_size=g, act_group_size=ags, zero_point=zp).resolved()
-        w, sc, z, _ = T.make_problem(cfg, seed=seed)
-        self.A, self.S = T.pack_reference_layout(w, sc, z, cfg)
-        self.wt = tb.upload_reference_layout(kc(cfg), self.A, self.S)
-        self.Mout, self.K = Mout, K
-
-
-@pytest.fixture
-def mk(stream):
-    made = []
-
-    def make(*a, **k):
-        made.append(Op(*a, **k))
-        return made[-1]
-    yield make
-    for o in made:
-        o.wt.free()
-
-
-def rms_input(h, w, eps):
-    """The norm input a of each row of h [N][K], in numpy float32 in the documented order: lane l sums the 4-element groups l, l + 32,
-    ... in ascending order as (h0*h0 + h1*h1) + (h2*h2 + h3*h3), the 32 lane sums meet in the shfl_xor butterfly 16, 8, 4, 2, 1."""
-    out = []
-    for row in np.asarray(h, np.float32).reshape(-1, np.shape(h)[-1]):
-        K = row.size
-        g = row.reshape(-1, 4)
-        q = (g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1]) + (g[:, 2] * g[:, 2] + g[:, 3] * g[:, 3])
-        q = np.concatenate([q, np.zeros(-len(q) % 32, np.float32)]).reshape(-1, 32)
-        s = np.zeros(32, np.float32)
-        for part in q:
-            s = s + part
-        for m in (16, 8, 4, 2, 1):
-            s = s + s[np.arange(32) ^ m]
-        inv = np.float32(1.0) / np.sqrt(s[0] / np.float32(K) + np.float32(eps))
-        out.append((row * inv) * np.asarray(w, np.float32))
-    return np.stack(out)
 
 
 def dev(x, dtype=torch.float32):
@@ -86,7 +27,7 @@ def nan_out(N, M, dtype=torch.float32):
 
 def grouped(ops, N, a):
     """gemv_grouped of the tensors on the fp32 input a (device [N][K]): the outputs as numpy float32."""
-    outs = [nan_out(N, o.Mout) for o in ops]
+    outs = [nan_out(N, o.cfg.Mout) for o in ops]
     tb.gemv_grouped([o.wt for o in ops], N, a, outs)
     torch.cuda.synchronize()
     return [x.cpu().numpy() for x in outs]
@@ -96,10 +37,6 @@ def glu_ref(G, U):
     """The GLU input on the GPU from device tensors G, U (fp32 or fp16, widened)."""
     g, u = G.float(), U.float()
     return g / (1 + torch.exp(-g)) * u
-
-
-def same_bits(a, b):
-    return a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
 
 
 def expect(got, want32, res=None, f16=False, what=""):
@@ -116,7 +53,7 @@ def check_norm(ops, N, H, w, eps=EPS, dtype=torch.float32):
     """gemv_rmsnorm of the tensors on H (host [N][K] float32, passed as dtype) against gemv_grouped on rms_input."""
     f16 = dtype == torch.float16
     dH = dev(H, dtype)
-    outs = [nan_out(N, o.Mout, dtype) for o in ops]
+    outs = [nan_out(N, o.cfg.Mout, dtype) for o in ops]
     tb.gemv_rmsnorm([o.wt for o in ops], N, dH, dev(w), eps, outs, dtype=tb.F16 if f16 else tb.F32)
     launch = tb.last_launch()
     torch.cuda.synchronize()
@@ -130,7 +67,7 @@ def check_glu(op, N, G, U, R=None, dtype=torch.float32):
     f16 = dtype == torch.float16
     dG, dU = dev(G, dtype), dev(U, dtype)
     dR = None if R is None else dev(R, dtype)
-    out = nan_out(N, op.Mout, dtype)
+    out = nan_out(N, op.cfg.Mout, dtype)
     tb.gemv_glu(op.wt, N, dG, dU, out, R=dR, dtype=tb.F16 if f16 else tb.F32)
     ref = grouped([op], N, glu_ref(dG, dU))[0]
     expect(out, ref, None if dR is None else dR.float().cpu().numpy(), f16, "gemv_glu")
@@ -139,18 +76,10 @@ def check_glu(op, N, G, U, R=None, dtype=torch.float32):
 def check_residual(op, N, B, R, dtype=torch.float32):
     f16 = dtype == torch.float16
     dB, dR = dev(B, dtype), dev(R, dtype)
-    out = nan_out(N, op.Mout, dtype)
+    out = nan_out(N, op.cfg.Mout, dtype)
     tb.gemv_residual(op.wt, N, dB, dR, out, dtype=tb.F16 if f16 else tb.F32)
     ref = grouped([op], N, dB.float())[0]
     expect(out, ref, dR.float().cpu().numpy(), f16, "gemv_residual")
-
-
-def norm_weight(rng, K):
-    """Norm weights around 1 with zeros and negative values."""
-    w = (1.0 + 0.2 * rng.standard_normal(K)).astype(np.float32)
-    w[rng.integers(0, K, size=K // 16)] = 0.0
-    w[rng.integers(0, K, size=K // 16)] *= -1.0
-    return w
 
 
 def normal(rng, *shape):
@@ -158,12 +87,8 @@ def normal(rng, *shape):
 
 
 # ---- 1: every chunking ------------------------------------------------------------------------------------------------------------
-CHUNKINGS = [(128, 128), (128, 64), (128, 32), (64, 64), (64, 32), (32, 32), (256, 64)]    # (group_size, act_group_size)
-CASES = [(g, a, b, b == 2) for g, a in CHUNKINGS for b in (1, 2, 4)] + [(128, 64, 3, True)]
-
-
 @pytest.mark.parametrize("N", [1, 3])
-@pytest.mark.parametrize("g,ags,bits,zp", CASES, ids=["g%d-ags%d-w%d%s" % (g, a, b, "zp" if z else "") for g, a, b, z in CASES])
+@pytest.mark.parametrize("g,ags,bits,zp", A_CASES, ids=A_IDS)
 def test_every_chunking(mk, g, ags, bits, zp, N):
     K = 20 * min(g, 128)                          # 20 chunks: some warps hold 2 blocks, some 1
     ops = [mk(768, K, bits, g=g, ags=ags, zp=zp, seed=s) for s in (1, 2)]

@@ -4,7 +4,6 @@ chain kernel, from small chains at every chunking to a decoder layer's half afte
 The batch kernel decodes each weight block once and runs each row's table part, folds and scales in the one-row kernel's order, so
 every check is first bit for bit: row t of every output must equal the same sequence built with one row and fed row t.  Rows are
 also checked against the oracle.  kfactor = act_group_size / 4 everywhere: the oracle (like the reference) is only right then."""
-import contextlib
 from types import SimpleNamespace
 
 import numpy as np
@@ -12,105 +11,11 @@ import pytest
 
 import tmac_b200 as tb
 import tmac_oracle as T
-from seq_util import kc, oracle_gemv
+from seq_util import (A_CASES, A_IDS, TIGHT_TOL, device, expect_kernel, fetch, form, glu, host, kc, mk, norm, norm_weight,
+                      oracle_gemv, run_form, same_bits, sequence, step, stream)
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
-
-TIGHT_TOL = 2e-5        # max |got - oracle| / max |oracle|, as the chain tests
-CHAIN_RING = -4         # info()["ring_slots"] of a sequence served by the resident chain kernel (-kChainCS)
-EPS = 1e-5
-
-# (seq_impl, chain_flags, seq_grid)
-FORMS = {"flow": (1, 0, 0), "barrier": (1, 1, 0), "auto": (2, 0, 0)}
-
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
-    torch.cuda.set_stream(torch.cuda.default_stream())
-
-
-class Op:
-    """One uploaded tensor and the problem it was made from (for the oracle)."""
-
-    def __init__(self, Mout, K, bits, g=128, ags=64, zp=False, seed=0):
-        self.cfg = cfg = T.Config(Mout, K, bits, kfactor=ags // 4, group_size=g, act_group_size=ags, zero_point=zp).resolved()
-        self.w, self.sc, self.z, _ = T.make_problem(cfg, seed=seed)
-        self.A, self.S = T.pack_reference_layout(self.w, self.sc, self.z, cfg)
-        self.wt = tb.upload_reference_layout(kc(cfg), self.A, self.S)
-
-
-@pytest.fixture
-def mk(stream):
-    made = []
-
-    def make(*a, **k):
-        made.append(Op(*a, **k))
-        return made[-1]
-    yield make
-    for o in made:
-        o.wt.free()
-
-
-@contextlib.contextmanager
-def form(name):
-    impl, flags, grid = FORMS[name]
-    try:
-        tb.debug_set("seq_impl", impl); tb.debug_set("chain_flags", flags); tb.debug_set("seq_grid", grid)
-        yield
-    finally:
-        tb.debug_set("seq_impl", 2); tb.debug_set("chain_flags", 0); tb.debug_set("seq_grid", 0)
-
-
-# A step: (op, src, off, res, f16).  src: the name of an external input | the index of an earlier op (its rows [off, off + K)) |
-# ("glu", gate_op, up_op) | ("norm", in_op, weight name).  res: None | external name | earlier op index.
-def step(op, src, off=0, res=None, f16=False):
-    return (op, src, off, res, f16)
-
-
-@contextlib.contextmanager
-def sequence(steps, ext, n, explicit=False):
-    """Builds the sequence for n rows; ext maps names to device tensors ([n][len] per-row vectors, [len] norm weights).  Every
-    output is observed, [n][Mout].  explicit: tmac_b200_seq_set_batch is called even for n = 1."""
-    seq = tb.Sequence(n)
-    try:
-        if explicit:
-            tb.check(tb.load().tmac_b200_seq_set_batch(seq.h, n), "tmac_b200_seq_set_batch")
-        outs = []
-        for i, (o, src, off, res, f16) in enumerate(steps):
-            out = torch.full((n, o.cfg.Mout), float("nan"), device="cuda", dtype=torch.float16 if f16 else torch.float32)
-            d = tb.F16 if f16 else tb.F32
-            if isinstance(src, str):
-                seq.add(o.wt, x=ext[src], out=out, dtype=d)
-            elif isinstance(src, int):
-                seq.add(o.wt, in_op=src, in_offset=off, out=out, dtype=d)
-            elif src[0] == "glu":
-                seq.add_glu(o.wt, src[1], off, src[2], off, out=out, dtype=d)
-            else:
-                seq.add_rmsnorm(o.wt, src[1], ext[src[2]], EPS, out=out, dtype=d)
-            if isinstance(res, str):
-                seq.residual(i, r=ext[res])
-            elif res is not None:
-                seq.residual(i, r_op=res)
-            outs.append(out)
-        seq.build()
-        yield seq, outs
-    finally:
-        seq.free()
-
-
-def device(hx):
-    return {k: torch.from_numpy(np.ascontiguousarray(v, np.float32)).cuda() for k, v in hx.items()}
 
 
 def row_of(hx, t):
@@ -120,21 +25,13 @@ def row_of(hx, t):
 
 def run(name, steps, hx, n, explicit=False):
     """Builds and launches the sequence in form `name` on the host inputs hx; asserts that the resident chain serves it.  Returns
-    the outputs as numpy arrays [n][Mout]."""
-    with form(name), sequence(steps, device(hx), n, explicit) as (seq, outs):
-        assert seq.info()["ring_slots"] == CHAIN_RING, seq.info()
-        seq.launch()
-        seq.status()
-        return [o.cpu().numpy() for o in outs]
+    the outputs as numpy arrays, [n][Mout] for n > 1."""
+    return run_form(name, steps, device(hx), chained=True, n=n, explicit_batch=explicit)[1]
 
 
 def singles(name, steps, hx, n):
     """[row t][op]: the one-row sequence fed row t."""
-    return [[o[0] for o in run(name, steps, row_of(hx, t), 1)] for t in range(n)]
-
-
-def same_bits(a, b):
-    return a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
+    return [run(name, steps, row_of(hx, t), 1) for t in range(n)]
 
 
 def check_rows(got, ones, what):
@@ -155,22 +52,7 @@ def check_oracle(oracle, steps, hx, got):
             assert err <= TIGHT_TOL, "op %d row %d (%dx%d W%d): rel err %.3g" % (i, t, o.cfg.Mout, o.cfg.K, o.cfg.bits, err)
 
 
-def rows(rng, n, L):
-    """fp16-representable activations [n][L]."""
-    return rng.standard_normal((n, L)).astype(np.float16).astype(np.float32)
-
-
-def norm_weight(rng, K):
-    w = (1.0 + 0.2 * rng.standard_normal(K)).astype(np.float32)
-    w[rng.integers(0, K, size=K // 16)] = 0.0
-    return w
-
-
 # ---- 1: every chunking, offset consumer and fan-out, both chain forms ------------------------------------------------------------
-CHUNKINGS = [(128, 128), (128, 64), (128, 32), (64, 64), (64, 32), (32, 32), (256, 64)]    # (group_size, act_group_size)
-A_CASES = [(g, a, b, b == 2) for g, a in CHUNKINGS for b in (1, 2, 4)] + [(128, 64, 3, True)]
-
-
 def chunking_chain(mk, g, ags, bits, zp):
     ck = min(g, 128)
     kw = dict(g=g, ags=ags, zp=zp)
@@ -182,10 +64,10 @@ def chunking_chain(mk, g, ags, bits, zp):
     ]
 
 
-@pytest.mark.parametrize("g,ags,bits,zp", A_CASES, ids=["g%d-ags%d-w%d%s" % (g, a, b, "zp" if z else "") for g, a, b, z in A_CASES])
+@pytest.mark.parametrize("g,ags,bits,zp", A_CASES, ids=A_IDS)
 def test_every_chunking(oracle, mk, g, ags, bits, zp):
     steps = chunking_chain(mk, g, ags, bits, zp)
-    hx = {"x0": rows(np.random.default_rng(g + ags + bits), 4, steps[0][0].cfg.K)}
+    hx = host(np.random.default_rng(g + ags + bits), x0=(4, steps[0].op.cfg.K))
     for name in ("flow", "barrier"):
         ones = singles(name, steps, hx, 4)
         for n in (2, 3, 4):
@@ -199,13 +81,13 @@ def test_every_chunking(oracle, mk, g, ags, bits, zp):
 def half_layer(mk, hidden, F, seed, f16=False):
     kw = dict(g=128, ags=64, zp=True)
     return [step(mk(hidden, hidden, 2, seed=seed, **kw), "att", res="x"),
-            step(mk(F, hidden, 2, seed=seed + 1, **kw), ("norm", 0, "w")),
-            step(mk(F, hidden, 2, seed=seed + 2, **kw), ("norm", 0, "w")),
-            step(mk(hidden, F, 2, seed=seed + 3, **kw), ("glu", 1, 2), res=0, f16=f16)]
+            step(mk(F, hidden, 2, seed=seed + 1, **kw), norm(0, "w")),
+            step(mk(F, hidden, 2, seed=seed + 2, **kw), norm(0, "w")),
+            step(mk(hidden, F, 2, seed=seed + 3, **kw), glu(1, 0, 2, 0), res=0, f16=f16)]
 
 
 def layer_inputs(rng, n, hidden):
-    return {"att": rows(rng, n, hidden), "x": rows(rng, n, hidden), "w": norm_weight(rng, hidden)}
+    return dict(host(rng, att=(n, hidden), x=(n, hidden)), w=norm_weight(rng, hidden))
 
 
 @pytest.mark.parametrize("name", ["flow", "barrier"])
@@ -261,7 +143,7 @@ def test_inputs_change_between_launches(stream, mk, name, graph):
     rng = np.random.default_rng(52)
     ext = {"att": torch.zeros((n, 512), device="cuda"), "x": torch.zeros((n, 512), device="cuda"), "w": torch.zeros(512, device="cuda")}
     with form(name), sequence(steps, ext, n) as (seq, outs):
-        assert seq.info()["ring_slots"] == CHAIN_RING, seq.info()
+        expect_kernel(seq.info(), True)
         g = None
         if graph:
             g = torch.cuda.CUDAGraph()
@@ -277,7 +159,7 @@ def test_inputs_change_between_launches(stream, mk, name, graph):
                 else:
                     seq.launch()
                 seq.status()
-                got = [o.cpu().numpy() for o in outs]
+                got = fetch(outs)
                 assert got[3].dtype == np.float16
                 check_rows(got, singles(name, steps, hx, n), name)
         finally:
@@ -297,7 +179,7 @@ def test_bench_chain(stream, oracle):
     wts = [base] + [tb.clone(base) for _ in range(31)]
     try:
         steps = [step(SimpleNamespace(wt=wt, cfg=cfg, A=A, S=S), "x0" if i == 0 else i - 1) for i, wt in enumerate(wts)]
-        hx = {"x0": rows(np.random.default_rng(62), 4, 4096)}
+        hx = host(np.random.default_rng(62), x0=(4, 4096))
         got = run("auto", steps, hx, 4)
         check_rows(got, singles("auto", steps, hx, 4), "bench chain")
         check_oracle(oracle, steps[:2], hx, got[:2])      # later ops grow past fp32 range with these random weights
@@ -340,19 +222,14 @@ def test_rejections(mk):
     build("flow")                                           # the sequence itself qualifies
     with pytest.raises(tb.TMACError, match="peer outputs"):
         build("flow", peers=True)
-    FORMS["streamk"], FORMS["streamk_g7"], FORMS["auto_g7"] = (0, 0, 0), (0, 0, 7), (2, 0, 7)
-    try:
-        for name in ("streamk", "streamk_g7", "auto_g7"):
-            with pytest.raises(tb.TMACError, match="resident chain"):
-                build(name)
-    finally:
-        for k in ("streamk", "streamk_g7", "auto_g7"):
-            del FORMS[k]
+    for name in ("streamk", "streamk_g7", "auto_g7"):
+        with pytest.raises(tb.TMACError, match="resident chain"):
+            build(name)
 
 
 def test_explicit_single_row_is_the_default(mk):
     steps = chunking_chain(mk, 128, 64, 2, True)
-    hx = {"x0": rows(np.random.default_rng(81), 1, steps[0][0].cfg.K)}
+    hx = host(np.random.default_rng(81), x0=(1, steps[0].op.cfg.K))
     for name in ("flow", "barrier"):
         a = run(name, steps, hx, 1, explicit=True)
         b = run(name, steps, hx, 1)

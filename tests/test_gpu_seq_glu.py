@@ -5,137 +5,35 @@ The gated activation a = silu(g) * u is restated on the device with torch from t
 (g / (1 + exp(-g)) * u, eager, one op after the other: the rounding the library documents).  The GLU op must then be bit for bit
 the op of the same sequence whose input is the external vector a, and within the oracle's tolerance of the oracle run on a.
 kfactor = act_group_size / 4 everywhere: the oracle (like the reference) is only right then."""
-import contextlib
-
 import numpy as np
 import pytest
 
 import tmac_b200 as tb
 import tmac_oracle as T
-from seq_util import kc, oracle_gemv
+from seq_util import (DENSE_NMSE, TIGHT_TOL, expect_kernel, fetch, form, glu, host, inputs, mk, oracle_gemv, run_form, same_bits,
+                      sequence, step, stream)
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-TIGHT_TOL = 2e-5        # max |got - oracle| / max |oracle|
-DENSE_NMSE = 5e-4       # against the dense dequantised GEMV (python/t_mac/ops/qgemm.py:277-282 of the reference)
-CHAIN_RING = -4         # info()["ring_slots"] of a sequence served by the resident chain kernel (-kChainCS)
 
-# (seq_impl, chain_flags, seq_grid) of the ways a sequence can be run; "auto*" let the build pick the chain when it qualifies
-FORMS = {"flow": (1, 0, 0), "barrier": (1, 1, 0), "streamk": (0, 0, 0), "streamk_g7": (0, 0, 7), "auto": (2, 0, 0),
-         "auto_barrier": (2, 1, 0)}
-
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
-    torch.cuda.set_stream(torch.cuda.default_stream())
-
-
-class Op:
-    """One uploaded tensor and the problem it was made from (for the oracle and the dense reference)."""
-
-    def __init__(self, Mout, K, bits, g=128, ags=64, zp=False, seed=0):
-        self.cfg = cfg = T.Config(Mout, K, bits, kfactor=ags // 4, group_size=g, act_group_size=ags, zero_point=zp).resolved()
-        self.w, self.sc, self.z, _ = T.make_problem(cfg, seed=seed)
-        self.A, self.S = T.pack_reference_layout(self.w, self.sc, self.z, cfg)
-        self.wt = tb.upload_reference_layout(kc(cfg), self.A, self.S)
-
-
-@pytest.fixture
-def mk(stream):
-    made = []
-
-    def make(*a, **k):
-        made.append(Op(*a, **k))
-        return made[-1]
-    yield make
-    for o in made:
-        o.wt.free()
-
-
-@contextlib.contextmanager
-def form(name):
-    impl, flags, grid = FORMS[name]
-    try:
-        tb.debug_set("seq_impl", impl); tb.debug_set("chain_flags", flags); tb.debug_set("seq_grid", grid)
-        yield
-    finally:
-        tb.debug_set("seq_impl", 2); tb.debug_set("chain_flags", 0); tb.debug_set("seq_grid", 0)
-
-
-def glu(gate_op, gate_off, up_op, up_off):
-    return ("glu", gate_op, gate_off, up_op, up_off)
-
-
-@contextlib.contextmanager
-def sequence(steps, ext):
-    """steps[i] = (op, src, offset): src names an external input in `ext`, or is the index of an earlier step whose outputs
-    [offset, offset + K) are the input, or is glu(...) (offset unused).  Every output is observed.  Yields (seq, outs)."""
-    seq = tb.Sequence()
-    try:
-        outs = []
-        for o, src, off in steps:
-            out = torch.full((o.cfg.Mout,), float("nan"), device="cuda")
-            if isinstance(src, str):
-                seq.add(o.wt, x=ext[src], out=out)
-            elif isinstance(src, tuple):
-                seq.add_glu(o.wt, *src[1:], out=out)
-            else:
-                seq.add(o.wt, in_op=src, in_offset=off, out=out)
-            outs.append(out)
-        seq.build()
-        yield seq, outs
-    finally:
-        seq.free()
-
-
-def expect_kernel(info, chained, grid=0):
-    if chained:
-        assert info["ring_slots"] == CHAIN_RING, info
-    else:
-        assert info["ring_slots"] > 0, info
-        assert info["grid"] == (grid or torch.cuda.get_device_properties(0).multi_processor_count), info
-
-
-def run_form(name, steps, ext, chained=None):
-    """Builds and launches the sequence in form `name`; asserts which kernel serves it.  Returns (info, device outputs)."""
-    impl, _, grid = FORMS[name]
-    with form(name), sequence(steps, ext) as (seq, outs):
-        info = seq.info()
-        expect_kernel(info, impl == 1 if chained is None else chained, grid)
-        seq.launch()
-        seq.status()
-        return info, outs
-
-
-def restate(outs, src, K):
+def restate(got, src, K):
     """The GLU op's input, restated on the device from the sequence's own gate and up outputs."""
     _, gi, go, ui, uo = src
-    g, u = outs[gi][go:go + K], outs[ui][uo:uo + K]
+    g, u = (torch.from_numpy(got[i][off:off + K]).cuda() for i, off in ((gi, go), (ui, uo)))
     return g / (1 + torch.exp(-g)) * u
 
 
-def check(oracle, steps, xs, outs, dense=True):
+def check(oracle, steps, xs, got, dense=True):
     """Every op against the oracle on the input the GPU op saw (a GLU op: the restated activation), and against the float64
     dense dequantised GEMV.  Returns the restated GLU inputs {step: device vector}."""
-    got = [o.cpu().numpy() for o in outs]
     acts = {}
-    for i, (o, src, off) in enumerate(steps):
+    for i, (o, src, off, *_) in enumerate(steps):
         K = o.cfg.K
         if isinstance(src, str):
             x = xs[src]
         elif isinstance(src, tuple):
-            acts[i] = restate(outs, src, K)
+            acts[i] = restate(got, src, K)
             x = acts[i].cpu().numpy()
         else:
             x = got[src][off:off + K]
@@ -148,21 +46,10 @@ def check(oracle, steps, xs, outs, dense=True):
     return acts
 
 
-def same_bits(a, b):
-    a, b = (t.cpu().numpy() if hasattr(t, "cpu") else t for t in (a, b))
-    return a.shape == b.shape and np.array_equal(a.view(np.uint8), b.view(np.uint8))
-
-
-def inputs(rng, **sizes):
-    """fp16-representable activations: host copies and device vectors."""
-    xs = {k: rng.standard_normal(n).astype(np.float16).astype(np.float32) for k, n in sizes.items()}
-    return xs, {k: torch.from_numpy(v).cuda() for k, v in xs.items()}
-
-
 def check_against_plain(name, steps, ext, outs, acts, chained=None):
     """Each GLU op equals, bit for bit, the same op of the same sequence (same form, same ops: stream-K's shares depend on all of
     them) whose input is the external restated activation."""
-    plain = [(o, "glu%d" % i, 0) if i in acts else (o, src, off) for i, (o, src, off) in enumerate(steps)]
+    plain = [step(s.op, "glu%d" % i) if i in acts else s for i, s in enumerate(steps)]
     _, pouts = run_form(name, plain, dict(ext, **{"glu%d" % i: a.contiguous() for i, a in acts.items()}), chained)
     for i in range(len(steps)):
         assert same_bits(outs[i], pouts[i]), "%s: op %d differs from the op fed with the restated activation" % (name, i)
@@ -170,8 +57,8 @@ def check_against_plain(name, steps, ext, outs, acts, chained=None):
 
 def ffn(mk, hidden, F, bits, g, ags, zp, seed):
     kw = dict(g=g, ags=ags, zp=zp)
-    return [(mk(F, hidden, bits, seed=seed, **kw), "x", 0), (mk(F, hidden, bits, seed=seed + 1, **kw), "x", 0),
-            (mk(hidden, F, bits, seed=seed + 2, **kw), glu(0, 0, 1, 0), None)]
+    return [step(mk(F, hidden, bits, seed=seed, **kw), "x"), step(mk(F, hidden, bits, seed=seed + 1, **kw), "x"),
+            step(mk(hidden, F, bits, seed=seed + 2, **kw), glu(0, 0, 1, 0))]
 
 
 # ---- 1: every form and chunking ----------------------------------------------------------------------------------------------------
@@ -198,7 +85,7 @@ def test_ffn_block_in_every_form(oracle, mk, bits, g, ags, zp):
 def test_fused_gate_up_tensor(oracle, mk, name):
     """Gate and up as the two halves of one 2F-row op."""
     F = 768
-    steps = [(mk(2 * F, 512, 2, zp=True, seed=101), "x", 0), (mk(512, F, 2, zp=True, seed=102), glu(0, 0, 0, F), None)]
+    steps = [step(mk(2 * F, 512, 2, zp=True, seed=101), "x"), step(mk(512, F, 2, zp=True, seed=102), glu(0, 0, 0, F))]
     xs, ext = inputs(np.random.default_rng(1), x=512)
     _, outs = run_form(name, steps, ext)
     acts = check(oracle, steps, xs, outs)
@@ -208,12 +95,12 @@ def test_fused_gate_up_tensor(oracle, mk, name):
 def depth_chain(mk, gate_off, up_off):
     kw = dict(zp=True)
     return [
-        (mk(1024, 512, 2, seed=111, **kw), "x0", 0),
-        (mk(1024, 1024, 2, seed=112, **kw), 0, 0),            # gate: three ops before the GLU op
-        (mk(768, 512, 2, seed=113, **kw), "x1", 0),
-        (mk(1024, 768, 2, seed=114, **kw), 2, 0),             # up
-        (mk(512, 768, 2, seed=115, **kw), glu(1, gate_off, 3, up_off), None),
-        (mk(256, 512, 2, seed=116, **kw), 4, 0),              # a plain op reading the GLU op
+        step(mk(1024, 512, 2, seed=111, **kw), "x0"),
+        step(mk(1024, 1024, 2, seed=112, **kw), 0),           # gate: three ops before the GLU op
+        step(mk(768, 512, 2, seed=113, **kw), "x1"),
+        step(mk(1024, 768, 2, seed=114, **kw), 2),            # up
+        step(mk(512, 768, 2, seed=115, **kw), glu(1, gate_off, 3, up_off)),
+        step(mk(256, 512, 2, seed=116, **kw), 4),             # a plain op reading the GLU op
     ]
 
 
@@ -262,7 +149,7 @@ def test_inputs_change_between_launches(stream, oracle, mk, name, graph):
                 seq.launch()
         try:
             for _ in range(3):
-                xs = {k: rng.standard_normal(v.numel()).astype(np.float16).astype(np.float32) for k, v in ext.items()}
+                xs = host(rng, **{k: v.numel() for k, v in ext.items()})
                 for k, v in ext.items():
                     v.copy_(torch.from_numpy(xs[k]))           # current stream = the library stream: ordered before the launch
                 if graph:
@@ -270,7 +157,7 @@ def test_inputs_change_between_launches(stream, oracle, mk, name, graph):
                 else:
                     seq.launch()
                 seq.status()
-                check(oracle, steps, xs, outs, dense=False)
+                check(oracle, steps, xs, fetch(outs), dense=False)
         finally:
             if g is not None:
                 torch.cuda.synchronize()

@@ -7,210 +7,60 @@ of them) without norm inputs or residuals -- a norm op reads the external vector
 order from the sequence's own producer output, a plain op reads its producer's output as an external vector -- and each op must
 equal the restated op plus, for a residual, a numpy float32 add (an fp16 C rounded once, at the store).
 kfactor = act_group_size / 4 everywhere: the oracle (like the reference) is only right then."""
-import contextlib
-
 import numpy as np
 import pytest
 
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
-from seq_util import kc, oracle_gemv
+from seq_util import (DENSE_NMSE, EPS, FORMS, TIGHT_TOL, device, expect_kernel, fetch, form, glu, host, mk, norm, norm_weight,
+                      oracle_gemv, rms_input, run_form, same_bits, sequence, step, stream)
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
-TIGHT_TOL = 2e-5        # max |got - oracle| / max |oracle|
-DENSE_NMSE = 5e-4
-CHAIN_RING = -4         # info()["ring_slots"] of a sequence served by the resident chain kernel (-kChainCS)
-EPS = 1e-5
-
-# (seq_impl, chain_flags, seq_grid) of the ways a sequence can be run; "auto" lets the build pick the chain when it qualifies
-FORMS = {"flow": (1, 0, 0), "barrier": (1, 1, 0), "streamk": (0, 0, 0), "streamk_g7": (0, 0, 7), "auto": (2, 0, 0)}
-ALL = list(FORMS)
-
-
-@pytest.fixture(scope="module")
-def stream():
-    if not torch.cuda.is_available():
-        pytest.fail("-m gpu tests need a CUDA device; libtmac_b200 has no CPU fallback")
-    lib = tb.load()
-    tb.check(lib.tmac_b200_init(0), "init")
-    st = torch.cuda.Stream()
-    torch.cuda.set_stream(st)
-    tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
-    yield st
-    torch.cuda.synchronize()
-    tb.check(lib.tmac_b200_set_stream(None), "set_stream")
-    torch.cuda.set_stream(torch.cuda.default_stream())
-
-
-class Op:
-    """One uploaded tensor and the problem it was made from (for the oracle and the dense reference)."""
-
-    def __init__(self, Mout, K, bits, g=128, ags=64, zp=False, seed=0):
-        self.cfg = cfg = T.Config(Mout, K, bits, kfactor=ags // 4, group_size=g, act_group_size=ags, zero_point=zp).resolved()
-        self.w, self.sc, self.z, _ = T.make_problem(cfg, seed=seed)
-        self.A, self.S = T.pack_reference_layout(self.w, self.sc, self.z, cfg)
-        self.wt = tb.upload_reference_layout(kc(cfg), self.A, self.S)
-
-
-@pytest.fixture
-def mk(stream):
-    made = []
-
-    def make(*a, **k):
-        made.append(Op(*a, **k))
-        return made[-1]
-    yield make
-    for o in made:
-        o.wt.free()
-
-
-@contextlib.contextmanager
-def form(name):
-    impl, flags, grid = FORMS[name]
-    try:
-        tb.debug_set("seq_impl", impl); tb.debug_set("chain_flags", flags); tb.debug_set("seq_grid", grid)
-        yield
-    finally:
-        tb.debug_set("seq_impl", 2); tb.debug_set("chain_flags", 0); tb.debug_set("seq_grid", 0)
-
-
-# A step: (op, src, res, f16).  src: the name of an external input | the index of an earlier op (its rows [0, K)) |
-# ("glu", gate_op, gate_off, up_op, up_off) | ("norm", in_op, weight name, eps).  res: None | external name | earlier op index.
-def step(op, src, res=None, f16=False):
-    return (op, src, res, f16)
-
-
-def norm(in_op, w, eps=EPS):
-    return ("norm", in_op, w, eps)
-
-
-def glu(g, go, u, uo):
-    return ("glu", g, go, u, uo)
-
-
-@contextlib.contextmanager
-def sequence(steps, ext):
-    """Builds the sequence; every output is observed (fp16 where the step says so).  Yields (seq, outs)."""
-    seq = tb.Sequence()
-    try:
-        outs = []
-        for i, (o, src, res, f16) in enumerate(steps):
-            dt = torch.float16 if f16 else torch.float32
-            out = torch.full((o.cfg.Mout,), float("nan"), device="cuda", dtype=dt)
-            d = tb.F16 if f16 else tb.F32
-            if isinstance(src, str):
-                seq.add(o.wt, x=ext[src], out=out, dtype=d)
-            elif isinstance(src, int):
-                seq.add(o.wt, in_op=src, out=out, dtype=d)
-            elif src[0] == "glu":
-                seq.add_glu(o.wt, *src[1:], out=out, dtype=d)
-            else:
-                seq.add_rmsnorm(o.wt, src[1], ext[src[2]], src[3], out=out, dtype=d)
-            if isinstance(res, str):
-                seq.residual(i, r=ext[res])
-            elif res is not None:
-                seq.residual(i, r_op=res)
-            outs.append(out)
-        seq.build()
-        yield seq, outs
-    finally:
-        seq.free()
-
-
-def run_form(name, steps, ext, chained=None):
-    """Builds and launches the sequence in form `name`; asserts which kernel serves it.  Returns the outputs as numpy arrays."""
-    impl, _, grid = FORMS[name]
-    chained = impl == 1 if chained is None else chained
-    with form(name), sequence(steps, ext) as (seq, outs):
-        expect_kernel(seq.info(), chained, grid)
-        seq.launch()
-        seq.status()
-        return [o.cpu().numpy() for o in outs]
-
-
-def expect_kernel(info, chained, grid=0):
-    if chained:
-        assert info["ring_slots"] == CHAIN_RING, info
-    else:
-        assert info["ring_slots"] > 0, info
-        assert info["grid"] == (grid or torch.cuda.get_device_properties(0).multi_processor_count), info
-
-
-def rms_input(h, w, eps):
-    """The norm op's input a, in numpy float32 in the documented order: lane l sums the 4-element groups l, l + 32, ... in
-    ascending order as (h0*h0 + h1*h1) + (h2*h2 + h3*h3), the 32 lane sums meet in the shfl_xor butterfly 16, 8, 4, 2, 1."""
-    h = np.asarray(h, np.float32)
-    K = h.size
-    g = h.reshape(-1, 4)
-    q = (g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1]) + (g[:, 2] * g[:, 2] + g[:, 3] * g[:, 3])
-    q = np.concatenate([q, np.zeros(-len(q) % 32, np.float32)]).reshape(-1, 32)
-    s = np.zeros(32, np.float32)
-    for row in q:
-        s = s + row
-    for m in (16, 8, 4, 2, 1):
-        s = s + s[np.arange(32) ^ m]
-    inv = np.float32(1.0) / np.sqrt(s[0] / np.float32(K) + np.float32(eps))
-    return (h * inv) * np.asarray(w, np.float32)
+ALL = ["flow", "barrier", "streamk", "streamk_g7", "auto"]
 
 
 def restated(steps, got, hext):
     """The same ops without norm inputs and residuals: a norm op reads a (rms_input of its producer's output in `got`), a plain op
     reads its producer's output as an external vector, a GLU op stays (its producers compute the same bits).  All outputs fp32."""
     plain, pext = [], {}
-    for i, (o, src, res, f16) in enumerate(steps):
+    for i, (o, src, *_) in enumerate(steps):
         name = "in%d" % i
         if isinstance(src, str):
             pext[name] = hext[src]
         elif isinstance(src, int):
             pext[name] = got[src][:o.cfg.K].astype(np.float32)
         elif src[0] == "norm":
-            pext[name] = rms_input(got[src[1]], hext[src[2]], src[3])
+            pext[name] = rms_input(got[src[1]], hext[src[2]], src[3])[0]
         plain.append(step(o, src if name not in pext else name))
     return plain, pext
-
-
-def device(xs):
-    return {k: torch.from_numpy(np.ascontiguousarray(v, np.float32)).cuda() for k, v in xs.items()}
 
 
 def check_restated(name, steps, hext, got, chained=None):
     """Every op bit for bit against the restated sequence (plus the residual, in numpy float32); returns the restated inputs."""
     plain, pext = restated(steps, got, hext)
-    pgot = run_form(name, plain, device(pext), chained)
-    for i, (o, src, res, f16) in enumerate(steps):
+    _, pgot = run_form(name, plain, device(pext), chained)
+    for i, (o, src, off, res, f16) in enumerate(steps):
         want = pgot[i]
         if res is not None:
             want = want + (hext[res] if isinstance(res, str) else got[res].astype(np.float32))
         if f16:
             want = want.astype(np.float16)
-        assert want.dtype == got[i].dtype and np.array_equal(want.view(np.uint8), got[i].view(np.uint8)), \
+        assert same_bits(want, got[i]), \
             "%s: op %d differs from the restated op%s" % (name, i, " plus its residual" if res is not None else "")
     return pext
 
 
 def check_norm_oracle(oracle, steps, pext, got):
-    for i, (o, src, res, f16) in enumerate(steps):
+    for i, (o, src, off, res, f16) in enumerate(steps):
         if isinstance(src, tuple) and src[0] == "norm":
             ref = oracle_gemv(oracle, o.cfg, o.A, o.S, pext["in%d" % i])
             if res is not None:
                 continue
             err = np.abs(got[i] - ref).max() / np.abs(ref).max()
             assert err <= TIGHT_TOL, "norm op %d: rel err %.3g against the oracle on a" % (i, err)
-
-
-def host(rng, **sizes):
-    return {k: rng.standard_normal(n).astype(np.float16).astype(np.float32) for k, n in sizes.items()}
-
-
-def norm_weight(rng, K):
-    """Norm weights around 1 with zeros and negative values."""
-    w = (1.0 + 0.2 * rng.standard_normal(K)).astype(np.float32)
-    w[rng.integers(0, K, size=K // 16)] = 0.0
-    w[rng.integers(0, K, size=K // 16)] *= -1.0
-    return w
 
 
 # ---- 1: residuals -----------------------------------------------------------------------------------------------------------------
@@ -221,7 +71,7 @@ def test_residual(mk, name, f16):
     a, b, c = mk(512, 512, 2, zp=True, seed=1), mk(512, 512, 2, zp=True, seed=2), mk(512, 512, 2, zp=True, seed=3)
     steps = [step(a, "x"), step(b, 0, res="r"), step(c, 1, res=0, f16=f16)]
     hx = host(np.random.default_rng(11), x=512, r=512)
-    got = run_form(name, steps, device(hx), chained=FORMS[name][0] != 0)
+    _, got = run_form(name, steps, device(hx), chained=FORMS[name][0] != 0)
     check_restated(name, steps, hx, got, chained=FORMS[name][0] != 0)
 
 
@@ -236,7 +86,7 @@ def test_norm_op(oracle, mk, name, bits, g, ags, zp):
     rng = np.random.default_rng(12)
     hx = dict(host(rng, x=512), w0=norm_weight(rng, 768), w1=norm_weight(rng, 768), w2=norm_weight(rng, 512))
     chained = FORMS[name][0] != 0
-    got = run_form(name, steps, device(hx), chained)
+    _, got = run_form(name, steps, device(hx), chained)
     pext = check_restated(name, steps, hx, got, chained)
     check_norm_oracle(oracle, steps, pext, got)
 
@@ -266,7 +116,7 @@ def test_llama2_7b_half_layer(mk, bits, zp, chained):
     steps = half_layer(mk, 4096, 11008, bits, zp, seed=40 + bits)
     rng = np.random.default_rng(13)
     hx = dict(host(rng, att=4096, x=4096), w=(1.0 + 0.1 * rng.standard_normal(4096)).astype(np.float32))
-    got = run_form("auto", steps, device(hx), chained=chained)
+    _, got = run_form("auto", steps, device(hx), chained=chained)
     check_restated("auto", steps, hx, got, chained=chained)
     e = T.nmse(dense_half_layer(steps, hx), got[3])
     assert e <= DENSE_NMSE, "NMSE %.3g against the dense dequantised layer" % e
@@ -278,14 +128,14 @@ def test_layer_chain_without_decode_ahead(mk):
     steps = half_layer(mk, 512, 768, 2, True, seed=45)
     rng = np.random.default_rng(16)
     hx = dict(host(rng, att=512, x=512), w=norm_weight(rng, 512))
-    ahead = run_form("flow", steps, device(hx))
+    _, ahead = run_form("flow", steps, device(hx))
     try:
         tb.debug_set("chain_ahead", 0)
-        plain = run_form("flow", steps, device(hx))
+        _, plain = run_form("flow", steps, device(hx))
     finally:
         tb.debug_set("chain_ahead", 1)
     for i, (a, b) in enumerate(zip(ahead, plain)):
-        assert np.array_equal(a.view(np.uint8), b.view(np.uint8)), "op %d" % i
+        assert same_bits(a, b), "op %d" % i
     check_restated("flow", steps, hx, plain)
 
 
@@ -316,7 +166,7 @@ def test_inputs_change_between_launches(stream, mk, name, graph):
                 else:
                     seq.launch()
                 seq.status()
-                got = [o.cpu().numpy() for o in outs]
+                got = fetch(outs)
                 with form(name):
                     check_restated(name, steps, hx, got, chained)
         finally:
@@ -345,7 +195,7 @@ def test_edge_rows(oracle, mk, name, kind, eps):
     hx["w"] = norm_weight(rng, K)
     steps = [step(mk(K, K, 2, zp=True, seed=61), "x", res="r"), step(mk(768, K, 2, zp=True, seed=62), norm(0, "w", eps))]
     chained = FORMS[name][0] != 0
-    got = run_form(name, steps, device(hx), chained)
+    _, got = run_form(name, steps, device(hx), chained)
     if kind != "normal":
         assert np.array_equal(got[0], hx["r"]), "h = 0 + r"
     if kind == "zero":
