@@ -183,6 +183,28 @@ TMAC_B200_API int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int 
                                          void *const *C);
 TMAC_B200_API int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
+/* Routed MoE experts: the router's top-k choice stays on the device, so a MoE FFN is two launches with no host sync and the token step
+ * stays graph-capturable: gemv_experts([gate, up], h2, ids) -> G, U, then gemv_experts_glu(down, G, U, ids, weights, h) -> y.
+ *   gemv_experts:     handles [count][n_experts] (host), entry i * n_experts + e = tensor i of expert e (e.g. i = 0 gate, 1 up).
+ *                     B [N][K]; ids: device int32 [N][topk], read only by the kernel; C[i] [N][topk][Mout] with
+ *                     C[i][n][j] = gemv(handles[i * n_experts + ids[n][j]], B[n]).
+ *   gemv_experts_glu: handles [n_experts], K the FFN width.  G, U [N][topk][K] (C[0], C[1] of the call above); weights: device fp32
+ *                     [N][topk]; R [N][Mout] or NULL, may equal C; C [N][Mout].  y_j = gemv(handles[ids[n][j]], a_j) with
+ *                     a_j = swiglu(G[n][j], U[n][j]) as for gemv_glu, and
+ *                     C[n] = fadd_rn(...fadd_rn(fmul_rn(w_0, y_0), fmul_rn(w_1, y_1))..., fmul_rn(w_{topk-1}, y_{topk-1})) (+ R[n]),
+ *                     j ascending, no fma contraction, fp16 R widened, rounded once to fp16 when dtype is F16; the result does not
+ *                     depend on which slot finishes first.
+ * Each slot's row sums are those of tmac_b200_gemv_grouped over the N * count * topk selected tensors at N = 1, fed row n (the same
+ * decomposition).  The rules of gemv_grouped apply: device pointers of dtype unless said otherwise, one geometry for all tensors,
+ * the GEMV kernel at every N, an armed tmac_b200_peer_outputs makes the call fail; fp-path tensors with the activation group inside a
+ * chunk only.  1 <= topk <= 8.  Repeated ids are allowed; each slot is computed on its own.  An id outside [0, n_experts) is never read
+ * out of bounds: in gemv_experts that slot's Mout outputs are quiet NaN, in gemv_experts_glu every output of that token is; other
+ * slots and tokens are unaffected.  gemv_experts_glu keeps a library workspace and arrival counters that return to zero by the end of
+ * each launch: make one eager call at the largest N * topk and Mout before capturing it in a CUDA graph. */
+TMAC_B200_API int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B,
+                                         const int32_t *ids, int topk, void *const *C);
+TMAC_B200_API int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
+                                             const int32_t *ids, const float *weights, int topk, const void *R, void *C);
 /* Fused convenience (llama_cpp_init + llama_cpp_compute of the whole tensor in one call,
  * workspaces owned by the library): C [N][M] = qgemm_lut(preprocessor(B)). */
 TMAC_B200_API int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C);

@@ -135,6 +135,7 @@ struct Context {
     std::vector<std::pair<std::vector<const void *>, void *>> ptr_tables;   // grouped-launch pointer tables
     // workspaces
     DevBuf d_b, d_qlut, d_ls, d_lb, d_c, d_cbits, d_trace, d_tiles, d_pf_scratch, d_pf_flags;
+    DevBuf d_moe_ws, d_moe_cnt;          // tmac_b200_gemv_experts_glu: the slots' rows and the arrival counters (zero between launches)
     int trace = 0, trace_ctas = 0, trace_seq = 0;
     int chain_flags = 0;                 // resident chain (tmac_chain.cuh): bit 0 = grid-barrier form (comparison); default: data flow
     int chain_ahead = 1;                 // resident chain: 0 = never the decode-ahead instantiation (comparison); default: when it fits
@@ -382,7 +383,8 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
     }
     if (fused_act) { p.act = fused_act; p.act_f16 = act_f16; sym = true; }
     const int agq = L.agq();
-    gemv3_fn fn = io_kind ? pick_gemv3_io(L.pb, L.qch, agq, minb, io_kind)
+    gemv3_fn fn = io_kind >= kIoExperts ? pick_gemv3_experts(L.pb, L.qch, agq, minb, io_kind)
+                : io_kind ? pick_gemv3_io(L.pb, L.qch, agq, minb, io_kind)
                           : fused_act ? pick_gemv3_fused(L.pb, L.qch, agq, minb) : pick_gemv3(L.pb, sym, L.qch, agq, minb);
     if (!fn) return fail("qgemm_lut: unsupported chunking (qch=" + std::to_string(L.qch) + ", agq=" + std::to_string(agq) + ")");
     p.nbuf = (p.bpw > 1) ? 2 : 1;
@@ -1276,6 +1278,61 @@ int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, con
     Gemv3Io io{};
     io.res = R;
     return gemv_io("gemv_residual", &handle, 1, N, dtype, kIoPlain, B, io, &C);
+}
+
+// tmac_b200_gemv_experts / _glu: the launch of tmac_b200_gemv_grouped over count * topk slots (so each slot's sums are those of
+// gemv_grouped at N * count * topk), with a pointer table of every tensor, count * n_experts entries, from which each slot picks its
+// tensor by the id it reads on the device.  Everything is checked before anything is launched.
+static int gemv_experts(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
+                        int io_kind, const void *A, Gemv3Io io, void *const *C, int nC) {
+    if (!handles || count <= 0 || n_experts <= 0 || (long long)count * n_experts > 65535 || N <= 0 || topk < 1 || topk > 8 || !A ||
+        !io.ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
+        return fail(what + ": bad arguments");
+    if (!is_device_ptr(A) || !is_device_ptr(io.ids) || (io.act2 && !is_device_ptr(io.act2)) || (io.wts && !is_device_ptr(io.wts)) ||
+        (io.res && !is_device_ptr(io.res)))
+        return fail(what + ": device pointers only");
+    for (int i = 0; i < nC; ++i)
+        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
+    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts is C[i] (kIoExpertsGlu: C[0] = C)
+    for (int i = 0; i < count; ++i)
+        for (int e = 0; e < n_experts; ++e) Cx[(size_t)i * n_experts + e] = C[nC > 1 ? i : 0];
+    const Resident *R = nullptr;
+    BatchPtrs bp;
+    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, Cx.data(), &R, &bp)) return -1;
+    const StreamLayout &L = R->L;
+    if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
+    bp.n = count * topk;                           // grid.z: the slots
+    io.topk = topk; io.n_experts = n_experts;
+    if (io_kind == kIoExpertsGlu) {
+        const size_t cnt_bytes = (size_t)N * ((L.Mout + L.rsb - 1) / L.rsb) * sizeof(unsigned);
+        if (g.d_moe_ws.ensure((size_t)N * topk * L.Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
+        if (g.d_moe_cnt.cap < cnt_bytes) {
+            if (g.d_moe_cnt.ensure(cnt_bytes)) return fail(what + ": out of device memory (workspace)");
+            CUDA_OK(cudaMemsetAsync(g.d_moe_cnt.p, 0, g.d_moe_cnt.cap, g.stream()));
+        }
+        io.ws = (float *)g.d_moe_ws.p; io.cnt = (unsigned *)g.d_moe_cnt.p;
+    }
+    return launch_gemv3(*R, 0, L.Mout, N, nullptr, nullptr, nullptr, nullptr, L.Mout, 0, dtype == TMAC_B200_F16, true, &bp, A,
+                        dtype == TMAC_B200_F16, &io, io_kind);
+}
+
+int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B, const int32_t *ids,
+                           int topk, void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    Gemv3Io io{};
+    io.ids = ids;
+    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kIoExperts, B, io, C, count > 0 ? count : 0);
+}
+
+int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
+                               const int32_t *ids, const float *weights, int topk, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    if (!U || !weights || !C) return fail("gemv_experts_glu: bad arguments");
+    Gemv3Io io{};
+    io.act2 = U; io.ids = ids; io.wts = weights; io.res = R;
+    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kIoExpertsGlu, G, io, &C, 1);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

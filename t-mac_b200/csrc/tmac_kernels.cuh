@@ -503,12 +503,19 @@ struct Gemv3Params {
 };
 // The input transform and residual of the gemv3_kernel instantiations with IO != kIoNone: the kernel's last parameter, so that
 // Gemv3Params, wtx and wty keep their parameter offsets.  The plain input / the norm's h / the GLU's g is p.act.
-enum : int { kIoNone = 0, kIoPlain = 1, kIoNorm = 2, kIoGlu = 3 };
+// The routed-expert kinds (kIoExperts, kIoExpertsGlu) pick each slot's tensor on the device: slot z = i * topk + j of token n
+// (blockIdx.z, blockIdx.y) runs pointer-table entry i * n_experts + ids[n * topk + j].
+enum : int { kIoNone = 0, kIoPlain = 1, kIoNorm = 2, kIoGlu = 3, kIoExperts = 4, kIoExpertsGlu = 5 };
 struct Gemv3Io {
-    const void *act2;              // kIoGlu: u [N][K], dtype of p.act
+    const void *act2;              // kIoGlu, kIoExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
     const float *nw;               // kIoNorm: the norm weight w [K] (16-byte aligned)
     float eps;                     // kIoNorm
     const void *res;               // residual r [N][ldc] of the output's dtype, or null; may equal C
+    const int32_t *ids;            // experts: [N][topk], written by earlier work in the stream (read after the dependency wait)
+    const float *wts;              // kIoExpertsGlu: combine weights [N][topk]
+    float *ws;                     // kIoExpertsGlu: the slots' fp32 rows [N][topk][ldc]
+    unsigned *cnt;                 // kIoExpertsGlu: arrivals per (token, row super-block) [N][nrsb], 0 between launches
+    int topk, n_experts;           // experts
 };
 __device__ __forceinline__ long long globaltimer_ns() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 #ifdef TMAC_ENABLE_TRACE
@@ -622,10 +629,16 @@ constexpr int kG3MaxWarps = 8;
 // IO (fused fp path only, instantiated in tmac_gemv_io.cu): the LUT input of row n is a transform of the activation rows -- kIoNorm
 // a[k] = rms_scale(h[k], inv_n, w[k]), kIoGlu a[k] = swiglu(g[k], u[k]), kIoPlain a = the row -- built into the chunk's slice
 // with lut_slice as a plain input; the leader adds io.res (when not null) to the row sums before the store.
+// Routed experts (instantiated in tmac_gemv_experts.cu): slot z = i * topk + j of token n takes its tensor from the pointer table at
+// i * n_experts + ids[n][j], read after the dependency wait, so the slot's first block request waits for it too.  kIoExperts reads row
+// n and stores row n * topk + j of C[i]; kIoExpertsGlu reads row n * topk + j of g and u, stores its rows into io.ws and counts
+// itself in io.cnt, and the leader that completes a (token, row super-block) combines the topk rows in ascending j into C.  A slot
+// whose id is outside [0, n_experts) streams no block and yields quiet NaN rows.
 template <int PB, bool SYM, int QCH, int AGQ, int MINB, bool FUSED = false, int IO = kIoNone>
 __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gemv3Params p, const uint32_t wtx, const uint32_t wty,
                                                                        const Gemv3Io io) {
     static_assert(IO == kIoNone || (FUSED && SYM && AGQ > 0), "input transforms: fused fp path only");
+    constexpr bool EXPERTS = IO == kIoExperts || IO == kIoExpertsGlu;
     constexpr int RW = 8 / PB;
     constexpr int RSB = 32 * RW;
     constexpr int TB = SYM ? 8 : 16;              // table bytes per group in shared memory
@@ -655,21 +668,25 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     if (!p.pdl_late) pdl_launch_dependents();     // the next launch may start its weight stream now
 
     const int c_first = (rank * WPC + warp) * p.bpw;
-    const int c_end = min(p.nchunk, c_first + p.bpw);
+    int c_end = min(p.nchunk, c_first + p.bpw);
     const unsigned char *Wb = p.W;
     const int8_t *qb = p.qlut;
     const float *lsb = p.lut_scales, *lbb = p.lut_biases;
     void *Cb = p.C;
+    const int xj = EXPERTS ? (int)blockIdx.z % io.topk : 0;   // experts: the slot's rank j among the token's topk and its tensor i
+    const int xi = EXPERTS ? (int)blockIdx.z / io.topk : 0;
     if (p.nbatch > 0) {
         const int z = blockIdx.z;
-        Wb = p.Wv[z]; Cb = p.Cv[z];
+        if (EXPERTS) Cb = p.Cv[xi * io.n_experts];
+        else { Wb = p.Wv[z]; Cb = p.Cv[z]; }
         if (!FUSED) { qb = p.qlutv[z]; lsb = p.lsv[z]; lbb = p.lbv[z]; }   // fused: the tensors of the group share the activation rows
     }
     const unsigned char *rsb_base = Wb + (size_t)rsb * p.rsb_stride;
     const int nag = p.K / p.ags;
+    const int arow = IO == kIoExpertsGlu ? n * io.topk + xj : n;   // the activation row of this CTA
     // fused: the 4 activations from element k of the row of act (p.act, or kIoGlu's u), fp32 or fp16
     auto load_group = [&](size_t k, float4 &x, const void *act = nullptr) {
-        const size_t k0 = (size_t)n * p.K + k;
+        const size_t k0 = (size_t)arow * p.K + k;
         if (!act) act = p.act;
         if (p.act_f16) {
             const uint2 h = __ldg(reinterpret_cast<const uint2 *>(reinterpret_cast<const __half *>(act) + k0));
@@ -685,7 +702,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         mbar_init(mbar, 1); mbar_init(mbar + 1, 1);
         mbar_fence_init();
         fence_proxy_async();
-        if (c_first < c_end) {
+        if (!EXPERTS && c_first < c_end) {
             bulk_load(stage0, rsb_base + (size_t)c_first * p.blk_bytes, (uint32_t)p.blk_bytes, mbar);
             if (p.Wnext)                           // pull the next tensor's blocks of this warp into L2
                 l2_prefetch_bulk(p.Wnext + (size_t)rsb * p.rsb_stride + (size_t)c_first * p.blk_bytes,
@@ -696,6 +713,14 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     if (tid == 0) TMAC_TRACE(1);
     pdl_wait();                                   // LUT / LUT scales come from the previous kernel
     if (tid == 0) TMAC_TRACE(2);
+    bool bad = false;                             // experts: the slot's id is outside [0, n_experts)
+    if (EXPERTS) {
+        const int id = io.ids[(size_t)n * io.topk + xj];
+        bad = (unsigned)id >= (unsigned)io.n_experts;
+        if (bad) c_end = c_first;                  // no block: the sums stay 0 and the rows become NaN in the epilogue
+        else rsb_base = p.Wv[xi * io.n_experts + id] + (size_t)rsb * p.rsb_stride;
+        if (lane == 0 && c_first < c_end) bulk_load(stage0, rsb_base + (size_t)c_first * p.blk_bytes, (uint32_t)p.blk_bytes, mbar);
+    }
 
     float cacc[RW];
     int iacc[RW];
@@ -823,7 +848,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
                     const float4 h = reinterpret_cast<const float4 *>(iscr)[g], w = __ldg(reinterpret_cast<const float4 *>(io.nw) + g);
                     x = make_float4(rms_scale(h.x, inv, w.x), rms_scale(h.y, inv, w.y), rms_scale(h.z, inv, w.z), rms_scale(h.w, inv, w.w));
                 }
-            } else if (IO == kIoGlu) {
+            } else if (IO == kIoGlu || IO == kIoExpertsGlu) {
                 if (lane < NG) {
                     float4 gv, uv;
                     load_group(((size_t)c * NG + lane) * 4, gv);
@@ -912,12 +937,47 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
                 out = int_path_out(isum, FUSED ? row_scale : __ldg(lsg), FUSED ? iscr[(p.K >> 5) + kG3MaxWarps] : __ldg(lbg), p.scale0);
             else
                 out = fsum;
-            const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
-            if (IO != kIoNone && io.res)           // read, then written by this thread: the residual may be C itself
-                out = __fadd_rn(out, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
-            store_out(Cb, o, out, p.out_f16);
-            for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
-                store_out(p.Cpeer[q], o, out, p.out_f16);
+            if (EXPERTS) {                          // row n * topk + j of C[i] / of the workspace (c_row0 = 0)
+                const size_t o = (size_t)(n * io.topk + xj) * p.ldc + row;
+                if (bad) out = __int_as_float(0x7fffffff);
+                if (IO == kIoExperts) store_out(Cb, o, out, p.out_f16);
+                else io.ws[o] = out;
+            } else {
+                const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
+                if (IO != kIoNone && io.res)           // read, then written by this thread: the residual may be C itself
+                    out = __fadd_rn(out, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
+                store_out(Cb, o, out, p.out_f16);
+                for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
+                    store_out(p.Cpeer[q], o, out, p.out_f16);
+            }
+        }
+    }
+    if (IO == kIoExpertsGlu) {
+        // The combine.  This slot's rows are in io.ws; thread 0 counts the slot in (release, for every thread's stores: they precede
+        // it by the barrier) and learns whether it completes the token's row super-block (acquire, for the other slots' rows).  The
+        // leader that completes it adds the topk rows in ascending j -- not in arrival order -- and resets the counter for the next
+        // launch, which touches it only after its dependency wait.
+        unsigned *last = reinterpret_cast<unsigned *>(red);   // red is free once the CTA and cluster sums are done
+        __syncthreads();
+        if (tid == 0) {
+            unsigned *c = io.cnt + (size_t)n * p.nrsb + rsb, prev;
+            asm volatile("atom.acq_rel.gpu.global.add.u32 %0, [%1], 1;" : "=r"(prev) : "l"(c) : "memory");
+            *last = prev == (unsigned)io.topk - 1;
+            if (*last) *c = 0;
+        }
+        __syncthreads();
+        if (!*last) return;
+        const float *wn = io.wts + (size_t)n * io.topk;
+        for (int t = tid; t < RSB; t += nthreads) {
+            const int row = (p.rsb0 + rsb) * RSB + t;
+            if (row < p.row_begin || row >= p.row_end) continue;
+            const float *y = io.ws + (size_t)n * io.topk * p.ldc + row;
+            float acc = __fmul_rn(wn[0], __ldcg(y));
+            for (int j = 1; j < io.topk; ++j) acc = __fadd_rn(acc, __fmul_rn(wn[j], __ldcg(y + (size_t)j * p.ldc)));
+            const size_t o = (size_t)n * p.ldc + row;
+            if (io.res)                            // read, then written by this thread: the residual may be C itself
+                acc = __fadd_rn(acc, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
+            store_out(Cb, o, acc, p.out_f16);
         }
     }
     if (tid == 0) TMAC_TRACE(7);
@@ -926,6 +986,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 typedef void (*gemv3_fn)(const Gemv3Params, const uint32_t, const uint32_t, const Gemv3Io);
 // the fused fp-path instantiations with an input transform (IO != kIoNone), in tmac_gemv_io.cu
 gemv3_fn pick_gemv3_io(int pb, int qch, int agq, int minb, int io);   // null: grouping not instantiated
+// the routed-expert instantiations (io = kIoExperts / kIoExpertsGlu), in tmac_gemv_experts.cu
+gemv3_fn pick_gemv3_experts(int pb, int qch, int agq, int minb, int io);
 
 // ------------------------------------------------------------------------------------------
 // cbits_kernel (debug / parity gate G2): per-plane int32 sums in the reference plane layout.

@@ -7,7 +7,8 @@ graph; `tokens_per_s()` reports the full step, bench.py reports the matmul-only 
 layer's FFN (gate, up, SiLU*mul, down) is one decode sequence launch instead (tools/ffn_bench.py times both); with
 `post_attn_sequence=True` everything after attention -- o-projection, residual add, RMSNorm, FFN and the second residual add -- is
 one; with `fused_ops=True` the seven linears run as four library launches whose inputs and outputs take the RMSNorms, the
-SiLU*mul and the residual adds (tools/layer_bench.py times the four).
+SiLU*mul and the residual adds (tools/layer_bench.py times the four); adding `experts=E` makes the FFN a routed MoE of E experts with
+top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them).
 
 Not a model implementation: no tokenizer, no sampling, no checkpoint loading (SURVEY 8 f1 scope).  torch is used for device
 memory, streams and the non-matmul ops only; every linear is a library launch.
@@ -63,22 +64,31 @@ class QLinear:
 
 class DecodeLayer:
     def __init__(self, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, seed: int, share: Optional["DecodeLayer"] = None, group_size: int = 128,
-                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False):
+                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2):
         """ffn_sequence: the FFN (gate, up, SiLU*mul, down) runs as ONE decode sequence whose down op reads the gated activation of
         the gate and up ops (tmac_b200_seq_add_gemv_glu) instead of three launches and a torch op.
         post_attn_sequence: the layer after attention runs as ONE decode sequence [o(att) + x, gate(rmsnorm(h) * w2),
         up(rmsnorm(h) * w2), down(silu(gate) * up) + h] (tmac_b200_seq_residual, tmac_b200_seq_add_gemv_rmsnorm); the layer keeps
         its input x in a buffer of its own, because the sequence's external vectors are fixed when it is built.
         fused_ops: the linears run as four launches and no torch op around them: gemv_rmsnorm([q, k, v], x, norm1),
-        gemv_residual(o, att, x) -> h, gemv_rmsnorm([gate, up], h, norm2), gemv_glu(down, gate, up, h)."""
+        gemv_residual(o, att, x) -> h, gemv_rmsnorm([gate, up], h, norm2), gemv_glu(down, gate, up, h).
+        experts > 0 (with fused_ops): the FFN is a MoE with Mixtral's structure -- `experts` gate/up/down triples, a dense fp32 router
+        Wr [experts][hidden] on h2 = rmsnorm(h) * norm2, the top `topk` logits and a softmax over them -- run as
+        gemv_experts([gate, up], h2, ids) and gemv_experts_glu(down, gate, up, ids, weights, h), with no host sync."""
         import torch
         if ffn_sequence and post_attn_sequence:
             raise ValueError("ffn_sequence and post_attn_sequence are alternatives: the second one contains the FFN")
         if fused_ops and (ffn_sequence or post_attn_sequence):
             raise ValueError("fused_ops runs the layer's linears as single launches; it cannot be combined with a sequence")
-        self.fused_ops = fused_ops
+        if experts and (not fused_ops or ffn_sequence or post_attn_sequence):
+            raise ValueError("experts > 0 runs the routed FFN with the fused_ops launches; it needs fused_ops and no sequence")
+        if experts and not 1 <= topk <= min(experts, 8):
+            raise ValueError("topk must lie in [1, min(experts, 8)]")
+        self.fused_ops, self.experts, self.topk = fused_ops, experts, topk
         self.torch, self.hidden, self.ffn, self.heads, self.hd = torch, hidden, ffn, heads, hidden // heads
-        names = [("q", hidden, hidden), ("k", hidden, hidden), ("v", hidden, hidden), ("o", hidden, hidden), ("gate", ffn, hidden), ("up", ffn, hidden), ("down", hidden, ffn)]
+        names = [("q", hidden, hidden), ("k", hidden, hidden), ("v", hidden, hidden), ("o", hidden, hidden)]
+        ffn_names = [("gate", ffn, hidden), ("up", ffn, hidden), ("down", hidden, ffn)]
+        names += ffn_names if not experts else [("%s.%d" % (n, e), m, k) for e in range(experts) for n, m, k in ffn_names]
         self.lin = {n: QLinear(m, k, bits, group_size, zero_point, seed + i, share=share.lin[n] if share else None) for i, (n, m, k) in enumerate(names)}
         g = torch.Generator(device="cpu").manual_seed(seed)
         self.norm1 = (1.0 + 0.1 * torch.randn(hidden, generator=g)).cuda()
@@ -86,6 +96,10 @@ class DecodeLayer:
         f = lambda n: torch.zeros((1, n), device="cuda")
         self.buf = {"h1": f(hidden), "q": f(hidden), "k": f(hidden), "v": f(hidden), "att": f(hidden), "o": f(hidden), "h2": f(hidden),
                     "gate": f(ffn), "up": f(ffn), "act": f(ffn), "down": f(hidden), "x": f(hidden), "out": f(hidden), "h": f(hidden)}
+        if experts:
+            self.router = (0.05 * torch.randn((experts, hidden), generator=g)).cuda()
+            self.buf.update(gate=torch.zeros((1, topk, ffn), device="cuda"), up=torch.zeros((1, topk, ffn), device="cuda"),
+                            ids=torch.zeros((1, topk), dtype=torch.int32, device="cuda"), wts=torch.zeros((1, topk), device="cuda"))
         self.ffn_seq = self.post_seq = None
         if ffn_sequence:
             seq = tb.Sequence()
@@ -124,9 +138,16 @@ class DecodeLayer:
         a, b = t[..., 0], t[..., 1]
         return self.torch.stack((a * pos_cos - b * pos_sin, a * pos_sin + b * pos_cos), dim=-1).reshape(1, -1)
 
-    def forward(self, x, kcache, vcache, pos: int, pos_cos, pos_sin, linear=None):
+    def route(self, h2):
+        """The MoE router on h2 [1, hidden]: the ids (int32) and softmax weights of the top `topk` logits, in the buffers."""
+        vals, idx = self.torch.topk(h2 @ self.router.T, self.topk, dim=-1)
+        self.buf["ids"].copy_(idx.to(self.torch.int32))
+        self.buf["wts"].copy_(self.torch.softmax(vals, dim=-1))
+
+    def forward(self, x, kcache, vcache, pos: int, pos_cos, pos_sin, linear=None, routed=None):
         """x [1, hidden] fp32 -> [1, hidden].  kcache / vcache [heads, ctx, hd]; `linear(name, inp, out)` overrides the library call
-        (the dense fp32 reference layer in the tests)."""
+        (the dense fp32 reference layer in the tests).  MoE layers: `routed` = (ids, weights) replaces the router's choice, so that a
+        reference can follow the choice of the library path; with `linear` every expert runs densely and the chosen ones are combined."""
         torch, b = self.torch, self.buf
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
         fused = self.fused_ops and linear is None
@@ -144,6 +165,8 @@ class DecodeLayer:
             b["x"].copy_(x)
             self.post_seq.launch()                  # o(att) + x, rmsnorm, gate, up, down(silu(gate) * up) + h -> b["out"]
             return b["out"]
+        if self.experts:
+            return self.moe(x, linear, routed)
         if fused:
             tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])                          # h = o(att) + x
             tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
@@ -160,6 +183,32 @@ class DecodeLayer:
             lin("down", b["act"], b["down"])
         return h + b["down"]
 
+    def moe(self, x, linear, routed):
+        """The layer after attention with the routed FFN: h = o(att) + x, h2 = rmsnorm(h) * norm2, out = h + sum_j w_j expert_j(h2)."""
+        torch, b, E = self.torch, self.buf, self.experts
+        if linear is None:
+            tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])
+        else:
+            linear("o", b["att"], b["o"])
+            b["h"].copy_(x + b["o"])
+        b["h2"].copy_(self.rmsnorm(torch, b["h"], self.norm2))
+        if routed is None:
+            self.route(b["h2"])
+        else:
+            b["ids"].copy_(routed[0]); b["wts"].copy_(routed[1])
+        if linear is None:
+            ex = lambda n: [self.lin["%s.%d" % (n, e)].wt for e in range(E)]
+            tb.gemv_experts([ex("gate"), ex("up")], 1, b["h2"], b["ids"], [b["gate"], b["up"]])
+            tb.gemv_experts_glu(ex("down"), 1, b["gate"], b["up"], b["ids"], b["wts"], b["out"], R=b["h"])
+            return b["out"]
+        ys = torch.zeros((E, self.hidden), device="cuda")                   # every expert, then the chosen ones: no host sync
+        g, u = torch.zeros((1, self.ffn), device="cuda"), torch.zeros((1, self.ffn), device="cuda")
+        for e in range(E):
+            linear("gate.%d" % e, b["h2"], g); linear("up.%d" % e, b["h2"], u)
+            linear("down.%d" % e, torch.nn.functional.silu(g) * u, ys[e:e + 1])
+        y = (b["wts"][0, :, None] * ys[b["ids"][0].long()]).sum(dim=0, keepdim=True)
+        return b["h"] + y
+
     def free(self):
         for s in (self.ffn_seq, self.post_seq):
             if s is not None:
@@ -174,10 +223,10 @@ class DecodeModel:
     weight byte of a token streams from HBM), a KV cache of `ctx` positions, one token step per call."""
 
     def __init__(self, layers: int, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, ctx: int = 512, seed: int = 0,
-                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False):
+                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2):
         import torch
         self.torch, self.hidden, self.ctx, self.heads, self.hd = torch, hidden, ctx, heads, hidden // heads
-        kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops)
+        kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk)
         first = DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, **kw)
         self.layers: List[DecodeLayer] = [first] + [DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, share=first, **kw)
                                                     for _ in range(layers - 1)]
