@@ -74,9 +74,13 @@ TMAC_B200_API int64_t tmac_b200_graph_end(void);
 TMAC_B200_API int tmac_b200_graph_launch(int64_t graph, int times);
 TMAC_B200_API int tmac_b200_graph_free(int64_t graph);
 TMAC_B200_API int tmac_b200_sync(void);
-/* Reporting: {cluster size, warps/CTA, chunks/warp, register variant, grid.x, planes/word, symmetric LUT,
- * batch} of the last qgemm_lut launch.  cluster size 0 = the stream-K lone-launch kernel (gemv4_kernel; chunks/warp then
- * holds blocks per CTA); batch < 0 = the tensor-core (wgmma) prefill tile over -batch activation rows. */
+/* Reporting: eight ints describing the last GEMV or prefill launch (qgemm_lut, gemv and their grouped and fused-input forms).
+ * gemv3_kernel: {cluster size cs (1, 2, 4, 8), warps per CTA wpc, chunks per warp bpw, register variant MINB (3 or 4),
+ *   grid.x = row super-blocks * cs, planes per word, symmetric LUT (1) or general (0), tensors in the launch (>= 1)}.
+ *   Warp w of cluster rank k owns the K chunks [(k*wpc + w)*bpw, +bpw); these three fields fix the fp-path summation order.
+ * int8 prefill tile: {1, warps per CTA, K chunks, 1, row tiles, planes per word, 1, -N}.
+ * fp16 prefill tile: {16, warps per CTA, K chunks, stream-K (1) or not (0), grid.x, planes per word, 1, -N}.
+ * A negative last field marks a prefill tile over N activation rows. */
 TMAC_B200_API int tmac_b200_debug_last_launch(int *out8);
 /* Tuning / A-B knobs at run time.  Each key is also read once, when the library initialises, from the environment variable
  * TMAC_B200_<key in upper case>; an unknown key fails.
