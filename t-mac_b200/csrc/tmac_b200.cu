@@ -37,6 +37,10 @@
 
 using namespace tmac_b200;
 
+namespace tmac_b200 {
+template gemv3_fn pick_gemv3_in<kInTable>(int, bool, int, int, int);   // the other kinds: tmac_gemv_io.cu, tmac_gemv_experts.cu
+}
+
 namespace {
 
 thread_local std::string t_err;
@@ -287,19 +291,16 @@ int ensure_init() {
 }
 
 // ---- kernel dispatch ---------------------------------------------------------------------
-// gemv3_kernel of every grouping, fp and integer path (agq 0); the fused-LUT form is symmetric by construction
-template <bool SYM, int MINB, bool FUSED> gemv3_fn pick_gemv3_of(int pb, int qch, int agq) {
-    return with_pb<gemv3_fn>(pb, [&](auto PB) {
-        const auto kernel = [&](auto QCH, auto AGQ) -> gemv3_fn { return gemv3_kernel<PB, SYM, QCH, AGQ, MINB, FUSED>; };
-        return agq ? FpGroupings::find<gemv3_fn>(qch, agq, kernel) : IntGroupings::find<gemv3_fn>(qch, agq, kernel);
-    });
-}
-gemv3_fn pick_gemv3(int pb, bool sym, int qch, int agq, int minb) {
-    if (sym) return minb == 3 ? pick_gemv3_of<true, 3, false>(pb, qch, agq) : pick_gemv3_of<true, 4, false>(pb, qch, agq);
-    return minb == 3 ? pick_gemv3_of<false, 3, false>(pb, qch, agq) : pick_gemv3_of<false, 4, false>(pb, qch, agq);
-}
-gemv3_fn pick_gemv3_fused(int pb, int qch, int agq, int minb) {
-    return minb == 3 ? pick_gemv3_of<true, 3, true>(pb, qch, agq) : pick_gemv3_of<true, 4, true>(pb, qch, agq);
+gemv3_fn pick_gemv3(int pb, bool sym, int qch, int agq, int minb, int in) {
+    switch (in) {
+        case kInTable: return pick_gemv3_in<kInTable>(pb, sym, qch, agq, minb);
+        case kInRow: return pick_gemv3_in<kInRow>(pb, sym, qch, agq, minb);
+        case kInNorm: return pick_gemv3_in<kInNorm>(pb, sym, qch, agq, minb);
+        case kInGlu: return pick_gemv3_in<kInGlu>(pb, sym, qch, agq, minb);
+        case kInExperts: return pick_gemv3_in<kInExperts>(pb, sym, qch, agq, minb);
+        case kInExpertsGlu: return pick_gemv3_in<kInExpertsGlu>(pb, sym, qch, agq, minb);
+        default: return nullptr;
+    }
 }
 
 // Decomposition of one launch: cluster size CS (K slices of a super-block), warps per CTA, chunks
@@ -329,9 +330,24 @@ void choose_decomposition(int nrsb, int nchunk, int N, int *cs_out, int *wpc_out
 struct BatchPtrs { int n = 0; const unsigned char *const *W = nullptr; const int8_t *const *q = nullptr; const float *const *ls = nullptr,
                    *const *lb = nullptr; void *const *C = nullptr; };
 
-int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int8_t *qlut, const float *ls, const float *lb, void *C,
-                 int ldc, int c_row0, int out_f16, bool sym, const BatchPtrs *batch = nullptr, const void *fused_act = nullptr,
-                 int act_f16 = 0, const Gemv3Io *io = nullptr, int io_kind = kIoNone) {
+// What a launch reads: LUT tables (kInTable; a grouped launch takes them from its pointer table), or activation rows [N][K] from
+// which the kernel builds a symmetric LUT (the other kinds), with the kind's Gemv3Io.
+struct Gemv3In {
+    int kind = kInTable;
+    bool sym = false;                              // kInTable: symmetric tables (8 stored entries)
+    const int8_t *qlut = nullptr;                  // kInTable, single launches
+    const float *ls = nullptr, *lb = nullptr;
+    const void *act = nullptr;                     // the other kinds
+    int act_f16 = 0;
+    Gemv3Io io{};
+    static Gemv3In tables(const int8_t *qlut, const float *ls, const float *lb, bool sym) { return {kInTable, sym, qlut, ls, lb}; }
+    static Gemv3In rows(int kind, const void *act, int act_f16, const Gemv3Io &io = Gemv3Io{}) {
+        return {kind, false, nullptr, nullptr, nullptr, act, act_f16, io};
+    }
+};
+
+int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const Gemv3In &in, void *C, int ldc, int c_row0, int out_f16,
+                 const BatchPtrs *batch = nullptr) {
     const StreamLayout &L = R.L;
     if (row_begin < 0 || row_end > L.Mout || row_begin >= row_end) return fail("qgemm_lut: bad row range");
     const int rsb0 = row_begin / L.rsb, rsb1 = (row_end + L.rsb - 1) / L.rsb, nrsb = rsb1 - rsb0;
@@ -343,7 +359,9 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
         if (it != g.res.end() && it->second.L.total == L.total && it->second.L.blk == L.blk) p.Wnext = it->second.d + (size_t)rsb0 * L.rsb_stride;
         g.next_hint = 0;
     }
-    p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C;
+    const bool sym = in.kind != kInTable || in.sym;
+    p.qlut = in.qlut; p.lut_scales = in.ls; p.lut_biases = in.lb; p.C = C;
+    p.act = in.act; p.act_f16 = in.act_f16;
     p.K = L.K; p.ldc = ldc; p.row_begin = row_begin; p.row_end = row_end; p.c_row0 = c_row0; p.bits = L.bits;
     p.nrsb = nrsb; p.rsb0 = rsb0; p.nchunk = L.nchunk;
     p.ags = L.act_group_size;
@@ -355,7 +373,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
         for (int q = 0; q < g.npeer; ++q) p.Cpeer[q] = g.peer_out[q];
         g.npeer = 0;
     }
-    p.pdl_late = (g.pdl_late >= 0) ? g.pdl_late : (fused_act ? 0 : 1);   // measured: fused launches prefer the early trigger
+    p.pdl_late = (g.pdl_late >= 0) ? g.pdl_late : (in.kind != kInTable ? 0 : 1);   // measured: row inputs prefer the early trigger
     const int nb = batch ? batch->n : 0;
     if (batch) { p.nbatch = nb; p.Wv = batch->W; p.qlutv = batch->q; p.lsv = batch->ls; p.lbv = batch->lb; p.Cv = batch->C; }
     choose_decomposition(nrsb, L.nchunk, N * std::max(1, nb), &p.cs, &p.wpc, &p.bpw);
@@ -381,18 +399,15 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
         p.trace = (long long *)g.d_trace.p + per * (size_t)(g.trace_seq++ % 8);
         g.trace_ctas = nrsb * p.cs;
     }
-    if (fused_act) { p.act = fused_act; p.act_f16 = act_f16; sym = true; }
     const int agq = L.agq();
-    gemv3_fn fn = io_kind >= kIoExperts ? pick_gemv3_experts(L.pb, L.qch, agq, minb, io_kind)
-                : io_kind ? pick_gemv3_io(L.pb, L.qch, agq, minb, io_kind)
-                          : fused_act ? pick_gemv3_fused(L.pb, L.qch, agq, minb) : pick_gemv3(L.pb, sym, L.qch, agq, minb);
+    gemv3_fn fn = pick_gemv3(L.pb, sym, L.qch, agq, minb, in.kind);
     if (!fn) return fail("qgemm_lut: unsupported chunking (qch=" + std::to_string(L.qch) + ", agq=" + std::to_string(agq) + ")");
     p.nbuf = (p.bpw > 1) ? 2 : 1;
     if (g.nbuf_override > 0) p.nbuf = std::min(p.nbuf, g.nbuf_override);
     const size_t wregion = std::max((size_t)p.wpc * (p.nbuf * L.blk + (size_t)L.qch * 4 * (sym ? 8 : 16)), (size_t)p.wpc * L.rsb * 4);
     size_t smem = (size_t)p.cs * L.rsb * 4 + ((wregion + 15) & ~(size_t)15) + (size_t)p.wpc * 16;   // + warp-private mbarriers
-    if (fused_act && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
-    if (io_kind == kIoNorm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
+    if (in.kind != kInTable && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
+    if (in.kind == kInNorm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
     if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t wtx, wty;
     plane_weight_regs(L.bits, sym, &wtx, &wty);
@@ -412,7 +427,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const int
         ++na;
     }
     cfg.attrs = attr; cfg.numAttrs = na;
-    CUDA_OK(cudaLaunchKernelEx(&cfg, fn, p, wtx, wty, io ? *io : Gemv3Io{}));
+    CUDA_OK(cudaLaunchKernelEx(&cfg, fn, p, wtx, wty, in.io));
     return 0;
 }
 
@@ -543,7 +558,7 @@ int launch_gemv(const Resident &R, int row_begin, int row_end, int N, const int8
         const int rc = launch_prefill(R, N, qlut, ls, lb, C, ldc, out_f16, sym);
         if (rc <= 0) return rc;
     }
-    return launch_gemv3(R, row_begin, row_end, N, qlut, ls, lb, C, ldc, c_row0, out_f16, sym);
+    return launch_gemv3(R, row_begin, row_end, N, Gemv3In::tables(qlut, ls, lb, sym), C, ldc, c_row0, out_f16);
 }
 
 int launch_preprocessor(int K, int N, int ags, int dtype, const void *B, float *ls, float *lb, int8_t *qlut) {
@@ -1212,7 +1227,7 @@ int tmac_b200_qgemm_lut_grouped(const int64_t *handles, int count, int N, int dt
     if (g.lut_mode == 1) sym = false;
     if (g.lut_mode == 2) sym = true;
     const StreamLayout &L = R->L;
-    return launch_gemv3(*R, 0, L.Mout, N, nullptr, nullptr, nullptr, nullptr, L.Mout, 0, dtype == TMAC_B200_F16, sym, &bp);
+    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::tables(nullptr, nullptr, nullptr, sym), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
 /* q/k/v or gate/up in ONE launch with the LUT built inside it: `count` tensors of one geometry applied to the SAME activation
@@ -1229,12 +1244,12 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
     if (grouped_setup("gemv_grouped", handles, count, nullptr, nullptr, nullptr, C, &R, &bp)) return -1;
     const StreamLayout &L = R->L;
     if (!(L.int_path() || L.act_group_size <= L.ck)) return fail("gemv_grouped: the activation group must lie inside a chunk (or be the whole row)");
-    return launch_gemv3(*R, 0, L.Mout, N, nullptr, nullptr, nullptr, nullptr, L.Mout, 0, dtype == TMAC_B200_F16, true, &bp, B, dtype == TMAC_B200_F16);
+    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kInRow, B, dtype == TMAC_B200_F16), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
 // tmac_b200_gemv_rmsnorm / _glu / _residual: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
-// gemv3_kernel whose input A is transformed in the LUT build (io_kind) and whose output takes io.res.
-static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int io_kind, const void *A,
+// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.
+static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
                    const Gemv3Io &io, void *const *C) {
     if (!handles || count <= 0 || count > 65535 || !A || !C || N <= 0 || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
         return fail(what + ": bad arguments");
@@ -1247,8 +1262,7 @@ static int gemv_io(const std::string &what, const int64_t *handles, int count, i
     if (grouped_setup(what.c_str(), handles, count, nullptr, nullptr, nullptr, C, &R, &bp)) return -1;
     const StreamLayout &L = R->L;
     if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
-    return launch_gemv3(*R, 0, L.Mout, N, nullptr, nullptr, nullptr, nullptr, L.Mout, 0, dtype == TMAC_B200_F16, true, &bp, A,
-                        dtype == TMAC_B200_F16, &io, io_kind);
+    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kind, A, dtype == TMAC_B200_F16, io), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
 int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
@@ -1259,7 +1273,7 @@ int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, 
     if (!(eps >= 0.f) || !std::isfinite(eps)) return fail("gemv_rmsnorm: eps must be finite and >= 0");
     Gemv3Io io{};
     io.nw = w; io.eps = eps;
-    return gemv_io("gemv_rmsnorm", handles, count, N, dtype, kIoNorm, H, io, C);
+    return gemv_io("gemv_rmsnorm", handles, count, N, dtype, kInNorm, H, io, C);
 }
 
 int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
@@ -1268,7 +1282,7 @@ int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const vo
     if (!U) return fail("gemv_glu: bad arguments");
     Gemv3Io io{};
     io.act2 = U; io.res = R;
-    return gemv_io("gemv_glu", &handle, 1, N, dtype, kIoGlu, G, io, &C);
+    return gemv_io("gemv_glu", &handle, 1, N, dtype, kInGlu, G, io, &C);
 }
 
 int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
@@ -1277,14 +1291,14 @@ int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, con
     if (!R) return fail("gemv_residual: R must not be null");
     Gemv3Io io{};
     io.res = R;
-    return gemv_io("gemv_residual", &handle, 1, N, dtype, kIoPlain, B, io, &C);
+    return gemv_io("gemv_residual", &handle, 1, N, dtype, kInRow, B, io, &C);
 }
 
 // tmac_b200_gemv_experts / _glu: the launch of tmac_b200_gemv_grouped over count * topk slots (so each slot's sums are those of
 // gemv_grouped at N * count * topk), with a pointer table of every tensor, count * n_experts entries, from which each slot picks its
 // tensor by the id it reads on the device.  Everything is checked before anything is launched.
 static int gemv_experts(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
-                        int io_kind, const void *A, Gemv3Io io, void *const *C, int nC) {
+                        int kind, const void *A, Gemv3Io io, void *const *C, int nC) {
     if (!handles || count <= 0 || n_experts <= 0 || (long long)count * n_experts > 65535 || N <= 0 || topk < 1 || topk > 8 || !A ||
         !io.ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
         return fail(what + ": bad arguments");
@@ -1293,7 +1307,7 @@ static int gemv_experts(const std::string &what, const int64_t *handles, int cou
         return fail(what + ": device pointers only");
     for (int i = 0; i < nC; ++i)
         if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
-    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts is C[i] (kIoExpertsGlu: C[0] = C)
+    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts is C[i] (kInExpertsGlu: C[0] = C)
     for (int i = 0; i < count; ++i)
         for (int e = 0; e < n_experts; ++e) Cx[(size_t)i * n_experts + e] = C[nC > 1 ? i : 0];
     const Resident *R = nullptr;
@@ -1303,7 +1317,7 @@ static int gemv_experts(const std::string &what, const int64_t *handles, int cou
     if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
     bp.n = count * topk;                           // grid.z: the slots
     io.topk = topk; io.n_experts = n_experts;
-    if (io_kind == kIoExpertsGlu) {
+    if (kind == kInExpertsGlu) {
         const size_t cnt_bytes = (size_t)N * ((L.Mout + L.rsb - 1) / L.rsb) * sizeof(unsigned);
         if (g.d_moe_ws.ensure((size_t)N * topk * L.Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
         if (g.d_moe_cnt.cap < cnt_bytes) {
@@ -1312,8 +1326,7 @@ static int gemv_experts(const std::string &what, const int64_t *handles, int cou
         }
         io.ws = (float *)g.d_moe_ws.p; io.cnt = (unsigned *)g.d_moe_cnt.p;
     }
-    return launch_gemv3(*R, 0, L.Mout, N, nullptr, nullptr, nullptr, nullptr, L.Mout, 0, dtype == TMAC_B200_F16, true, &bp, A,
-                        dtype == TMAC_B200_F16, &io, io_kind);
+    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kind, A, dtype == TMAC_B200_F16, io), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
 int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B, const int32_t *ids,
@@ -1322,7 +1335,7 @@ int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int
     if (ensure_init()) return -1;
     Gemv3Io io{};
     io.ids = ids;
-    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kIoExperts, B, io, C, count > 0 ? count : 0);
+    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kInExperts, B, io, C, count > 0 ? count : 0);
 }
 
 int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
@@ -1332,7 +1345,7 @@ int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int
     if (!U || !weights || !C) return fail("gemv_experts_glu: bad arguments");
     Gemv3Io io{};
     io.act2 = U; io.ids = ids; io.wts = weights; io.res = R;
-    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kIoExpertsGlu, G, io, &C, 1);
+    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kInExpertsGlu, G, io, &C, 1);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {
@@ -1352,8 +1365,7 @@ int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {
     const bool can_fuse = g.use_fused && (L.int_path() || L.act_group_size <= L.ck) && g.lut_mode != 1 && !takes_prefill_tile(L, N);
     auto launch_compute = [&](const void *dB, void *dC) -> int {
         if (can_fuse)   // one launch: the GEMV builds each chunk's LUT slice itself (bit-identical tables)
-            return launch_gemv3(R, 0, L.Mout, N, nullptr, nullptr, nullptr, dC, L.Mout, 0, dtype == TMAC_B200_F16, true, nullptr, dB,
-                                dtype == TMAC_B200_F16);
+            return launch_gemv3(R, 0, L.Mout, N, Gemv3In::rows(kInRow, dB, dtype == TMAC_B200_F16), dC, L.Mout, 0, dtype == TMAC_B200_F16);
         if (g.d_qlut.ensure(qb) || g.d_ls.ensure(sb) || g.d_lb.ensure(sb)) return fail("out of device memory");
         if (launch_preprocessor(L.K, N, L.act_group_size, dtype, dB, (float *)g.d_ls.p, (float *)g.d_lb.p, (int8_t *)g.d_qlut.p)) return -1;
         return launch_gemv(R, 0, L.Mout, N, (const int8_t *)g.d_qlut.p, (const float *)g.d_ls.p, (const float *)g.d_lb.p, dC, L.Mout, 0,

@@ -1,31 +1,13 @@
-// tmac_gemv_io.cu -- the gemv3_kernel instantiations with an input transform or a residual (tmac_kernels.cuh, IO != kIoNone): the
-// fused fp-path GEMV behind an RMSNorm or SwiGLU input or before a residual add, 3 bit widths x 6 fp groupings x 2 register bounds
-// x 3 input kinds.  In their own translation unit so that they compile in parallel with tmac_b200.cu.
+// tmac_gemv_io.cu -- the gemv3_kernel instantiations that build the LUT from activation rows (tmac_kernels.cuh): the plain row with
+// an optional residual (kInRow: 3 bit widths x (6 fp + 3 integer-path groupings) x 2 register bounds), and the fp-path GEMV behind
+// an RMSNorm or SwiGLU input (kInNorm, kInGlu: 3 bit widths x 6 fp groupings x 2 register bounds each).  In their own translation
+// unit so that they compile in parallel with tmac_b200.cu.
 #include "tmac_kernels.cuh"
-#include "tmac_layout.h"
 
 namespace tmac_b200 {
 
-namespace {
-template <int MINB, int IO> gemv3_fn pick_io(int pb, int qch, int agq) {
-    return with_pb<gemv3_fn>(pb, [&](auto PB) {
-        return FpGroupings::find<gemv3_fn>(qch, agq, [&](auto QCH, auto AGQ) -> gemv3_fn {
-            return gemv3_kernel<PB, true, QCH, AGQ, MINB, true, IO>;
-        });
-    });
-}
-template <int MINB> gemv3_fn pick_io_kind(int pb, int qch, int agq, int io) {
-    switch (io) {
-        case kIoPlain: return pick_io<MINB, kIoPlain>(pb, qch, agq);
-        case kIoNorm: return pick_io<MINB, kIoNorm>(pb, qch, agq);
-        case kIoGlu: return pick_io<MINB, kIoGlu>(pb, qch, agq);
-        default: return nullptr;
-    }
-}
-}  // namespace
-
-gemv3_fn pick_gemv3_io(int pb, int qch, int agq, int minb, int io) {
-    return minb == 3 ? pick_io_kind<3>(pb, qch, agq, io) : pick_io_kind<4>(pb, qch, agq, io);
-}
+template gemv3_fn pick_gemv3_in<kInRow>(int, bool, int, int, int);
+template gemv3_fn pick_gemv3_in<kInNorm>(int, bool, int, int, int);
+template gemv3_fn pick_gemv3_in<kInGlu>(int, bool, int, int, int);
 
 }  // namespace tmac_b200

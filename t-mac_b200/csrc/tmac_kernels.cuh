@@ -32,6 +32,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "tmac_layout.h"
+
 namespace tmac_b200 {
 
 // (a & b) | c in ONE LOP3 (the compiler splits it in two when b and c are immediates)
@@ -276,7 +278,7 @@ __device__ __forceinline__ uint32_t row_codes(const uint32_t *w4, int k, int i) 
 // ------------------------------------------------------------------------------------------
 // The activation LUT: the operation order of the AVX2 branch of lut_ctor.cc, with explicit round-to-nearest operations so
 // that no FMA contraction can change a rounding.  Every kernel that builds LUT bytes, LUT scales or LUT biases
-// (preprocessor_kernel, gemv3_kernel's FUSED path, chain_kernel, seq_kernel) builds them with these functions.
+// (preprocessor_kernel, gemv3_kernel's row inputs, chain_kernel, seq_kernel) builds them with these functions.
 // ------------------------------------------------------------------------------------------
 // abs-sum of one K-group, whose maximum over the activation group gives the LUT scale (lut_ctor.cc:242-256; association :251)
 __device__ __forceinline__ float lut_abs_sum(float x0, float x1, float x2, float x3) {
@@ -380,7 +382,7 @@ __device__ __forceinline__ float rms_scale(float h, float inv, float w) { return
 // too: the fp32 operation order decides the result, so they run this one code.  The block is the stream layout (tmac_layout.h):
 // QCH quads of 32 lanes x 16 code bytes, then RSB weight scales and (zp) RSB zero points of sd bytes each; tab is the warp's LUT
 // slice of the chunk.  These are macros, not functions: the compiler simplifies a callee before it inlines it, and as
-// __forceinline__ functions the step changed the kernels' SASS (gemv3_kernel<2,true,8,4,3,true> 1752 -> 1768 instructions,
+// __forceinline__ functions the step changed the kernels' SASS (the row-input gemv3_kernel<2,true,8,4,3> 1752 -> 1768 instructions,
 // chain_kernel<2,8,4> another shared-memory load mix).  Expanded in place they compile to the instructions of the code they
 // replaced.
 // ------------------------------------------------------------------------------------------
@@ -489,10 +491,10 @@ struct Gemv3Params {
     const int8_t *const *qlutv;
     const float *const *lsv, *const *lbv;
     void *const *Cv;
-    // fused LUT construction (FUSED instantiations): activations [N][K] f32 or f16 instead of qlut / lut_scales / lut_biases
+    // LUT built inside the kernel (IN != kInTable): activations [N][K] f32 or f16 instead of qlut / lut_scales / lut_biases
     const void *act;
     int act_f16;
-    int ioff;                      // fused integer path (activation group = K): byte offset of the row-scan scratch in shared memory
+    int ioff;                      // byte offset in shared memory of the integer path's row-scan scratch / kInNorm's row
     size_t rsb_stride;
     float scale0;
     long long *trace;
@@ -501,20 +503,23 @@ struct Gemv3Params {
     int npeer;
     void *Cpeer[7];
 };
-// The input transform and residual of the gemv3_kernel instantiations with IO != kIoNone: the kernel's last parameter, so that
-// Gemv3Params, wtx and wty keep their parameter offsets.  The plain input / the norm's h / the GLU's g is p.act.
-// The routed-expert kinds (kIoExperts, kIoExpertsGlu) pick each slot's tensor on the device: slot z = i * topk + j of token n
+// The input of a gemv3_kernel instantiation, its template parameter IN: kInTable reads QLUT / LUT_Scales / LUT_Biases; every other
+// kind builds the LUT from activation rows p.act (the plain row, the norm's h, the GLU's g) with a symmetric table.
+// The routed-expert kinds (kInExperts, kInExpertsGlu) pick each slot's tensor on the device: slot z = i * topk + j of token n
 // (blockIdx.z, blockIdx.y) runs pointer-table entry i * n_experts + ids[n * topk + j].
-enum : int { kIoNone = 0, kIoPlain = 1, kIoNorm = 2, kIoGlu = 3, kIoExperts = 4, kIoExpertsGlu = 5 };
+enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5 };
+// The input transform and residual of the row kinds: the kernel's last parameter, so that Gemv3Params, wtx and wty keep their
+// parameter offsets.
 struct Gemv3Io {
-    const void *act2;              // kIoGlu, kIoExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
-    const float *nw;               // kIoNorm: the norm weight w [K] (16-byte aligned)
-    float eps;                     // kIoNorm
-    const void *res;               // residual r [N][ldc] of the output's dtype, or null; may equal C
+    const void *act2;              // kInGlu, kInExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
+    const float *nw;               // kInNorm: the norm weight w [K] (16-byte aligned)
+    float eps;                     // kInNorm
+    const void *res;               // fp path, kInRow / kInNorm / kInGlu / kInExpertsGlu: residual r [N][ldc] of the output's dtype,
+                                   // or null; may equal C
     const int32_t *ids;            // experts: [N][topk], written by earlier work in the stream (read after the dependency wait)
-    const float *wts;              // kIoExpertsGlu: combine weights [N][topk]
-    float *ws;                     // kIoExpertsGlu: the slots' fp32 rows [N][topk][ldc]
-    unsigned *cnt;                 // kIoExpertsGlu: arrivals per (token, row super-block) [N][nrsb], 0 between launches
+    const float *wts;              // kInExpertsGlu: combine weights [N][topk]
+    float *ws;                     // kInExpertsGlu: the slots' fp32 rows [N][topk][ldc]
+    unsigned *cnt;                 // kInExpertsGlu: arrivals per (token, row super-block) [N][nrsb], 0 between launches
     int topk, n_experts;           // experts
 };
 __device__ __forceinline__ long long globaltimer_ns() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
@@ -619,26 +624,27 @@ constexpr int kG3MaxWarps = 8;
 
 // MINB = minimum resident CTAs per SM the register allocation is tuned for: 3 (85 registers, more ILP;
 // best for a single launch per tensor) or 4 (64 registers, more CTAs in flight; best for grouped launches).
-// FUSED = build the LUT slice of each chunk inside the GEMV from the activation row (with the LUT functions above,
+// IN != kInTable: build the LUT slice of each chunk inside the GEMV from the activation row (with the LUT functions above,
 // as preprocessor_kernel, so QLUT bytes, LUT scales and LUT biases are bit-identical to the two-kernel path)
 // instead of reading QLUT / LUT_Scales / LUT_Biases.  Requires SYM.  AGQ > 0: activation
 // group inside a chunk, scale and bias per chunk by warp shuffles.  AGQ == 0 (integer path, ONE activation group
-// = the whole row, BitNet): every CTA scans the row once (K * 4 bytes, L2-resident) for the row-wide abs-sum
-// maximum -- cheaper than a cluster-wide exchange, which costs a rendezvous -- and the cluster leader also forms
+// = the whole row, BitNet; kInTable and kInRow only): every CTA scans the row once (K * 4 bytes, L2-resident) for the row-wide
+// abs-sum maximum -- cheaper than a cluster-wide exchange, which costs a rendezvous -- and the cluster leader also forms
 // the row's LUT bias in the reference's order (addv tree per 32 activations, serial over the blocks).
-// IO (fused fp path only, instantiated in tmac_gemv_io.cu): the LUT input of row n is a transform of the activation rows -- kIoNorm
-// a[k] = rms_scale(h[k], inv_n, w[k]), kIoGlu a[k] = swiglu(g[k], u[k]), kIoPlain a = the row -- built into the chunk's slice
-// with lut_slice as a plain input; the leader adds io.res (when not null) to the row sums before the store.
-// Routed experts (instantiated in tmac_gemv_experts.cu): slot z = i * topk + j of token n takes its tensor from the pointer table at
-// i * n_experts + ids[n][j], read after the dependency wait, so the slot's first block request waits for it too.  kIoExperts reads row
-// n and stores row n * topk + j of C[i]; kIoExpertsGlu reads row n * topk + j of g and u, stores its rows into io.ws and counts
+// The LUT input of row n is the row itself (kInRow) or a transform of the activation rows -- kInNorm a[k] = rms_scale(h[k], inv_n,
+// w[k]), kInGlu a[k] = swiglu(g[k], u[k]) -- built into the chunk's slice with lut_slice as a plain input; on the fp path the
+// leader adds io.res (when not null) to the row sums before the store.
+// Routed experts: slot z = i * topk + j of token n takes its tensor from the pointer table at
+// i * n_experts + ids[n][j], read after the dependency wait, so the slot's first block request waits for it too.  kInExperts reads row
+// n and stores row n * topk + j of C[i]; kInExpertsGlu reads row n * topk + j of g and u, stores its rows into io.ws and counts
 // itself in io.cnt, and the leader that completes a (token, row super-block) combines the topk rows in ascending j into C.  A slot
 // whose id is outside [0, n_experts) streams no block and yields quiet NaN rows.
-template <int PB, bool SYM, int QCH, int AGQ, int MINB, bool FUSED = false, int IO = kIoNone>
+template <int PB, bool SYM, int QCH, int AGQ, int MINB, int IN>
 __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gemv3Params p, const uint32_t wtx, const uint32_t wty,
                                                                        const Gemv3Io io) {
-    static_assert(IO == kIoNone || (FUSED && SYM && AGQ > 0), "input transforms: fused fp path only");
-    constexpr bool EXPERTS = IO == kIoExperts || IO == kIoExpertsGlu;
+    static_assert(IN == kInTable || SYM, "a LUT built from activation rows is symmetric");
+    static_assert(IN == kInTable || IN == kInRow || AGQ > 0, "input transforms and experts: fp path only");
+    constexpr bool EXPERTS = IN == kInExperts || IN == kInExpertsGlu;
     constexpr int RW = 8 / PB;
     constexpr int RSB = 32 * RW;
     constexpr int TB = SYM ? 8 : 16;              // table bytes per group in shared memory
@@ -679,12 +685,12 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         const int z = blockIdx.z;
         if (EXPERTS) Cb = p.Cv[xi * io.n_experts];
         else { Wb = p.Wv[z]; Cb = p.Cv[z]; }
-        if (!FUSED) { qb = p.qlutv[z]; lsb = p.lsv[z]; lbb = p.lbv[z]; }   // fused: the tensors of the group share the activation rows
+        if (IN == kInTable) { qb = p.qlutv[z]; lsb = p.lsv[z]; lbb = p.lbv[z]; }   // else the tensors of the group share the activation rows
     }
     const unsigned char *rsb_base = Wb + (size_t)rsb * p.rsb_stride;
     const int nag = p.K / p.ags;
-    const int arow = IO == kIoExpertsGlu ? n * io.topk + xj : n;   // the activation row of this CTA
-    // fused: the 4 activations from element k of the row of act (p.act, or kIoGlu's u), fp32 or fp16
+    const int arow = IN == kInExpertsGlu ? n * io.topk + xj : n;   // the activation row of this CTA
+    // row inputs: the 4 activations from element k of the row of act (p.act, or the GLU's u), fp32 or fp16
     auto load_group = [&](size_t k, float4 &x, const void *act = nullptr) {
         const size_t k0 = (size_t)arow * p.K + k;
         if (!act) act = p.act;
@@ -729,7 +735,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     float row_scale = 0.f, row_ts = 0.f;          // fused integer path: LUT scale of the row and its reciprocal
     float *iscr = reinterpret_cast<float *>(smem + p.ioff);   // [K/32] block sums (leader) | [8] warp maxima | [1] bias
     bool scan_split = false;                      // fused integer path: the cluster splits the row scan (else every CTA scans the row)
-    if (FUSED && INT_PATH) {
+    if (IN != kInTable && INT_PATH) {
         // Row-wide LUT scale and bias (lut_ctor.cc:232-260 partial_max over the whole row, :157 bias) without a preprocessor launch.
         // Short rows (one round of four 16-byte loads per thread covers the row, K = 3200): every CTA scans the whole row itself,
         // no exchange.  Long rows (K = 8640): that is 200 CTAs x 34 KB of reads on the same few L2 lines, several serial rounds;
@@ -807,8 +813,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             if (lane == 0) *bias_out = bias;       // forwarded to the leader with the partial sums below
         }
     }
-    float inv = 0.f;                              // kIoNorm: 1 / rms of the row
-    if (IO == kIoNorm) {
+    float inv = 0.f;                              // kInNorm: 1 / rms of the row
+    if (IN == kInNorm) {
         // Every CTA computes inv itself.  All threads stage the row, widened to fp32, in shared memory (iscr [K] | inv), with
         // their loads in flight together; warp 0 then sums its squares in the order of rms_sumsq / rms_warp_sum.
         const int ngrp = p.K >> 2, nth = WPC * 32;
@@ -839,16 +845,16 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     for (int c = c_first; c < c_end; ++c) {
         // ---- LUT slice of this chunk -> warp-private table (lane = group) ---------------------
         float lsv[NAG], lbsum = 0.f;
-        if (FUSED) {
+        if (IN != kInTable) {
             constexpr int NG = QCH * 4;            // lane = K-group of the chunk
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (IO == kIoNorm) {
+            if (IN == kInNorm) {
                 if (lane < NG) {
                     const size_t g = (size_t)c * NG + lane;
                     const float4 h = reinterpret_cast<const float4 *>(iscr)[g], w = __ldg(reinterpret_cast<const float4 *>(io.nw) + g);
                     x = make_float4(rms_scale(h.x, inv, w.x), rms_scale(h.y, inv, w.y), rms_scale(h.z, inv, w.z), rms_scale(h.w, inv, w.w));
                 }
-            } else if (IO == kIoGlu || IO == kIoExpertsGlu) {
+            } else if (IN == kInGlu || IN == kInExpertsGlu) {
                 if (lane < NG) {
                     float4 gv, uv;
                     load_group(((size_t)c * NG + lane) * 4, gv);
@@ -907,7 +913,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
     if (tid == 0) TMAC_TRACE(5);
     const int nthreads = WPC * 32;
     if (p.cs > 1 && !scan_split) cluster_wait();  // every CTA of the cluster has started: its shared memory may be written
-    if (FUSED && INT_PATH && p.cs > 1 && rank == p.cs - 1 && tid == (WPC - 1) * 32) {
+    if (IN != kInTable && INT_PATH && p.cs > 1 && rank == p.cs - 1 && tid == (WPC - 1) * 32) {
         float *bias_out = iscr + (p.K >> 5) + kG3MaxWarps;
         st_cluster_f32(bias_out, 0, *bias_out);    // written by this thread after the row scan
     }
@@ -934,17 +940,17 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         if (row >= p.row_begin && row < p.row_end) {
             float out;
             if (INT_PATH)
-                out = int_path_out(isum, FUSED ? row_scale : __ldg(lsg), FUSED ? iscr[(p.K >> 5) + kG3MaxWarps] : __ldg(lbg), p.scale0);
+                out = int_path_out(isum, IN != kInTable ? row_scale : __ldg(lsg), IN != kInTable ? iscr[(p.K >> 5) + kG3MaxWarps] : __ldg(lbg), p.scale0);
             else
                 out = fsum;
             if (EXPERTS) {                          // row n * topk + j of C[i] / of the workspace (c_row0 = 0)
                 const size_t o = (size_t)(n * io.topk + xj) * p.ldc + row;
                 if (bad) out = __int_as_float(0x7fffffff);
-                if (IO == kIoExperts) store_out(Cb, o, out, p.out_f16);
+                if (IN == kInExperts) store_out(Cb, o, out, p.out_f16);
                 else io.ws[o] = out;
             } else {
                 const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
-                if (IO != kIoNone && io.res)           // read, then written by this thread: the residual may be C itself
+                if (IN != kInTable && !INT_PATH && io.res)   // read, then written by this thread: the residual may be C itself
                     out = __fadd_rn(out, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
                 store_out(Cb, o, out, p.out_f16);
                 for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
@@ -952,7 +958,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             }
         }
     }
-    if (IO == kIoExpertsGlu) {
+    if (IN == kInExpertsGlu) {
         // The combine.  This slot's rows are in io.ws; thread 0 counts the slot in (release, for every thread's stores: they precede
         // it by the barrier) and learns whether it completes the token's row super-block (acquire, for the other slots' rows).  The
         // leader that completes it adds the topk rows in ascending j -- not in arrival order -- and resets the counter for the next
@@ -984,10 +990,33 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 }
 
 typedef void (*gemv3_fn)(const Gemv3Params, const uint32_t, const uint32_t, const Gemv3Io);
-// the fused fp-path instantiations with an input transform (IO != kIoNone), in tmac_gemv_io.cu
-gemv3_fn pick_gemv3_io(int pb, int qch, int agq, int minb, int io);   // null: grouping not instantiated
-// the routed-expert instantiations (io = kIoExperts / kIoExpertsGlu), in tmac_gemv_experts.cu
-gemv3_fn pick_gemv3_experts(int pb, int qch, int agq, int minb, int io);
+// gemv3_kernel<PB, SYM, QCH, AGQ, MINB, IN> for a tensor's (pb, qch, agq), the LUT's symmetry (kInTable; the other kinds are
+// symmetric) and minb; null for a grouping that is not instantiated.  Each kind's kernels are compiled in the one translation unit
+// that instantiates pick_gemv3_in for it, so that the kinds compile in parallel: kInTable in tmac_b200.cu, kInRow, kInNorm and
+// kInGlu in tmac_gemv_io.cu, kInExperts and kInExpertsGlu in tmac_gemv_experts.cu.
+template <int IN> gemv3_fn pick_gemv3_in(int pb, bool sym, int qch, int agq, int minb) {
+    const auto pick = [&](auto SYM, auto MINB) {
+        return with_pb<gemv3_fn>(pb, [&](auto PB) {
+            const auto kernel = [&](auto QCH, auto AGQ) -> gemv3_fn { return gemv3_kernel<PB, SYM, QCH, AGQ, MINB, IN>; };
+            if constexpr (IN == kInTable || IN == kInRow) {
+                if (!agq) return IntGroupings::find<gemv3_fn>(qch, agq, kernel);
+            }
+            return FpGroupings::find<gemv3_fn>(qch, agq, kernel);
+        });
+    };
+    using Minb3 = std::integral_constant<int, 3>;
+    using Minb4 = std::integral_constant<int, 4>;
+    if constexpr (IN == kInTable) {
+        if (!sym) return minb == 3 ? pick(std::false_type{}, Minb3{}) : pick(std::false_type{}, Minb4{});
+    }
+    return minb == 3 ? pick(std::true_type{}, Minb3{}) : pick(std::true_type{}, Minb4{});
+}
+extern template gemv3_fn pick_gemv3_in<kInTable>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInRow>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInNorm>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInGlu>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInExperts>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInExpertsGlu>(int, bool, int, int, int);
 
 // ------------------------------------------------------------------------------------------
 // cbits_kernel (debug / parity gate G2): per-plane int32 sums in the reference plane layout.
