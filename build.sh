@@ -9,7 +9,7 @@ OBJ=$(mktemp -d)
 trap 'rm -rf "$OBJ"' EXIT
 FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC,-fvisibility=hidden,-O2"
 PIDS=""
-for tu in tmac_b200 tmac_seq tmac_chain_batch tmac_gemv_io tmac_gemv_experts; do
+for tu in tmac_b200 tmac_seq tmac_chain_batch tmac_gemv_io tmac_gemv_experts tmac_prefill_experts; do
   $NVCC $FLAGS -c -o "$OBJ/$tu.o" t-mac_b200/csrc/$tu.cu "$@" &
   PIDS="$PIDS $!"
 done

@@ -209,6 +209,35 @@ TMAC_B200_API int tmac_b200_gemv_experts(const int64_t *handles, int count, int 
                                          const int32_t *ids, int topk, void *const *C);
 TMAC_B200_API int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
                                              const int32_t *ids, const float *weights, int topk, const void *R, void *C);
+/* Routed MoE experts at prefill sizes (a prompt, a decode batch of many requests): the arguments and output layouts of
+ * gemv_experts / gemv_experts_glu, so a caller switches between the two forms by N (from N * topk of about 16 * n_experts on
+ * Mixtral-8x7B's FFN, DESIGN.md 3.3), but each expert's tokens are grouped on the device and run on the prefill tiles (wgmma), which stream each
+ * expert's weights once per 128 rows instead of once per slot.  Still no host sync, and the calls are graph-capturable.
+ *   Slots.  Slot s = n * topk + j.  The slots of expert e in ascending s are that expert's rows.  The plain form's row of slot s is
+ *           B[n]; the GLU form's is a_s = swiglu(G[n][j], U[n][j]) in fp32, rounded as for seq_add_gemv_glu.
+ *   Per-slot equality.  Slot s's output row equals, bit for bit, row r of tmac_b200_gemv(handle_e, n_e, dtype, rows_e, .) on the same
+ *           tile kind, where rows_e are expert e's n_e rows in order and s is the r-th of them: the preprocessor builds each row's LUT
+ *           on its own, a token column of either tile depends only on its own column, and an expert's token tiles start at its first
+ *           row, so each row sits at the tile position it has in that dense call.  Against the float oracle: the fp16 tile within
+ *           5e-4 of max|C|, the int8 tile within 2e-5.
+ *   Tile.   One kind per launch: the fp16 tile when the prefill16 knob is on and N * topk >= 256 * n_experts, else the int8 tile
+ *           (prefill, prefill_min_n and pf_streamk do not apply; no stream-K).  tmac_b200_debug_last_launch reports that tile in its
+ *           own format with -(N * topk) as the last field.
+ *   prefill_experts:     C[i][n][j] = tensor i of expert ids[n][j] applied to B[n]; layouts as tmac_b200_gemv_experts.
+ *   prefill_experts_glu: C[n] = fadd_rn(...fadd_rn(fmul_rn(w_0, y_0), fmul_rn(w_1, y_1))..., fmul_rn(w_{topk-1}, y_{topk-1}))
+ *                        (+ R[n]), y_j the fp32 row of slot n * topk + j; the expression and layouts of gemv_experts_glu (no fma
+ *                        contraction, fp16 R widened, rounded once for F16, R may equal C).
+ * Tensors: W2/W3/W4 fp-path tensors (per-row scales with or without zero points, K % 128 == 0, chunk 128/64/32 K, act group inside
+ * the chunk), one geometry for all.  An id outside [0, n_experts) is dropped from the grouping and nothing is read out of bounds:
+ * prefill_experts stores quiet NaN in that slot's row, prefill_experts_glu in that token's whole output; other slots and tokens are
+ * unaffected.  Repeated ids are independent slots.  -1 with a message, nothing launched: W1, integer-path and other tensors the tiles
+ * do not take (gemv_experts is the call for them), host pointers, topk outside 1..8, n_experts outside 1..256,
+ * count * n_experts > 65535, mixed geometry, an armed tmac_b200_peer_outputs (disarmed).  Workspaces are library buffers that grow
+ * with N * topk, K and Mout: make one eager call at the largest of them before capturing a call in a CUDA graph. */
+TMAC_B200_API int tmac_b200_prefill_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B,
+                                            const int32_t *ids, int topk, void *const *C);
+TMAC_B200_API int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
+                                                const int32_t *ids, const float *weights, int topk, const void *R, void *C);
 /* Fused convenience (llama_cpp_init + llama_cpp_compute of the whole tensor in one call,
  * workspaces owned by the library): C [N][M] = qgemm_lut(preprocessor(B)). */
 TMAC_B200_API int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C);

@@ -140,6 +140,7 @@ struct Context {
     // workspaces
     DevBuf d_b, d_qlut, d_ls, d_lb, d_c, d_cbits, d_trace, d_tiles, d_pf_scratch, d_pf_flags;
     DevBuf d_moe_ws, d_moe_cnt;          // tmac_b200_gemv_experts_glu: the slots' rows and the arrival counters (zero between launches)
+    DevBuf d_moe_route, d_moe_act;       // tmac_b200_prefill_experts / _glu: tile table + sorted slots; the GLU form's fp32 inputs
     int trace = 0, trace_ctas = 0, trace_seq = 0;
     int chain_flags = 0;                 // resident chain (tmac_chain.cuh): bit 0 = grid-barrier form (comparison); default: data flow
     int chain_ahead = 1;                 // resident chain: 0 = never the decode-ahead instantiation (comparison); default: when it fits
@@ -706,7 +707,8 @@ void tmac_b200_shutdown(void) {
         std::free(kv.second.host_scales);
     }
     g.res.clear();
-    for (DevBuf *b : {&g.d_b, &g.d_qlut, &g.d_ls, &g.d_lb, &g.d_c, &g.d_cbits, &g.d_trace, &g.d_tiles, &g.d_pf_scratch, &g.d_pf_flags}) { if (b->p) cudaFree(b->p); b->p = nullptr; b->cap = 0; }
+    for (DevBuf *b : {&g.d_b, &g.d_qlut, &g.d_ls, &g.d_lb, &g.d_c, &g.d_cbits, &g.d_trace, &g.d_tiles, &g.d_pf_scratch, &g.d_pf_flags,
+                      &g.d_moe_route, &g.d_moe_act}) { if (b->p) cudaFree(b->p); b->p = nullptr; b->cap = 0; }
     for (HostLut &e : g.hluts) {
         for (DevBuf *b : {&e.dq, &e.dls, &e.dlb}) { if (b->p) cudaFree(b->p); b->p = nullptr; b->cap = 0; }
         if (e.res.p) cudaFreeHost(e.res.p);
@@ -1346,6 +1348,131 @@ int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int
     Gemv3Io io{};
     io.act2 = U; io.ids = ids; io.wts = weights; io.res = R;
     return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kInExpertsGlu, G, io, &C, 1);
+}
+
+// The tile of a routed launch: the fp16 tile when it is on and the average expert fills one of its 256-token tiles,
+// N * topk >= 256 * n_experts, else the int8 tile.  On Mixtral-8x7B's FFN (8 experts, top-2, W2 and W4) the int8 tile is up to 1.5x
+// faster at N = 256 and 512, the fp16 tile faster at N = 2048 and with uniform routing at 1024 (H100 SXM at 700 W, DESIGN.md 3.3).
+static bool experts_take_tile16(int N, int topk, int n_experts) { return g.use_prefill16 && (long long)N * topk >= 256LL * n_experts; }
+
+// tmac_b200_prefill_experts / _glu: route the slots on the device (pf_route_kernel), build the LUT of every input row once
+// (plain: B's N rows; GLU: the N * topk rows swiglu(G[s], U[s]), materialised in fp32), gather each table entry's LUT records, run
+// the routed tile over (row tiles, table entries, count), and for the GLU form combine the slots' fp32 rows.  Everything is checked
+// and every workspace allocated before anything is launched.
+static int prefill_experts(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
+                           int N, int dtype, int topk, const void *A, const void *U, const int32_t *ids, const float *wts, const void *Rres,
+                           void *const *C) {
+    const bool glu = U != nullptr;
+    if (g.npeer) { g.npeer = 0; return fail(what + ": peer outputs are for N = 1 single-tensor launches"); }
+    if (!handles || count <= 0 || N <= 0 || !A || !ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
+        return fail(what + ": bad arguments");
+    if (topk < 1 || topk > 8) return fail(what + ": topk must be 1..8");
+    if (n_experts < 1 || n_experts > 256) return fail(what + ": n_experts must be 1..256");
+    if ((long long)count * n_experts > 65535) return fail(what + ": count * n_experts must be <= 65535");
+    if (!is_device_ptr(A) || !is_device_ptr(ids) || (glu && (!is_device_ptr(U) || !is_device_ptr(wts))) || (Rres && !is_device_ptr(Rres)))
+        return fail(what + ": device pointers only");
+    const int nC = glu ? 1 : count;
+    for (int i = 0; i < nC; ++i)
+        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
+    auto it0 = g.res.find(handles[0]);
+    if (it0 == g.res.end()) return fail(what + ": bad weight handle");
+    const StreamLayout &L = it0->second.L;
+    const bool tile_ok = !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0 &&
+                         (L.pb == 2 || L.pb == 4);
+    if (!tile_ok)
+        return fail(what + ": the tiles take W2/W3/W4 fp-path tensors (per-row scales, K % 128 == 0, chunk 128/64/32 K, act group inside "
+                    "the chunk); use " + gemv_name + " for the others");
+    const int S = N * topk, Mout = L.Mout, K = L.K, f16 = dtype == TMAC_B200_F16;
+    if (glu && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
+    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts + e: C[i] (GLU: the slots' fp32 rows)
+    for (int i = 0; i < count; ++i)
+        for (int e = 0; e < n_experts; ++e) Cx[(size_t)i * n_experts + e] = glu ? g.d_moe_ws.p : C[i];
+    const Resident *R = nullptr;
+    BatchPtrs bp;
+    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, Cx.data(), &R, &bp)) return -1;
+    const int agq = L.agq();
+    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, agq);
+    if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
+    // shared memory of both tiles as in launch_prefill
+    const size_t rawsz = ((size_t)(8 / L.qch) * L.blk + 127) & ~(size_t)127;
+    const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
+    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;
+    const int nmain = K / 64, nextra = (L.nchunk + 31) / 32;
+    const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
+    const size_t rec = pf_rec_bytes(false, L.qch, agq);
+    const size_t smem8 = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
+    const bool t16 = experts_take_tile16(N, topk, n_experts) && smem16 <= 227 * 1024;
+    if (!t16 && smem8 > 225 * 1024) return fail(what + ": the tensor's blocks do not fit the int8 tile's shared memory");
+    const int T = t16 ? kP16NT : kPfNT;
+    const long long cap = S / T + std::min(n_experts, S);
+    if (cap > 65535) return fail(what + ": N * topk too large for one launch");
+    const int rows = glu ? S : N, nag = K / L.act_group_size, nsteps = t16 ? nmain + nextra : nmain;
+    const size_t recb = t16 ? (size_t)kP16BBytes : rec;
+    if (g.d_moe_route.ensure((size_t)cap * sizeof(int4) + (size_t)S * sizeof(int)) || (glu && g.d_moe_act.ensure((size_t)S * K * sizeof(float))) ||
+        g.d_qlut.ensure((size_t)rows * K * 4) || g.d_ls.ensure((size_t)rows * nag * 4) || g.d_lb.ensure((size_t)rows * nag * 4) ||
+        g.d_tiles.ensure((size_t)cap * nsteps * recb))
+        return fail(what + ": out of device memory (workspace)");
+    int4 *tiles = (int4 *)g.d_moe_route.p;
+    int *perm = (int *)(tiles + cap);
+    const int8_t *qlut = (const int8_t *)g.d_qlut.p;
+    const float *ls = (const float *)g.d_ls.p, *lb = (const float *)g.d_lb.p;
+    unsigned char *recs = (unsigned char *)g.d_tiles.p;
+    const cudaStream_t st = g.stream();
+
+    pf_route_launch(ids, S, n_experts, T, (int)cap, tiles, perm, glu ? nullptr : bp.C, count, Mout, f16, st);
+    CUDA_OK(cudaGetLastError());
+    if (glu) {
+        pf_swiglu_launch(A, U, f16, (size_t)S * K, (float *)g.d_moe_act.p, st);
+        CUDA_OK(cudaGetLastError());
+        if (launch_preprocessor(K, S, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
+    } else if (launch_preprocessor(K, N, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
+    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts};
+    const int div = glu ? 1 : topk, out_f16 = glu ? 0 : f16;
+    const dim3 grid(nrt, (unsigned)cap, count);
+    if (t16) {
+        fk.lut16<<<dim3(nsteps, (unsigned)cap), 256, 0, st>>>(qlut, ls, lb, recs, K, nmain, nextra, tiles, perm, div);
+        CUDA_OK(cudaGetLastError());
+        Prefill16Params q{};
+        q.N = N; q.K = K; q.Mout = Mout; q.ldc = Mout; q.out_f16 = out_f16;
+        q.nchunk = L.nchunk; q.zp = L.zp; q.sd = L.sd; q.blk_bytes = (int)L.blk; q.nmain = nmain; q.nextra = nextra;
+        q.rsb_stride = L.rsb_stride; q.tiles = recs; q.nrsb = L.nrsb; q.nrt = nrt; q.bits = L.bits; q.ntiles = nrt * (int)cap;
+        CUDA_OK(cudaFuncSetAttribute((const void *)fk.tile16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
+        fk.tile16<<<grid, kP16Threads, smem16, st>>>(q, route);
+        CUDA_OK(cudaGetLastError());
+        g.last_launch[0] = 16; g.last_launch[1] = kP16Threads / 32; g.last_launch[3] = 0;
+    } else {
+        fk.lut<<<dim3(nsteps, (unsigned)cap), 128, 0, st>>>(qlut, ls, lb, recs, K, tiles, perm, div);
+        CUDA_OK(cudaGetLastError());
+        PrefillParams p{};
+        p.lut_tiles = recs; p.N = N; p.K = K; p.Mout = Mout; p.ldc = Mout; p.out_f16 = out_f16;
+        p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride;
+        p.nrsb = L.nrsb; p.bits = L.bits; p.qch = L.qch;
+        CUDA_OK(cudaFuncSetAttribute((const void *)fk.tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem8));
+        fk.tile<<<grid, kPfThreads2, smem8, st>>>(p, route);
+        CUDA_OK(cudaGetLastError());
+        g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[3] = 1;
+    }
+    g.last_launch[2] = L.nchunk; g.last_launch[4] = nrt; g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -S;
+    if (glu) {
+        pf_combine_launch((const float *)g.d_moe_ws.p, ids, wts, topk, n_experts, Rres, C[0], N, Mout, f16, st);
+        CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+int tmac_b200_prefill_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B, const int32_t *ids,
+                              int topk, void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    return prefill_experts("prefill_experts", "gemv_experts", handles, count, n_experts, N, dtype, topk, B, nullptr, ids, nullptr, nullptr, C);
+}
+
+int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
+                                  const int32_t *ids, const float *weights, int topk, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    if (!U || !weights || !C) return fail("prefill_experts_glu: bad arguments");
+    return prefill_experts("prefill_experts_glu", "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, ids, weights, R, &C);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

@@ -131,19 +131,26 @@ constexpr int kPfTab = 16384;
 __host__ __device__ constexpr int pf_rec_bytes(bool int_path, int qch = 8, int agq = 4) {
     return int_path ? kPfTab : kPfTab + 512 * ((agq == 2 ? 2 : 1) + (qch == 2 ? 2 : 1) * (qch / agq));   // PfGroups NLS + NLB
 }
-template <bool INT_PATH, int QCH = 8, int AGQ = 4>
-__global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K) {
+//
+// Routed experts (tmac_prefill_experts.cu) gather their records: the record of table entry k (PfRoute) at token position t holds
+// LUT row perm[start + t] / div (div = topk: a token's slots share its row; div = 1: one row per slot); positions >= ntok are zero.
+// Both record kernels of a tile share the body of one record (token row n, `live` = the token exists).
+struct PfRoute {
+    const int4 *tiles;                   // [cap] {expert, first position in perm, ntok (0 = unused entry), 0}; tiles never straddle experts
+    const int *perm;                     // [N * topk] the valid slots s = n * topk + j sorted by expert, ascending s inside an expert
+    const unsigned char *const *W;       // W[i * n_experts + e]: tensor i of expert e (the grouped pointer table)
+    void *const *C;                      // C[i * n_experts + e]: where tensor i stores slot s's row, at row s of [N * topk][Mout]
+    int n_experts;
+};
+template <bool INT_PATH, int QCH, int AGQ>
+__device__ __forceinline__ void lut_tile_rec(const int8_t *qlut, const float *ls, const float *lb, unsigned char *rec, int n, bool live,
+                                             int K, int step, int t) {
     using G = PfGroups<QCH, AGQ>;
-    constexpr int REC = pf_rec_bytes(INT_PATH, QCH, AGQ);
-    static_assert(INT_PATH || REC == kPfTab + 512 * (G::NLS + G::NLB), "record size");
-    const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * 128 + t;
-    const int nsteps = K / 64;
-    unsigned char *rec = out + ((size_t)tile * nsteps + step) * REC;
     const uint2 *src = reinterpret_cast<const uint2 *>(qlut) + ((size_t)n * (K / 4) + (size_t)step * 16) * 2;
 #pragma unroll
     for (int kc = 0; kc < 8; ++kc) {
         uint2 lo = make_uint2(0, 0), hi = make_uint2(0, 0);
-        if (n < N) { lo = __ldg(src + kc * 4); hi = __ldg(src + kc * 4 + 2); }
+        if (live) { lo = __ldg(src + kc * 4); hi = __ldg(src + kc * 4 + 2); }
         *reinterpret_cast<uint4 *>(rec + ((size_t)(kc * 16 + (t >> 3)) * 128 + (t & 7) * 16)) = make_uint4(lo.x, lo.y, hi.x, hi.y);
     }
     if constexpr (INT_PATH) return;
@@ -152,9 +159,30 @@ __global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const
     const int lb0 = (QCH == 8 ? step >> 1 : step * G::NCS) * G::APC;     // first activation group of the step's chunk set
     float *lsd = reinterpret_cast<float *>(rec + 16384) + t * G::NLS, *lbd = reinterpret_cast<float *>(rec + 16384 + 512 * G::NLS) + t * G::NLB;
 #pragma unroll
-    for (int i = 0; i < G::NLS; ++i) lsd[i] = n < N ? ls[(size_t)n * nag + ag0 + i] : 0.f;
+    for (int i = 0; i < G::NLS; ++i) lsd[i] = live ? ls[(size_t)n * nag + ag0 + i] : 0.f;
 #pragma unroll
-    for (int i = 0; i < G::NLB; ++i) lbd[i] = n < N ? lb[(size_t)n * nag + lb0 + i] : 0.f;
+    for (int i = 0; i < G::NLB; ++i) lbd[i] = live ? lb[(size_t)n * nag + lb0 + i] : 0.f;
+}
+template <bool INT_PATH, int QCH = 8, int AGQ = 4>
+__global__ void __launch_bounds__(128) lut_tile_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K) {
+    constexpr int REC = pf_rec_bytes(INT_PATH, QCH, AGQ);
+    static_assert(INT_PATH || REC == kPfTab + 512 * (PfGroups<QCH, AGQ>::NLS + PfGroups<QCH, AGQ>::NLB), "record size");
+    const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * 128 + t;
+    const int nsteps = K / 64;
+    lut_tile_rec<INT_PATH, QCH, AGQ>(qlut, ls, lb, out + ((size_t)tile * nsteps + step) * REC, n, n < N, K, step, t);
+}
+// grid = (steps, table entries): the records of the routed int8 tile, [entry][step]; an unused entry's records are not written
+// (its tile CTAs exit without reading them).  fp path only.
+template <int QCH, int AGQ>
+__global__ void __launch_bounds__(128) lut_tile_gather_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int K,
+                                                              const int4 *tiles, const int *perm, int div) {
+    constexpr int REC = pf_rec_bytes(false, QCH, AGQ);
+    const int step = blockIdx.x, k = blockIdx.y, t = threadIdx.x;
+    const int4 e = __ldg(tiles + k);
+    if (e.z == 0) return;
+    const bool live = t < e.z;
+    const int n = live ? __ldg(perm + e.y + t) / div : 0;
+    lut_tile_rec<false, QCH, AGQ>(qlut, ls, lb, out + ((size_t)k * (K / 64) + step) * REC, n, live, K, step, t);
 }
 
 // NV consecutive floats of shared memory (NV = 2, 4 or 8, aligned to their size) as vector loads
@@ -250,9 +278,13 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 // warpgroup; when nrsb is odd the last tile's second super-block does not exist and its A rows are zero.
 // fp path: a step is 64 K, two per 128-K window.  INT_PATH: the integer path (see the header); a step is 64 K, p.qch / 4 of them
 // per chunk, and the staging unit is one chunk.
-template <int PB, bool INT_PATH, int QCH = 8, int AGQ = 4>
-__global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
+// ROUTE (routed experts, fp path, prefill_experts_kernel): grid = (row tiles, table entries, count); the CTA of entry k = blockIdx.y
+// and tensor i = blockIdx.z exits at once when the entry is unused, else takes the weights W[i * n_experts + expert] of the pointer
+// table, the records of entry k (lut_tile_gather_kernel) and stores token t's row at row perm[start + t] of C[i * n_experts + expert].
+template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE>
+__device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    static_assert(!(ROUTE && INT_PATH), "routed experts: fp path only");
     using G = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
@@ -269,7 +301,12 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rt = blockIdx.x, tile = blockIdx.y, n0 = tile * kPfNT;
-    const int ntok = min(kPfNT, p.N - n0);
+    int4 ent = make_int4(0, 0, 0, 0);                                      // ROUTE: {expert, start, ntok, 0} of the CTA's entry
+    if constexpr (ROUTE) {
+        ent = __ldg(route.tiles + tile);
+        if (ent.z == 0) return;
+    }
+    const int ntok = ROUTE ? ent.z : min(kPfNT, p.N - n0);
     const int nag = p.K / 64;
 
     pf_build_xtab<PB>(xtab, p.bits, false, tid, kPfThreads2);
@@ -278,7 +315,8 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
         mbar_fence_init();
     }
     __syncthreads();
-    const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
+    // first super-block of the row tile
+    const unsigned char *rsb_base = (ROUTE ? route.W[blockIdx.z * route.n_experts + ent.x] : p.W) + (size_t)rt * NSB * p.rsb_stride;
     const int spc = INT_PATH ? p.qch >> 2 : 2;       // steps (64 K) per staging unit
     const int nunits = p.nchunk / WB;                // fp path: 128-K windows; integer path: chunks
     const int nsteps = spc * nunits;
@@ -444,6 +482,22 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
             if (lane == 0) mbar_arrive(empty + s);        // A tile and record of this step are dead: the stage may be refilled
             __syncwarp();
         }
+        if constexpr (ROUTE) {
+            void *const Cr = route.C[blockIdx.z * route.n_experts + ent.x];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = rt * 128 + r0 + 8 * h;
+                if (row >= p.Mout) continue;
+#pragma unroll
+                for (int c8 = 0; c8 < 16; ++c8)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int t = 8 * c8 + tc + e;
+                        if (t < ntok) store_out(Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row, accf[4 * c8 + 2 * h + e], p.out_f16);
+                    }
+            }
+            return;
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = rt * 128 + r0 + 8 * h;
@@ -461,6 +515,14 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
                 }
         }
     }
+}
+template <int PB, bool INT_PATH, int QCH = 8, int AGQ = 4>
+__global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
+    prefill_body<PB, INT_PATH, QCH, AGQ, false>(p, PfRoute{});
+}
+template <int PB, int QCH, int AGQ>
+__global__ void __launch_bounds__(kPfThreads2, 1) prefill_experts_kernel(const PrefillParams p, const PfRoute route) {
+    prefill_body<PB, false, QCH, AGQ, true>(p, route);
 }
 
 }  // namespace tmac_b200

@@ -69,23 +69,24 @@ __device__ __forceinline__ void wg_mma_f16_n256(float (&d)[128], uint64_t da, ui
 //                  ((g*32 + t/8)*128 + (t%8)*16), ag(g) = the activation group of K-group g
 //   bias steps   : column 4*wg + {0,1,2,3} = {LBhi, LBlo, LBhi, LBlo}, LB = the sum of lut_bias[n][ag] over the activation groups
 //                  ag of chunk wg in order (ck 128, ags 64: lut_bias[n][2wg] + lut_bias[n][2wg+1]); 8 columns per chunk
-template <int QCH = 8, int AGQ = 4>
-__global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K,
-                                                         int nmain, int nextra) {
+// Record `tile` of B tiles [tile][nmain + nextra]: token row n (live: the token exists, else zero) at position t, the body of both
+// B-tile kernels.
+template <int QCH, int AGQ>
+__device__ __forceinline__ void lut_tile16_rec(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int tile, int n, bool live,
+                                               int K, int nmain, int nextra, int step, int t) {
     using G = PfGroups<QCH, AGQ>;
-    const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * kP16NT + t;
     const int nag = K / (16 * AGQ), nwg = K / (16 * QCH);
     unsigned char *rec = out + ((size_t)tile * (nmain + nextra) + step) * kP16BBytes;
     if (step < nmain) {
         float ll[G::NLS];                            // the LUT scales of the step's activation groups
 #pragma unroll
-        for (int i = 0; i < G::NLS; ++i) ll[i] = (n < N) ? ls[(size_t)n * nag + step * 4 / AGQ + i] : 0.f;
+        for (int i = 0; i < G::NLS; ++i) ll[i] = live ? ls[(size_t)n * nag + step * 4 / AGQ + i] : 0.f;
         const uint2 *src = reinterpret_cast<const uint2 *>(qlut) + ((size_t)n * (K / 4) + (size_t)step * 16) * 2;
 #pragma unroll
         for (int g = 0; g < 16; ++g) {
             const float l = ll[g * G::NLS / 16];
             uint2 q = make_uint2(0, 0);
-            if (n < N) q = __ldg(src + g * 2);       // the 8 stored entries of the group
+            if (live) q = __ldg(src + g * 2);        // the 8 stored entries of the group
             uint32_t o[4];
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -106,7 +107,7 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
             for (int u = 0; u < 2; ++u) {
                 const int wg = e * 32 + kc * 2 + u;
                 float LB = 0.f;
-                if (n < N && wg < nwg) {
+                if (live && wg < nwg) {
                     LB = lb[(size_t)n * nag + G::APC * wg];
 #pragma unroll
                     for (int a = 1; a < G::APC; ++a) LB += lb[(size_t)n * nag + G::APC * wg + a];
@@ -119,6 +120,24 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
             *reinterpret_cast<uint4 *>(rec + ((size_t)(kc * 32 + (t >> 3)) * 128 + (t & 7) * 16)) = make_uint4(o[0], o[1], o[2], o[3]);
         }
     }
+}
+template <int QCH = 8, int AGQ = 4>
+__global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int N, int K,
+                                                         int nmain, int nextra) {
+    const int step = blockIdx.x, tile = blockIdx.y, t = threadIdx.x, n = tile * kP16NT + t;
+    lut_tile16_rec<QCH, AGQ>(qlut, ls, lb, out, tile, n, n < N, K, nmain, nextra, step, t);
+}
+// grid = (nmain + nextra, table entries): the B tiles of the routed fp16 tile, [entry][step], token position t = perm position
+// start + t of the entry (PfRoute, lut_tile_gather_kernel); an unused entry's tiles are not written.
+template <int QCH, int AGQ>
+__global__ void __launch_bounds__(256) lut_tile16_gather_kernel(const int8_t *qlut, const float *ls, const float *lb, unsigned char *out, int K,
+                                                                int nmain, int nextra, const int4 *tiles, const int *perm, int div) {
+    const int step = blockIdx.x, k = blockIdx.y, t = threadIdx.x;
+    const int4 e = __ldg(tiles + k);
+    if (e.z == 0) return;
+    const bool live = t < e.z;
+    const int n = live ? __ldg(perm + e.y + t) / div : 0;
+    lut_tile16_rec<QCH, AGQ>(qlut, ls, lb, out, k, n, live, K, nmain, nextra, step, t);
 }
 
 // One CTA walks a contiguous run [L0, L1) of the linear (tile, step) sequence -- tile = (row super-block, token tile), nsteps
@@ -135,8 +154,13 @@ __global__ void __launch_bounds__(256) lut_tile16_kernel(const int8_t *qlut, con
 // Row tile = 128 rows.  PB 2 (W2): one super-block.  PB 4 (W3/W4): super-blocks 2*rt and 2*rt + 1 (64 rows each), producer
 // threads 0..63 / 64..127 and consumer warpgroups 0 / 1; when nrsb is odd the last tile's second super-block does not exist and
 // its A rows are zero.
-template <int PB, int QCH = 8, int AGQ = 4>
-__global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill16Params p) {
+//
+// ROUTE (routed experts, prefill16_experts_kernel): grid = (row tiles, table entries, count), no stream-K.  As in the int8 tile
+// (prefill_body): the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the entry is unused, else runs tile
+// k * nrt + blockIdx.x on the weights W[i * n_experts + expert], the B tiles of entry k, and stores token t's row at row
+// perm[start + t] of C[i * n_experts + expert].
+template <int PB, int QCH, int AGQ, bool ROUTE>
+__device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
     using PG = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
@@ -152,7 +176,13 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nsteps = p.nmain + p.nextra;
-    const int G = gridDim.x, cta = blockIdx.x;
+    int4 ent = make_int4(0, 0, 0, 0);                                      // ROUTE: {expert, start, ntok, 0} of the CTA's entry
+    if constexpr (ROUTE) {
+        ent = __ldg(route.tiles + blockIdx.y);
+        if (ent.z == 0) return;
+    }
+    const int G = gridDim.x, cta = ROUTE ? blockIdx.y * p.nrt + blockIdx.x : blockIdx.x;
+    const unsigned char *W = ROUTE ? route.W[blockIdx.z * route.n_experts + ent.x] : p.W;
     const long long Stot = (long long)p.ntiles * nsteps;
     const int L0 = p.streamk ? (int)(Stot * cta / G) : cta * nsteps, L1 = p.streamk ? (int)(Stot * (cta + 1) / G) : (cta + 1) * nsteps;
     // fragments: f = 0 -> [L0, min(L1, end of L0's tile)), f = 1 -> the rest (head of the next tile)
@@ -200,7 +230,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
         for (int f = 0; f < 2; ++f) {
             if (f == nfrag) break;
             const int rt = ft[f] % p.nrt;
-            const unsigned char *rsb_base = p.W + (size_t)rt * NSB * p.rsb_stride;   // first super-block of the row tile
+            const unsigned char *rsb_base = W + (size_t)rt * NSB * p.rsb_stride;     // first super-block of the row tile
             const bool live = PB == 2 || rt * NSB + sb < p.nrsb;
             const unsigned char *sb_base = rsb_base + (size_t)sb * p.rsb_stride;
             const int s0 = fs0[f], s1m = min(fs1[f], p.nmain);
@@ -315,6 +345,23 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
                 if (lane == 0) mbar_arrive(empty + s);              // both tiles of the stage are free
                 __syncwarp();
             }
+            if constexpr (ROUTE) {                   // one whole tile per CTA
+                void *const Cr = route.C[blockIdx.z * route.n_experts + ent.x];
+                const int row0 = (int)blockIdx.x * 128 + r0;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = row0 + 8 * h;
+#pragma unroll
+                    for (int c8 = 0; c8 < 32; ++c8)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int t = 8 * c8 + tc + e;
+                            if (t < ent.z && row < p.Mout)
+                                store_out(Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row, acc[4 * c8 + 2 * h + e], p.out_f16);
+                        }
+                }
+                continue;
+            }
             const bool whole = fs0[f] == 0 && fs1[f] == nsteps, last = fs1[f] == nsteps;
             const int rt = ft[f] % p.nrt, tile = ft[f] / p.nrt, n0 = tile * kP16NT, ntok = min(kP16NT, p.N - n0);
             if (whole) {
@@ -369,5 +416,29 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill
         }
     }
 }
+template <int PB, int QCH = 8, int AGQ = 4>
+__global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill16Params p) {
+    prefill16_body<PB, QCH, AGQ, false>(p, PfRoute{});
+}
+template <int PB, int QCH, int AGQ>
+__global__ void __launch_bounds__(kP16Threads, 1) prefill16_experts_kernel(const Prefill16Params p, const PfRoute route) {
+    prefill16_body<PB, QCH, AGQ, true>(p, route);
+}
+
+// The routed-expert launches (tmac_b200_prefill_experts / _glu): the kernels of one tensor kind (PB) and fp grouping, instantiated
+// in tmac_prefill_experts.cu.  route sorts the slots by expert and writes the tile table; swiglu materialises the GLU form's
+// inputs; combine adds the GLU form's slot rows.
+struct PfExpertKernels {
+    void (*tile)(const PrefillParams, const PfRoute);
+    void (*lut)(const int8_t *, const float *, const float *, unsigned char *, int, const int4 *, const int *, int);
+    void (*tile16)(const Prefill16Params, const PfRoute);
+    void (*lut16)(const int8_t *, const float *, const float *, unsigned char *, int, int, int, const int4 *, const int *, int);
+};
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq);
+void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
+                     int out_f16, cudaStream_t st);
+void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st);
+void pf_combine_launch(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R, void *C, int N, int Mout,
+                       int out_f16, cudaStream_t st);
 
 }  // namespace tmac_b200

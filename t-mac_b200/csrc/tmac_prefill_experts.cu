@@ -1,0 +1,127 @@
+// tmac_prefill_experts.cu -- the routed-expert launches at prefill sizes (tmac_b200_prefill_experts / _glu): the routing kernel
+// that groups the slots by expert, the routed instantiations of both wgmma tiles and their gathered LUT records (3 bit widths x 6 fp
+// groupings; tmac_prefill.cuh, tmac_prefill16.cuh), the GLU form's input and its combine.  In their own translation unit so that
+// they compile in parallel with tmac_b200.cu.
+#include "tmac_prefill16.cuh"
+
+namespace tmac_b200 {
+
+namespace {
+
+constexpr int kRouteThreads = 1024, kRouteWarps = kRouteThreads / 32, kRouteMaxE = 256;
+
+// One CTA.  Slot s = n * topk + j of expert e = ids[s] (valid: 0 <= e < E).  A counting sort that depends only on ids: the counts of
+// each expert, their exclusive prefix off[e], then rounds of 1024 slots in which a slot's position is off[e] + (the slots of e in
+// earlier rounds) + (those in earlier warps of the round) + (those in earlier lanes of its warp) -- ascending s inside an expert.
+// Tile table: expert e's rows in runs of T from off[e], entries in expert order, the rest of the cap entries unused (ntok 0).
+// Cnan != null (the plain form): the Mout-wide rows of every invalid slot in C_i = Cnan[i * E] are quiet NaN.
+__global__ void __launch_bounds__(kRouteThreads) pf_route_kernel(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm,
+                                                                 void *const *Cnan, int count, int ldc, int out_f16) {
+    __shared__ int cnt[kRouteMaxE], off[kRouteMaxE], tb[kRouteMaxE], run[kRouteMaxE], wc[kRouteWarps][kRouteMaxE];
+    __shared__ int used;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    for (int e = tid; e < E; e += kRouteThreads) { cnt[e] = 0; run[e] = 0; }
+    __syncthreads();
+    for (int s = tid; s < S; s += kRouteThreads) {
+        const int e = ids[s];
+        if ((unsigned)e < (unsigned)E) atomicAdd(&cnt[e], 1);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int o = 0, k = 0;
+        for (int e = 0; e < E; ++e) { off[e] = o; tb[e] = k; o += cnt[e]; k += (cnt[e] + T - 1) / T; }
+        used = k;
+    }
+    __syncthreads();
+    for (int e = tid; e < E; e += kRouteThreads)
+        for (int q = 0; q * T < cnt[e]; ++q) tiles[tb[e] + q] = make_int4(e, off[e] + q * T, min(T, cnt[e] - q * T), 0);
+    for (int k = used + tid; k < cap; k += kRouteThreads) tiles[k] = make_int4(0, 0, 0, 0);
+    for (int base = 0; base < S; base += kRouteThreads) {
+        const int s = base + tid;
+        int e = s < S ? ids[s] : -1;
+        if ((unsigned)e >= (unsigned)E) e = -1;
+        for (int i = tid; i < kRouteWarps * E; i += kRouteThreads) wc[i / E][i % E] = 0;
+        __syncthreads();
+        const unsigned same = __match_any_sync(0xffffffffu, e);
+        const int rank = __popc(same & ((1u << lane) - 1u));
+        if (e >= 0 && rank == 0) wc[warp][e] = __popc(same);
+        __syncthreads();
+        for (int x = tid; x < E; x += kRouteThreads) {   // per expert: the warps' exclusive prefix, on top of the earlier rounds
+            int acc = run[x];
+            for (int w = 0; w < kRouteWarps; ++w) { const int c = wc[w][x]; wc[w][x] = acc; acc += c; }
+            run[x] = acc;
+        }
+        __syncthreads();
+        if (e >= 0) perm[off[e] + wc[warp][e] + rank] = s;
+        __syncthreads();
+    }
+    if (!Cnan) return;
+    for (int s = warp; s < S; s += kRouteWarps) {
+        if ((unsigned)ids[s] < (unsigned)E) continue;
+        for (int i = 0; i < count; ++i) {
+            void *const Ci = Cnan[(size_t)i * E];
+            for (int r = lane; r < ldc; r += 32) store_out(Ci, (size_t)s * ldc + r, __int_as_float(0x7fffffff), out_f16);
+        }
+    }
+}
+
+// a[i] = swiglu(g[i], u[i]) in fp32, fp16 inputs widened first: the input the GEMV's GLU kinds build their LUT from
+template <typename T>
+__global__ void __launch_bounds__(256) pf_swiglu_kernel(const T *g, const T *u, size_t n, float *a) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        a[i] = swiglu(ld_act(g, i), ld_act(u, i));
+}
+
+// C[n][row] = fadd_rn(...fadd_rn(fmul_rn(w_0, y_0), fmul_rn(w_1, y_1))..., fmul_rn(w_{topk-1}, y_{topk-1})) (+ R[n][row]), y_j =
+// ys[n * topk + j][row]; quiet NaN for a token with an id outside [0, E) (its slots' rows were never computed)
+__global__ void __launch_bounds__(256) pf_combine_kernel(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R,
+                                                         void *C, int N, int Mout, int out_f16) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)N * Mout) return;
+    const int n = (int)(i / Mout), row = (int)(i % Mout);
+    bool bad = false;
+    for (int j = 0; j < topk; ++j) bad |= (unsigned)ids[n * topk + j] >= (unsigned)E;
+    float acc = __int_as_float(0x7fffffff);
+    if (!bad) {
+        const float *y = ys + (size_t)n * topk * Mout + row, *wn = w + (size_t)n * topk;
+        acc = __fmul_rn(wn[0], y[0]);
+        for (int j = 1; j < topk; ++j) acc = __fadd_rn(acc, __fmul_rn(wn[j], y[(size_t)j * Mout]));
+        if (R)                                   // read, then written by this thread: the residual may be C itself
+            acc = __fadd_rn(acc, out_f16 ? __half2float(reinterpret_cast<const __half *>(R)[i]) : reinterpret_cast<const float *>(R)[i]);
+    }
+    store_out(C, i, acc, out_f16);
+}
+
+template <int PB> PfExpertKernels pick_pf_experts_pb(int qch, int agq) {
+    return FpGroupings::find<PfExpertKernels>(qch, agq, [](auto QCH, auto AGQ) -> PfExpertKernels {
+        return {prefill_experts_kernel<PB, QCH, AGQ>, lut_tile_gather_kernel<QCH, AGQ>, prefill16_experts_kernel<PB, QCH, AGQ>,
+                lut_tile16_gather_kernel<QCH, AGQ>};
+    });
+}
+
+}  // namespace
+
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq) {
+    if (pb == 4) return pick_pf_experts_pb<4>(qch, agq);
+    if (pb == 2) return pick_pf_experts_pb<2>(qch, agq);
+    return PfExpertKernels{};
+}
+
+void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
+                     int out_f16, cudaStream_t st) {
+    pf_route_kernel<<<1, kRouteThreads, 0, st>>>(ids, S, E, T, cap, tiles, perm, Cnan, count, ldc, out_f16);
+}
+
+void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st) {
+    const int grid = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
+    if (f16) pf_swiglu_kernel<__half><<<grid, 256, 0, st>>>((const __half *)G, (const __half *)U, n, a);
+    else pf_swiglu_kernel<float><<<grid, 256, 0, st>>>((const float *)G, (const float *)U, n, a);
+}
+
+void pf_combine_launch(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R, void *C, int N, int Mout,
+                       int out_f16, cudaStream_t st) {
+    const size_t n = (size_t)N * Mout;
+    pf_combine_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ys, ids, w, topk, E, R, C, N, Mout, out_f16);
+}
+
+}  // namespace tmac_b200

@@ -44,7 +44,7 @@ EXPORTS = [
     "tmac_b200_find_kcfg", "tmac_b200_clear_kcfg", "tmac_b200_upload_weights", "tmac_b200_upload_plain",
     "tmac_b200_upload_plain_rows", "tmac_b200_debug_encode", "tmac_b200_free_weights", "tmac_b200_clone_weights", "tmac_b200_hint_next_weights",
     "tmac_b200_graph_begin", "tmac_b200_graph_end", "tmac_b200_graph_launch", "tmac_b200_graph_free", "tmac_b200_sync", "tmac_b200_debug_trace", "tmac_b200_debug_last_launch", "tmac_b200_debug_set", "tmac_b200_weights_nbytes", "tmac_b200_preprocessor",
-    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
+    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
     "ggml_tmac_init", "ggml_tmac_free", "ggml_tmac_mul_mat_task_init", "ggml_tmac_mul_mat_task_compute",
     "ggml_tmac_set_n_threads", "ggml_tmac_get_type_bits", "ggml_tmac_b200_can_mul_mat",
     "ggml_tmac_b200_mul_mat_get_wsize", "ggml_tmac_b200_get_nbytes", "ggml_tmac_b200_transform_tensor",
@@ -91,6 +91,8 @@ def load() -> C.CDLL:
         "tmac_b200_gemv_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_gemv_residual": (i, [i64, i, i, vp, vp, vp]),
         "tmac_b200_gemv_experts": (i, [vp, i, i, i, i, vp, vp, i, vp]),
         "tmac_b200_gemv_experts_glu": (i, [vp, i, i, i, vp, vp, vp, vp, i, vp, vp]),
+        "tmac_b200_prefill_experts": (i, [vp, i, i, i, i, vp, vp, i, vp]),
+        "tmac_b200_prefill_experts_glu": (i, [vp, i, i, i, vp, vp, vp, vp, i, vp, vp]),
         "tmac_b200_gemv": (i, [i64, i, i, vp, vp]), "tmac_b200_cbits": (i, [i64, i, vp, vp]),
         "qgemm_lut_int8": (i, [i, i, i, i, vp, vp, vp, vp, vp, vp]),
         "preprocessor_int8": (i, [i, i, i, i, vp, vp, vp, vp]),
@@ -270,6 +272,26 @@ def gemv_experts_glu(wts, N, G, U, ids, weights, Cout, R=None, dtype=F32):
     topk = ids.shape[-1] if hasattr(ids, "shape") else 0
     check(load().tmac_b200_gemv_experts_glu(H, len(wts), N, dtype, ptr(G), ptr(U), ptr(ids), ptr(weights), topk, ptr(R), ptr(Cout)),
           "tmac_b200_gemv_experts_glu")
+
+
+def prefill_experts(tables, N, B, ids, outs, dtype=F32):
+    """gemv_experts' arguments and output, run on the prefill tiles with each expert's tokens grouped on the device (the form for
+    large N * topk, tmac_b200_prefill_experts)."""
+    count, n_experts = len(tables), len(tables[0]) if tables else 0
+    if any(len(t) != n_experts for t in tables):
+        raise ValueError("prefill_experts: every tensor needs one entry per expert")
+    H = (C.c_int64 * (count * n_experts))(*[w.handle for t in tables for w in t])
+    O = (C.c_void_p * count)(*[ptr(x) for x in outs])
+    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
+    check(load().tmac_b200_prefill_experts(H, count, n_experts, N, dtype, ptr(B), ptr(ids), topk, O), "tmac_b200_prefill_experts")
+
+
+def prefill_experts_glu(wts, N, G, U, ids, weights, Cout, R=None, dtype=F32):
+    """gemv_experts_glu's arguments and output, run on the prefill tiles (tmac_b200_prefill_experts_glu)."""
+    H = (C.c_int64 * len(wts))(*[w.handle for w in wts])
+    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
+    check(load().tmac_b200_prefill_experts_glu(H, len(wts), N, dtype, ptr(G), ptr(U), ptr(ids), ptr(weights), topk, ptr(R), ptr(Cout)),
+          "tmac_b200_prefill_experts_glu")
 
 
 def gemv(wt: Weights, N, B, Cout, dtype=F32):
