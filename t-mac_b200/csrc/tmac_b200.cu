@@ -449,12 +449,61 @@ int tile_min_n(const StreamLayout &L) {
     return 32;
 }
 
-// Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): W2 or W3/W4 streams, N >= tile_min_n,
-// and either the fp path (per-row scales, K % 128 == 0, chunk 128, 64 or 32 K; the layout keeps the act group, 128, 64 or 32 K,
-// inside the chunk) or the integer path (one scale, act group K, chunk 128 or 64).
+// The fp-path tensors both tiles take, dense and routed: W2 or W3/W4 streams with per-row scales, K % 128 == 0, chunk 128, 64 or
+// 32 K, and the act group (128, 64 or 32 K) inside the chunk.
+static bool tiles_take_fp(const StreamLayout &L) {
+    return !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0 && (L.pb == 2 || L.pb == 4);
+}
+
+// Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): N >= tile_min_n, and either an fp-path
+// tensor the tiles take or the integer path (W2 or W3/W4 streams, one scale, act group K, chunk 128 or 64).
 bool takes_prefill_tile(const StreamLayout &L, int N) {
-    const bool fp_path = !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0;
-    return g.use_prefill && N >= tile_min_n(L) && (L.pb == 2 || L.pb == 4) && (fp_path || (L.int_path() && (L.qch == 8 || L.qch == 4)));
+    return g.use_prefill && N >= tile_min_n(L) && (tiles_take_fp(L) || (L.int_path() && (L.pb == 2 || L.pb == 4) && (L.qch == 8 || L.qch == 4)));
+}
+
+// Both tiles' geometry and shared memory for a tensor (int_path: the int8 tile's integer-path form), dense and routed alike.
+constexpr size_t kP16MaxSmem = 227 * 1024, kPfMaxSmem = 225 * 1024;   // the largest carve-up each tile is launched with
+struct TilePlan {
+    int nrt, nmain, nextra;        // row tiles of 128 rows; the 64-K steps, and the fp16 tile's bias steps
+    size_t rec, smem16, smem8;     // the int8 tile's LUT record bytes; both tiles' dynamic shared memory
+    bool fits16, fits8;
+    TilePlan(const StreamLayout &L, bool int_path) {
+        // the producers stage a 128-K window of 128 / ck chunk blocks (integer path: one chunk)
+        const size_t rawsz = ((int_path ? 1 : 8 / L.qch) * L.blk + 127) & ~(size_t)127;
+        // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
+        const int nsb = 128 / L.rsb;
+        const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
+        nrt = (L.nrsb + nsb - 1) / nsb; nmain = L.K / 64; nextra = (L.nchunk + 31) / 32;
+        rec = pf_rec_bytes(int_path, L.qch, L.agq());
+        smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
+        smem8 = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
+        fits16 = smem16 <= kP16MaxSmem; fits8 = smem8 <= kPfMaxSmem;
+    }
+};
+
+// The fields of a tile's parameters (Prefill16Params or PrefillParams) that come from the tensor and the call; the callers set the
+// pointers, the tile count and (dense fp16 tile) the stream-K split.
+template <class P> static P tile_params(const StreamLayout &L, const TilePlan &t, int N, int ldc, int out_f16) {
+    P p{};
+    p.N = N; p.K = L.K; p.Mout = L.Mout; p.ldc = ldc; p.out_f16 = out_f16;
+    p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride; p.nrsb = L.nrsb; p.bits = L.bits;
+    if constexpr (std::is_same_v<P, PrefillParams>) p.qch = L.qch;
+    else { p.nrt = t.nrt; p.nmain = t.nmain; p.nextra = t.nextra; }
+    return p;
+}
+
+// Launch the fp16 tile (fp16) or the int8 tile with its shared memory from the plan, and report it in last_launch: {16 or 1, warps, chunks,
+// split, grid.x, PB, 1, -rows} (a batch < 0 marks the tensor-core prefill tile).
+template <class F, class... P>
+static int launch_tile(bool fp16, F fn, dim3 grid, const TilePlan &t, int split, const StreamLayout &L, int rows, const P &...args) {
+    const int threads = fp16 ? kP16Threads : kPfThreads2;
+    const size_t smem = fp16 ? t.smem16 : t.smem8;
+    CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    fn<<<grid, threads, smem, g.stream()>>>(args...);
+    CUDA_OK(cudaGetLastError());
+    const int rep[8] = {fp16 ? 16 : 1, threads / 32, L.nchunk, split, (int)grid.x, L.pb, 1, -rows};
+    std::memcpy(g.last_launch, rep, sizeof rep);
+    return 0;
 }
 
 // The fp path's kernels of one grouping (QCH quads per chunk, AGQ quads per activation group): int8 tile, its LUT records,
@@ -477,78 +526,51 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
     const StreamLayout &L = R.L;
     if (!sym || !takes_prefill_tile(L, N)) return 1;
     const bool int_path = L.int_path();
-    const int agq = L.agq();
     PfKernels fk{};
     if (!int_path) {
-        fk = L.pb == 4 ? pick_pf<4>(L.qch, agq) : pick_pf<2>(L.qch, agq);
+        fk = L.pb == 4 ? pick_pf<4>(L.qch, L.agq()) : pick_pf<2>(L.qch, L.agq());
         if (!fk.tile) return fail("prefill: no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
     }
-    // the producers stage a 128-K window of 128 / ck chunk blocks (integer path: one chunk)
-    const size_t rawsz = ((int_path ? 1 : 8 / L.qch) * L.blk + 127) & ~(size_t)127;
-    // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
-    const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
-    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
+    const TilePlan t(L, int_path);
     // fp path: scales folded into fp16 operands, fp32 accumulation over K in registers (tmac_prefill16.cuh).  Not exact, so the
     // integer path never takes it.
-    if (g.use_prefill16 && N >= 64 && !int_path) {
-        const int nmain = L.K / 64, nextra = (L.nchunk + 31) / 32, ntile16 = (N + kP16NT - 1) / kP16NT;
-        const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
-        if (smem16 <= 227 * 1024) {
-            if (g.d_tiles.ensure((size_t)ntile16 * (nmain + nextra) * kP16BBytes)) return fail("out of device memory (LUT tiles)");
-            fk.lut16<<<dim3(nmain + nextra, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, nmain, nextra);
-            CUDA_OK(cudaGetLastError());
-            Prefill16Params q{};
-            q.W = R.d; q.C = C; q.N = N; q.K = L.K; q.Mout = L.Mout; q.ldc = ldc; q.out_f16 = out_f16;
-            q.nchunk = L.nchunk; q.zp = L.zp; q.sd = L.sd; q.blk_bytes = (int)L.blk; q.nmain = nmain; q.nextra = nextra;
-            q.rsb_stride = L.rsb_stride; q.tiles = (const unsigned char *)g.d_tiles.p;
-            q.nrsb = L.nrsb; q.nrt = nrt; q.bits = L.bits; q.ntiles = nrt * ntile16;
-            // fewer tiles than SMs (e.g. 86 at N = 256): stream-K over all SMs, partial tiles through `scratch`
-            q.streamk = (g.pf_streamk && q.ntiles < g.sms && (long)q.ntiles * (nmain + nextra) >= 2L * g.sms) ? 1 : 0;
-            const int grid = q.streamk ? g.sms : q.ntiles;
-            if (q.streamk) {
-                const size_t sb = (size_t)2 * grid * kP16NT * 128 * sizeof(float);
-                if (g.d_pf_scratch.ensure(sb)) return fail("out of device memory (stream-K scratch)");
-                if (g.d_pf_flags.cap < (size_t)grid * sizeof(int)) {
-                    if (g.d_pf_flags.ensure((size_t)grid * sizeof(int))) return fail("out of device memory (stream-K flags)");
-                    CUDA_OK(cudaMemsetAsync(g.d_pf_flags.p, 0, g.d_pf_flags.cap, g.stream()));
-                }
-                q.scratch = (float *)g.d_pf_scratch.p; q.flags = (int *)g.d_pf_flags.p;
+    if (g.use_prefill16 && N >= 64 && !int_path && t.fits16) {
+        const int nsteps = t.nmain + t.nextra, ntile16 = (N + kP16NT - 1) / kP16NT;
+        if (g.d_tiles.ensure((size_t)ntile16 * nsteps * kP16BBytes)) return fail("out of device memory (LUT tiles)");
+        fk.lut16<<<dim3(nsteps, ntile16), 256, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K, t.nmain, t.nextra);
+        CUDA_OK(cudaGetLastError());
+        auto q = tile_params<Prefill16Params>(L, t, N, ldc, out_f16);
+        q.W = R.d; q.C = C; q.tiles = (const unsigned char *)g.d_tiles.p; q.ntiles = t.nrt * ntile16;
+        // fewer tiles than SMs (e.g. 86 at N = 256): stream-K over all SMs, partial tiles through `scratch`
+        q.streamk = (g.pf_streamk && q.ntiles < g.sms && (long)q.ntiles * nsteps >= 2L * g.sms) ? 1 : 0;
+        const int grid = q.streamk ? g.sms : q.ntiles;
+        if (q.streamk) {
+            const size_t sb = (size_t)2 * grid * kP16NT * 128 * sizeof(float);
+            if (g.d_pf_scratch.ensure(sb)) return fail("out of device memory (stream-K scratch)");
+            if (g.d_pf_flags.cap < (size_t)grid * sizeof(int)) {
+                if (g.d_pf_flags.ensure((size_t)grid * sizeof(int))) return fail("out of device memory (stream-K flags)");
+                CUDA_OK(cudaMemsetAsync(g.d_pf_flags.p, 0, g.d_pf_flags.cap, g.stream()));
             }
-            const auto fn16 = fk.tile16;
-            CUDA_OK(cudaFuncSetAttribute((const void *)fn16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
-            fn16<<<dim3(grid), kP16Threads, smem16, g.stream()>>>(q);
-            CUDA_OK(cudaGetLastError());
-            g.last_launch[0] = 16; g.last_launch[1] = kP16Threads / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = q.streamk; g.last_launch[4] = grid;
-            g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;
-            return 0;
+            q.scratch = (float *)g.d_pf_scratch.p; q.flags = (int *)g.d_pf_flags.p;
         }
+        return launch_tile(true, fk.tile16, dim3(grid), t, q.streamk, L, N, q);
     }
-    const size_t rec = pf_rec_bytes(int_path, L.qch, agq);
-    const size_t smem = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
-    if (smem > 225 * 1024) return 1;
-    const int nag = L.K / 64, ntile = (N + kPfNT - 1) / kPfNT;   // records: one per 64-K step
-    if (g.d_tiles.ensure((size_t)ntile * nag * rec)) return fail("out of device memory (LUT tiles)");
-    if (int_path) lut_tile_kernel<true><<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, nullptr, nullptr, (unsigned char *)g.d_tiles.p, N, L.K);
-    else fk.lut<<<dim3(nag, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
+    if (!t.fits8) return 1;
+    const int ntile = (N + kPfNT - 1) / kPfNT;   // records: one per 64-K step
+    if (g.d_tiles.ensure((size_t)ntile * t.nmain * t.rec)) return fail("out of device memory (LUT tiles)");
+    if (int_path) lut_tile_kernel<true><<<dim3(t.nmain, ntile), 128, 0, g.stream()>>>(qlut, nullptr, nullptr, (unsigned char *)g.d_tiles.p, N, L.K);
+    else fk.lut<<<dim3(t.nmain, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
     CUDA_OK(cudaGetLastError());
-    PrefillParams p{};
-    p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C;
+    auto p = tile_params<PrefillParams>(L, t, N, ldc, out_f16);
+    p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C; p.scale0 = L.scale0;
     p.lut_tiles = (const unsigned char *)g.d_tiles.p;
-    p.N = N; p.K = L.K; p.Mout = L.Mout; p.ldc = ldc; p.out_f16 = out_f16;
-    p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride;
-    p.nrsb = L.nrsb; p.bits = L.bits; p.qch = L.qch; p.scale0 = L.scale0;
     if (g.trace) {
         if (g.d_trace.ensure(8192)) return fail("out of device memory (trace)");
         CUDA_OK(cudaMemsetAsync(g.d_trace.p, 0, 3 * 32 * 4 * sizeof(long long), g.stream()));
         p.dbg = (long long *)g.d_trace.p; g.trace_ctas = 12;   // 96 rows of 4 = 48 rows of 8
     }
     const auto fn = int_path ? (L.pb == 4 ? prefill_kernel<4, true> : prefill_kernel<2, true>) : fk.tile;
-    CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fn<<<dim3(nrt, ntile), kPfThreads2, smem, g.stream()>>>(p);
-    CUDA_OK(cudaGetLastError());
-    g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[2] = L.nchunk; g.last_launch[3] = 1; g.last_launch[4] = nrt;
-    g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -N;   // batch < 0 marks the tensor-core prefill tile
-    return 0;
+    return launch_tile(false, fn, dim3(t.nrt, ntile), t, 1, L, N, p);
 }
 
 // Launch qgemm_lut over rows [row_begin,row_end) (relative to the resident tensor): the tensor-core tile for whole-tensor batches,
@@ -1174,10 +1196,10 @@ int tmac_b200_qgemm_lut(int64_t handle, int row0, int rows, int N, int dtype, co
 }
 
 // The setup both grouped launches share: the tensors of `handles`, which must share one geometry (*first: the first of them), and the
-// device pointer table {W, QLUT, LUT_Scales, LUT_Biases, C}[count] of the call (null q / ls / lb: null entries).  Pointer tables: one
-// device allocation per distinct call signature (stable under graph capture), at most 256.
+// device pointer table {W, QLUT, LUT_Scales, LUT_Biases, C[i / per_c]}[count] of the call (null q / ls / lb: null entries).  Pointer
+// tables: one device allocation per distinct call signature (stable under graph capture), at most 256.
 static int grouped_setup(const char *what, const int64_t *handles, int count, const void *const *q, const void *const *ls,
-                         const void *const *lb, void *const *C, const Resident **first, BatchPtrs *bp) {
+                         const void *const *lb, void *const *C, const Resident **first, BatchPtrs *bp, int per_c = 1) {
     std::vector<const void *> tab(5 * (size_t)count, nullptr);
     for (int i = 0; i < count; ++i) {
         auto it = g.res.find(handles[i]);
@@ -1187,7 +1209,7 @@ static int grouped_setup(const char *what, const int64_t *handles, int count, co
         if (a.Mout != b.Mout || a.K != b.K || a.bits != b.bits || a.blk != b.blk || a.nchunk != b.nchunk || a.zp != b.zp ||
             a.one_scale != b.one_scale || a.sd != b.sd || a.act_group_size != b.act_group_size || a.scale0 != b.scale0)
             return fail(std::string(what) + ": all tensors must share one geometry");
-        tab[i] = it->second.d; tab[4 * count + i] = C[i];
+        tab[i] = it->second.d; tab[4 * count + i] = C[i / per_c];
         if (q) { tab[count + i] = q[i]; tab[2 * count + i] = ls[i]; tab[3 * count + i] = lb[i]; }
     }
     void *dtab = nullptr;
@@ -1296,25 +1318,31 @@ int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, con
     return gemv_io("gemv_residual", &handle, 1, N, dtype, kInRow, B, io, &C);
 }
 
+// The checks both routed-expert call forms share (tmac_b200_gemv_experts / _glu and tmac_b200_prefill_experts / _glu): the
+// arguments, then that A, ids, C[count] and every U, weights and R given are device pointers.
+static int experts_check(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
+                         const void *A, const void *U, const int32_t *ids, const float *wts, const void *R, void *const *C) {
+    if (!handles || count <= 0 || n_experts <= 0 || N <= 0 || !A || !ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
+        return fail(what + ": bad arguments");
+    if (topk < 1 || topk > 8) return fail(what + ": topk must be 1..8");
+    if ((long long)count * n_experts > 65535) return fail(what + ": count * n_experts must be <= 65535");
+    if (!is_device_ptr(A) || !is_device_ptr(ids) || (U && !is_device_ptr(U)) || (wts && !is_device_ptr(wts)) || (R && !is_device_ptr(R)))
+        return fail(what + ": device pointers only");
+    for (int i = 0; i < count; ++i)
+        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
+    return 0;
+}
+
 // tmac_b200_gemv_experts / _glu: the launch of tmac_b200_gemv_grouped over count * topk slots (so each slot's sums are those of
 // gemv_grouped at N * count * topk), with a pointer table of every tensor, count * n_experts entries, from which each slot picks its
 // tensor by the id it reads on the device.  Everything is checked before anything is launched.
 static int gemv_experts(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
-                        int kind, const void *A, Gemv3Io io, void *const *C, int nC) {
-    if (!handles || count <= 0 || n_experts <= 0 || (long long)count * n_experts > 65535 || N <= 0 || topk < 1 || topk > 8 || !A ||
-        !io.ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
-        return fail(what + ": bad arguments");
-    if (!is_device_ptr(A) || !is_device_ptr(io.ids) || (io.act2 && !is_device_ptr(io.act2)) || (io.wts && !is_device_ptr(io.wts)) ||
-        (io.res && !is_device_ptr(io.res)))
-        return fail(what + ": device pointers only");
-    for (int i = 0; i < nC; ++i)
-        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
-    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts is C[i] (kInExpertsGlu: C[0] = C)
-    for (int i = 0; i < count; ++i)
-        for (int e = 0; e < n_experts; ++e) Cx[(size_t)i * n_experts + e] = C[nC > 1 ? i : 0];
+                        int kind, const void *A, Gemv3Io io, void *const *C) {
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, Cx.data(), &R, &bp)) return -1;
+    if (experts_check(what, handles, count, n_experts, N, dtype, topk, A, io.act2, io.ids, io.wts, io.res, C) ||
+        grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, C, &R, &bp, n_experts))
+        return -1;
     const StreamLayout &L = R->L;
     if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
     bp.n = count * topk;                           // grid.z: the slots
@@ -1337,7 +1365,7 @@ int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int
     if (ensure_init()) return -1;
     Gemv3Io io{};
     io.ids = ids;
-    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kInExperts, B, io, C, count > 0 ? count : 0);
+    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kInExperts, B, io, C);
 }
 
 int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
@@ -1347,7 +1375,7 @@ int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int
     if (!U || !weights || !C) return fail("gemv_experts_glu: bad arguments");
     Gemv3Io io{};
     io.act2 = U; io.ids = ids; io.wts = weights; io.res = R;
-    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kInExpertsGlu, G, io, &C, 1);
+    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kInExpertsGlu, G, io, &C);
 }
 
 // The tile of a routed launch: the fp16 tile when it is on and the average expert fills one of its 256-token tiles,
@@ -1364,50 +1392,30 @@ static int prefill_experts(const std::string &what, const std::string &gemv_name
                            void *const *C) {
     const bool glu = U != nullptr;
     if (g.npeer) { g.npeer = 0; return fail(what + ": peer outputs are for N = 1 single-tensor launches"); }
-    if (!handles || count <= 0 || N <= 0 || !A || !ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
-        return fail(what + ": bad arguments");
-    if (topk < 1 || topk > 8) return fail(what + ": topk must be 1..8");
-    if (n_experts < 1 || n_experts > 256) return fail(what + ": n_experts must be 1..256");
-    if ((long long)count * n_experts > 65535) return fail(what + ": count * n_experts must be <= 65535");
-    if (!is_device_ptr(A) || !is_device_ptr(ids) || (glu && (!is_device_ptr(U) || !is_device_ptr(wts))) || (Rres && !is_device_ptr(Rres)))
-        return fail(what + ": device pointers only");
-    const int nC = glu ? 1 : count;
-    for (int i = 0; i < nC; ++i)
-        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
+    if (experts_check(what, handles, count, n_experts, N, dtype, topk, A, U, ids, wts, Rres, C)) return -1;
+    if (n_experts > 256) return fail(what + ": n_experts must be 1..256");   // the routing kernel's shared arrays
     auto it0 = g.res.find(handles[0]);
     if (it0 == g.res.end()) return fail(what + ": bad weight handle");
     const StreamLayout &L = it0->second.L;
-    const bool tile_ok = !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0 &&
-                         (L.pb == 2 || L.pb == 4);
-    if (!tile_ok)
+    if (!tiles_take_fp(L))
         return fail(what + ": the tiles take W2/W3/W4 fp-path tensors (per-row scales, K % 128 == 0, chunk 128/64/32 K, act group inside "
                     "the chunk); use " + gemv_name + " for the others");
     const int S = N * topk, Mout = L.Mout, K = L.K, f16 = dtype == TMAC_B200_F16;
+    // GLU: the table's C is the slots' fp32 rows, so the workspace is allocated before the table is built
     if (glu && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
-    std::vector<void *> Cx((size_t)count * n_experts);     // the table's C entry i * n_experts + e: C[i] (GLU: the slots' fp32 rows)
-    for (int i = 0; i < count; ++i)
-        for (int e = 0; e < n_experts; ++e) Cx[(size_t)i * n_experts + e] = glu ? g.d_moe_ws.p : C[i];
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, Cx.data(), &R, &bp)) return -1;
-    const int agq = L.agq();
-    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, agq);
+    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, glu ? &g.d_moe_ws.p : C, &R, &bp, n_experts)) return -1;
+    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq());
     if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
-    // shared memory of both tiles as in launch_prefill
-    const size_t rawsz = ((size_t)(8 / L.qch) * L.blk + 127) & ~(size_t)127;
-    const int nsb = 128 / L.rsb, nrt = (L.nrsb + nsb - 1) / nsb;
-    const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;
-    const int nmain = K / 64, nextra = (L.nchunk + 31) / 32;
-    const size_t smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
-    const size_t rec = pf_rec_bytes(false, L.qch, agq);
-    const size_t smem8 = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
-    const bool t16 = experts_take_tile16(N, topk, n_experts) && smem16 <= 227 * 1024;
-    if (!t16 && smem8 > 225 * 1024) return fail(what + ": the tensor's blocks do not fit the int8 tile's shared memory");
+    const TilePlan t(L, false);
+    const bool t16 = experts_take_tile16(N, topk, n_experts) && t.fits16;
+    if (!t16 && !t.fits8) return fail(what + ": the tensor's blocks do not fit the int8 tile's shared memory");
     const int T = t16 ? kP16NT : kPfNT;
     const long long cap = S / T + std::min(n_experts, S);
     if (cap > 65535) return fail(what + ": N * topk too large for one launch");
-    const int rows = glu ? S : N, nag = K / L.act_group_size, nsteps = t16 ? nmain + nextra : nmain;
-    const size_t recb = t16 ? (size_t)kP16BBytes : rec;
+    const int rows = glu ? S : N, nag = K / L.act_group_size, nsteps = t16 ? t.nmain + t.nextra : t.nmain;
+    const size_t recb = t16 ? (size_t)kP16BBytes : t.rec;
     if (g.d_moe_route.ensure((size_t)cap * sizeof(int4) + (size_t)S * sizeof(int)) || (glu && g.d_moe_act.ensure((size_t)S * K * sizeof(float))) ||
         g.d_qlut.ensure((size_t)rows * K * 4) || g.d_ls.ensure((size_t)rows * nag * 4) || g.d_lb.ensure((size_t)rows * nag * 4) ||
         g.d_tiles.ensure((size_t)cap * nsteps * recb))
@@ -1428,31 +1436,20 @@ static int prefill_experts(const std::string &what, const std::string &gemv_name
     } else if (launch_preprocessor(K, N, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
     const PfRoute route{tiles, perm, bp.W, bp.C, n_experts};
     const int div = glu ? 1 : topk, out_f16 = glu ? 0 : f16;
-    const dim3 grid(nrt, (unsigned)cap, count);
+    const dim3 grid(t.nrt, (unsigned)cap, count);
     if (t16) {
-        fk.lut16<<<dim3(nsteps, (unsigned)cap), 256, 0, st>>>(qlut, ls, lb, recs, K, nmain, nextra, tiles, perm, div);
+        fk.lut16<<<dim3(nsteps, (unsigned)cap), 256, 0, st>>>(qlut, ls, lb, recs, K, t.nmain, t.nextra, tiles, perm, div);
         CUDA_OK(cudaGetLastError());
-        Prefill16Params q{};
-        q.N = N; q.K = K; q.Mout = Mout; q.ldc = Mout; q.out_f16 = out_f16;
-        q.nchunk = L.nchunk; q.zp = L.zp; q.sd = L.sd; q.blk_bytes = (int)L.blk; q.nmain = nmain; q.nextra = nextra;
-        q.rsb_stride = L.rsb_stride; q.tiles = recs; q.nrsb = L.nrsb; q.nrt = nrt; q.bits = L.bits; q.ntiles = nrt * (int)cap;
-        CUDA_OK(cudaFuncSetAttribute((const void *)fk.tile16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16));
-        fk.tile16<<<grid, kP16Threads, smem16, st>>>(q, route);
-        CUDA_OK(cudaGetLastError());
-        g.last_launch[0] = 16; g.last_launch[1] = kP16Threads / 32; g.last_launch[3] = 0;
+        auto q = tile_params<Prefill16Params>(L, t, N, Mout, out_f16);
+        q.tiles = recs; q.ntiles = t.nrt * (int)cap;   // no stream-K split
+        if (launch_tile(true, fk.tile16, grid, t, 0, L, S, q, route)) return -1;
     } else {
         fk.lut<<<dim3(nsteps, (unsigned)cap), 128, 0, st>>>(qlut, ls, lb, recs, K, tiles, perm, div);
         CUDA_OK(cudaGetLastError());
-        PrefillParams p{};
-        p.lut_tiles = recs; p.N = N; p.K = K; p.Mout = Mout; p.ldc = Mout; p.out_f16 = out_f16;
-        p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride;
-        p.nrsb = L.nrsb; p.bits = L.bits; p.qch = L.qch;
-        CUDA_OK(cudaFuncSetAttribute((const void *)fk.tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem8));
-        fk.tile<<<grid, kPfThreads2, smem8, st>>>(p, route);
-        CUDA_OK(cudaGetLastError());
-        g.last_launch[0] = 1; g.last_launch[1] = kPfThreads2 / 32; g.last_launch[3] = 1;
+        auto p = tile_params<PrefillParams>(L, t, N, Mout, out_f16);
+        p.lut_tiles = recs;   // qlut, lut_scales, lut_biases and scale0 are read on the integer path only
+        if (launch_tile(false, fk.tile, grid, t, 1, L, S, p, route)) return -1;
     }
-    g.last_launch[2] = L.nchunk; g.last_launch[4] = nrt; g.last_launch[5] = L.pb; g.last_launch[6] = 1; g.last_launch[7] = -S;
     if (glu) {
         pf_combine_launch((const float *)g.d_moe_ws.p, ids, wts, topk, n_experts, Rres, C[0], N, Mout, f16, st);
         CUDA_OK(cudaGetLastError());
