@@ -172,7 +172,8 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
 /* tmac_b200_gemv_grouped behind an input transform or before a residual add, so that a decoder layer's linears run as four launches
  * with no other ops between them: gemv_rmsnorm(q/k/v, x, w1), gemv_residual(o, att, x) -> h, gemv_rmsnorm(gate/up, h, w2),
  * gemv_glu(down, gate, up, h).  The rules of tmac_b200_gemv_grouped apply: device pointers only, the LUT built inside the launch,
- * the GEMV kernel at every N (no prefill tile), and an armed tmac_b200_peer_outputs makes the call fail.  fp-path tensors with the
+ * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual below are the prompt-sized forms), and
+ * an armed tmac_b200_peer_outputs makes the call fail.  fp-path tensors with the
  * activation group inside a chunk only.  The transform is applied in fp32 (fp16 inputs widened first) to give the input a, whose
  * LUT is built as for any input.  Each call gives exactly tmac_b200_gemv_grouped(handles, count, N, F32, a, C32) with a
  * materialised in fp32, then y = fadd_rn(C32, R) when there is a residual R (fp16 R widened), rounded once to fp16 when dtype is
@@ -187,6 +188,34 @@ TMAC_B200_API int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int 
                                          void *const *C);
 TMAC_B200_API int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
+/* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm / gemv_glu /
+ * gemv_residual, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
+ * which stream each tensor once per 128 or 256 tokens instead of once per token.  They are the routed-expert tiles of
+ * tmac_b200_prefill_experts run as one expert with the identity routing, written on the device: no host sync, graph-capturable.
+ *   Input.  The call builds the input a in fp32 exactly as the gemv_* form does (fp16 inputs widened first): prefill_rmsnorm
+ *           a[n][k] = fmul_rn(fmul_rn(H[n][k], inv_n), w[k]) with inv_n and its sum of squares in the order of seq_add_gemv_rmsnorm,
+ *           prefill_glu a = swiglu(G, U), prefill_residual a = B.  The preprocessor builds the LUT of each of the N rows once, and all
+ *           count tensors share it.
+ *   Per-row equality.  For every tensor i, row n of C[i] equals, bit for bit, row n of tmac_b200_gemv(handles[i], N, F32, a) on the
+ *           same tile kind, then y = fadd_rn(that row, R) when there is a residual R (fp16 R widened), rounded once to fp16 when dtype
+ *           is F16.  Against the float oracle: the fp16 tile within 5e-4 of max|C|, the int8 tile within 2e-5.
+ *   Tile.   One kind per launch: the fp16 tile when the prefill16 knob is on, N >= 64 and the tensor fits it, else the int8 tile -- the
+ *           dense calls' own rule, so without knobs the result is tmac_b200_gemv's wherever that call takes a tile.  prefill,
+ *           prefill_min_n and pf_streamk do not apply; no stream-K; any N >= 1.  tmac_b200_debug_last_launch reports the tile in its
+ *           own format with -N as the last field.
+ *   prefill_rmsnorm: C[i] [N][Mout] for count >= 1 tensors of one geometry (q/k/v, gate/up), all in ONE tile launch over
+ *                    (row tiles, token tiles, count).  w: fp32 [K], 16-byte aligned; eps finite, >= 0.
+ *   prefill_glu:     C = gemv(handle, a) (+ R when R != NULL), G, U [N][K], R and C [N][Mout].
+ *   prefill_residual: C = fadd_rn(gemv(handle, B), R), B [N][K], R and C [N][Mout].
+ * R may equal C.  Tensors: W2/W3/W4 fp-path tensors (per-row scales with or without zero points, K % 128 == 0, chunk 128/64/32 K, act
+ * group inside the chunk), one geometry for all.  -1 with a message, nothing launched: tensors the tiles do not take (the message
+ * names the gemv_* form to use), mixed geometry, host pointers, the gemv_* forms' own rejections (w, eps, a null R for
+ * prefill_residual), more than 65535 token tiles, an armed tmac_b200_peer_outputs (disarmed).  Workspaces are library buffers that grow
+ * with N, K and Mout: make one eager call at the largest of them before capturing a call in a CUDA graph. */
+TMAC_B200_API int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                                            void *const *C);
+TMAC_B200_API int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
+TMAC_B200_API int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
 /* Routed MoE experts: the router's top-k choice stays on the device, so a MoE FFN is two launches with no host sync and the token step
  * stays graph-capturable: gemv_experts([gate, up], h2, ids) -> G, U, then gemv_experts_glu(down, G, U, ids, weights, h) -> y.
  *   gemv_experts:     handles [count][n_experts] (host), entry i * n_experts + e = tensor i of expert e (e.g. i = 0 gate, 1 up).

@@ -1271,16 +1271,44 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
     return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kInRow, B, dtype == TMAC_B200_F16), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
-// tmac_b200_gemv_rmsnorm / _glu / _residual: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
-// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.
-static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
-                   const Gemv3Io &io, void *const *C) {
+// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual and tmac_b200_prefill_rmsnorm
+// / _glu / _residual): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w and R given are device pointers.
+static int io_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *A, const Gemv3Io &io,
+                    void *const *C) {
     if (!handles || count <= 0 || count > 65535 || !A || !C || N <= 0 || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
         return fail(what + ": bad arguments");
     if (!is_device_ptr(A) || (io.act2 && !is_device_ptr(io.act2)) || (io.nw && !is_device_ptr(io.nw)) || (io.res && !is_device_ptr(io.res)))
         return fail(what + ": device pointers only");
     for (int i = 0; i < count; ++i)
         if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
+    return 0;
+}
+static int rmsnorm_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
+                         float eps, void *const *C, Gemv3Io *io) {
+    if (!w || ((uintptr_t)w & 15)) return fail(what + ": w must be a 16-byte aligned device vector");
+    if (!(eps >= 0.f) || !std::isfinite(eps)) return fail(what + ": eps must be finite and >= 0");
+    *io = Gemv3Io{};
+    io->nw = w; io->eps = eps;
+    return io_check(what, handles, count, N, dtype, H, *io, C);
+}
+static int glu_check(const std::string &what, int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C,
+                     Gemv3Io *io) {
+    if (!U) return fail(what + ": bad arguments");
+    *io = Gemv3Io{};
+    io->act2 = U; io->res = R;
+    return io_check(what, &handle, 1, N, dtype, G, *io, &C);
+}
+static int residual_check(const std::string &what, int64_t handle, int N, int dtype, const void *B, const void *R, void *C, Gemv3Io *io) {
+    if (!R) return fail(what + ": R must not be null");
+    *io = Gemv3Io{};
+    io->res = R;
+    return io_check(what, &handle, 1, N, dtype, B, *io, &C);
+}
+
+// tmac_b200_gemv_rmsnorm / _glu / _residual: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
+// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.  The arguments are checked.
+static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
+                   const Gemv3Io &io, void *const *C) {
     const Resident *R = nullptr;
     BatchPtrs bp;
     if (grouped_setup(what.c_str(), handles, count, nullptr, nullptr, nullptr, C, &R, &bp)) return -1;
@@ -1293,28 +1321,24 @@ int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, 
                            void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    if (!w || ((uintptr_t)w & 15)) return fail("gemv_rmsnorm: w must be a 16-byte aligned device vector");
-    if (!(eps >= 0.f) || !std::isfinite(eps)) return fail("gemv_rmsnorm: eps must be finite and >= 0");
-    Gemv3Io io{};
-    io.nw = w; io.eps = eps;
+    Gemv3Io io;
+    if (rmsnorm_check("gemv_rmsnorm", handles, count, N, dtype, H, w, eps, C, &io)) return -1;
     return gemv_io("gemv_rmsnorm", handles, count, N, dtype, kInNorm, H, io, C);
 }
 
 int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    if (!U) return fail("gemv_glu: bad arguments");
-    Gemv3Io io{};
-    io.act2 = U; io.res = R;
+    Gemv3Io io;
+    if (glu_check("gemv_glu", handle, N, dtype, G, U, R, C, &io)) return -1;
     return gemv_io("gemv_glu", &handle, 1, N, dtype, kInGlu, G, io, &C);
 }
 
 int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    if (!R) return fail("gemv_residual: R must not be null");
-    Gemv3Io io{};
-    io.res = R;
+    Gemv3Io io;
+    if (residual_check("gemv_residual", handle, N, dtype, B, R, C, &io)) return -1;
     return gemv_io("gemv_residual", &handle, 1, N, dtype, kInRow, B, io, &C);
 }
 
@@ -1383,16 +1407,24 @@ int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int
 // faster at N = 256 and 512, the fp16 tile faster at N = 2048 and with uniform routing at 1024 (H100 SXM at 700 W, DESIGN.md 3.3).
 static bool experts_take_tile16(int N, int topk, int n_experts) { return g.use_prefill16 && (long long)N * topk >= 256LL * n_experts; }
 
-// tmac_b200_prefill_experts / _glu: route the slots on the device (pf_route_kernel), build the LUT of every input row once
-// (plain: B's N rows; GLU: the N * topk rows swiglu(G[s], U[s]), materialised in fp32), gather each table entry's LUT records, run
-// the routed tile over (row tiles, table entries, count), and for the GLU form combine the slots' fp32 rows.  Everything is checked
-// and every workspace allocated before anything is launched.
-static int prefill_experts(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
-                           int N, int dtype, int topk, const void *A, const void *U, const int32_t *ids, const float *wts, const void *Rres,
-                           void *const *C) {
-    const bool glu = U != nullptr;
-    if (g.npeer) { g.npeer = 0; return fail(what + ": peer outputs are for N = 1 single-tensor launches"); }
-    if (experts_check(what, handles, count, n_experts, N, dtype, topk, A, U, ids, wts, Rres, C)) return -1;
+// An armed tmac_b200_peer_outputs makes a prefill-sized call fail, and is disarmed.
+static int refuse_peer(const std::string &what) {
+    if (!g.npeer) return 0;
+    g.npeer = 0;
+    return fail(what + ": peer outputs are for N = 1 single-tensor launches");
+}
+
+// The routed tile launch of the prefill-sized calls, their arguments checked by the caller.  Routed experts (ids != null): route the
+// slots on the device (pf_route_kernel).  The dense forms (ids == null, n_experts = topk = 1): the identity routing, one table entry
+// per token tile.  Then build the LUT of every input row once (B's N rows; U != null: the N * topk rows swiglu(A[s], U[s]); nw != null:
+// the N rows rms_scale(A[n], inv_n, nw), both materialised in fp32), gather each table entry's LUT records and run the routed tile over
+// (row tiles, table entries, count).  wts != null (the GLU experts): the tile stores the slots' fp32 rows and the combine adds them
+// (+ R); otherwise the tile adds R (when not null) in its epilogue.  Everything is checked and every workspace allocated before
+// anything is launched.
+static int prefill_routed(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
+                          int N, int dtype, int topk, const void *A, const void *U, const float *nw, float eps, const int32_t *ids,
+                          const float *wts, const void *Rres, void *const *C) {
+    const bool combine = wts != nullptr, slot_rows = U != nullptr;   // slot_rows: one input row per slot (GLU), else per token
     if (n_experts > 256) return fail(what + ": n_experts must be 1..256");   // the routing kernel's shared arrays
     auto it0 = g.res.find(handles[0]);
     if (it0 == g.res.end()) return fail(what + ": bad weight handle");
@@ -1401,22 +1433,25 @@ static int prefill_experts(const std::string &what, const std::string &gemv_name
         return fail(what + ": the tiles take W2/W3/W4 fp-path tensors (per-row scales, K % 128 == 0, chunk 128/64/32 K, act group inside "
                     "the chunk); use " + gemv_name + " for the others");
     const int S = N * topk, Mout = L.Mout, K = L.K, f16 = dtype == TMAC_B200_F16;
-    // GLU: the table's C is the slots' fp32 rows, so the workspace is allocated before the table is built
-    if (glu && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
+    // combine: the table's C is the slots' fp32 rows, so the workspace is allocated before the table is built
+    if (combine && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, glu ? &g.d_moe_ws.p : C, &R, &bp, n_experts)) return -1;
+    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : C, &R, &bp, n_experts))
+        return -1;
     const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq());
     if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
     const TilePlan t(L, false);
-    const bool t16 = experts_take_tile16(N, topk, n_experts) && t.fits16;
+    // the tile rule: routed experts as experts_take_tile16, the dense forms as the dense calls (launch_prefill)
+    const bool t16 = (ids ? experts_take_tile16(N, topk, n_experts) : g.use_prefill16 && N >= 64) && t.fits16;
     if (!t16 && !t.fits8) return fail(what + ": the tensor's blocks do not fit the int8 tile's shared memory");
     const int T = t16 ? kP16NT : kPfNT;
     const long long cap = S / T + std::min(n_experts, S);
     if (cap > 65535) return fail(what + ": N * topk too large for one launch");
-    const int rows = glu ? S : N, nag = K / L.act_group_size, nsteps = t16 ? t.nmain + t.nextra : t.nmain;
+    const int rows = slot_rows ? S : N, nag = K / L.act_group_size, nsteps = t16 ? t.nmain + t.nextra : t.nmain;
+    const bool act = U || nw;                      // a materialised fp32 input
     const size_t recb = t16 ? (size_t)kP16BBytes : t.rec;
-    if (g.d_moe_route.ensure((size_t)cap * sizeof(int4) + (size_t)S * sizeof(int)) || (glu && g.d_moe_act.ensure((size_t)S * K * sizeof(float))) ||
+    if (g.d_moe_route.ensure((size_t)cap * sizeof(int4) + (size_t)S * sizeof(int)) || (act && g.d_moe_act.ensure((size_t)rows * K * sizeof(float))) ||
         g.d_qlut.ensure((size_t)rows * K * 4) || g.d_ls.ensure((size_t)rows * nag * 4) || g.d_lb.ensure((size_t)rows * nag * 4) ||
         g.d_tiles.ensure((size_t)cap * nsteps * recb))
         return fail(what + ": out of device memory (workspace)");
@@ -1427,15 +1462,16 @@ static int prefill_experts(const std::string &what, const std::string &gemv_name
     unsigned char *recs = (unsigned char *)g.d_tiles.p;
     const cudaStream_t st = g.stream();
 
-    pf_route_launch(ids, S, n_experts, T, (int)cap, tiles, perm, glu ? nullptr : bp.C, count, Mout, f16, st);
+    pf_route_launch(ids, S, n_experts, T, (int)cap, tiles, perm, ids && !combine ? bp.C : nullptr, count, Mout, f16, st);
     CUDA_OK(cudaGetLastError());
-    if (glu) {
-        pf_swiglu_launch(A, U, f16, (size_t)S * K, (float *)g.d_moe_act.p, st);
+    if (act) {
+        if (U) pf_swiglu_launch(A, U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st);
+        else pf_rmsnorm_launch(A, f16, nw, eps, rows, K, (float *)g.d_moe_act.p, st);
         CUDA_OK(cudaGetLastError());
-        if (launch_preprocessor(K, S, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
-    } else if (launch_preprocessor(K, N, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
-    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts};
-    const int div = glu ? 1 : topk, out_f16 = glu ? 0 : f16;
+        if (launch_preprocessor(K, rows, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
+    } else if (launch_preprocessor(K, rows, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
+    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts, combine ? nullptr : Rres};
+    const int div = slot_rows ? 1 : topk, out_f16 = combine ? 0 : f16;
     const dim3 grid(t.nrt, (unsigned)cap, count);
     if (t16) {
         fk.lut16<<<dim3(nsteps, (unsigned)cap), 256, 0, st>>>(qlut, ls, lb, recs, K, t.nmain, t.nextra, tiles, perm, div);
@@ -1450,7 +1486,7 @@ static int prefill_experts(const std::string &what, const std::string &gemv_name
         p.lut_tiles = recs;   // qlut, lut_scales, lut_biases and scale0 are read on the integer path only
         if (launch_tile(false, fk.tile, grid, t, 1, L, S, p, route)) return -1;
     }
-    if (glu) {
+    if (combine) {
         pf_combine_launch((const float *)g.d_moe_ws.p, ids, wts, topk, n_experts, Rres, C[0], N, Mout, f16, st);
         CUDA_OK(cudaGetLastError());
     }
@@ -1461,15 +1497,49 @@ int tmac_b200_prefill_experts(const int64_t *handles, int count, int n_experts, 
                               int topk, void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    return prefill_experts("prefill_experts", "gemv_experts", handles, count, n_experts, N, dtype, topk, B, nullptr, ids, nullptr, nullptr, C);
+    const std::string what = "prefill_experts";
+    if (refuse_peer(what) || experts_check(what, handles, count, n_experts, N, dtype, topk, B, nullptr, ids, nullptr, nullptr, C)) return -1;
+    return prefill_routed(what, "gemv_experts", handles, count, n_experts, N, dtype, topk, B, nullptr, nullptr, 0.f, ids, nullptr, nullptr, C);
 }
 
 int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
                                   const int32_t *ids, const float *weights, int topk, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    if (!U || !weights || !C) return fail("prefill_experts_glu: bad arguments");
-    return prefill_experts("prefill_experts_glu", "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, ids, weights, R, &C);
+    const std::string what = "prefill_experts_glu";
+    if (!U || !weights || !C) return fail(what + ": bad arguments");
+    if (refuse_peer(what) || experts_check(what, handles, 1, n_experts, N, dtype, topk, G, U, ids, weights, R, &C)) return -1;
+    return prefill_routed(what, "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, nullptr, 0.f, ids, weights, R, &C);
+}
+
+// tmac_b200_prefill_rmsnorm / _glu / _residual: the arguments and checks of the gemv_* form, the launch of the routed tile as one
+// expert with the identity routing.
+int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                              void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_rmsnorm";
+    Gemv3Io io;
+    if (refuse_peer(what) || rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io)) return -1;
+    return prefill_routed(what, "gemv_rmsnorm", handles, count, 1, N, dtype, 1, H, nullptr, w, eps, nullptr, nullptr, nullptr, C);
+}
+
+int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_glu";
+    Gemv3Io io;
+    if (refuse_peer(what) || glu_check(what, handle, N, dtype, G, U, R, C, &io)) return -1;
+    return prefill_routed(what, "gemv_glu", &handle, 1, 1, N, dtype, 1, G, U, nullptr, 0.f, nullptr, nullptr, R, &C);
+}
+
+int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_residual";
+    Gemv3Io io;
+    if (refuse_peer(what) || residual_check(what, handle, N, dtype, B, R, C, &io)) return -1;
+    return prefill_routed(what, "gemv_residual", &handle, 1, 1, N, dtype, 1, B, nullptr, nullptr, 0.f, nullptr, nullptr, R, &C);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

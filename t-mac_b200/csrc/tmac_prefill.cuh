@@ -141,7 +141,16 @@ struct PfRoute {
     const unsigned char *const *W;       // W[i * n_experts + e]: tensor i of expert e (the grouped pointer table)
     void *const *C;                      // C[i * n_experts + e]: where tensor i stores slot s's row, at row s of [N * topk][Mout]
     int n_experts;
+    const void *R;                       // null, or the residual added to every output: R[s][row] of C's type (the dense forms)
 };
+// A routed tile's output element C[o] = v (RES: + R[o], fp16 R widened).  R is read, then C written, by the same thread: R may be C.
+// The epilogues branch on route.R once and run a store loop per case, so the experts' loop (no R) stores as it did without it.
+template <bool RES>
+__device__ __forceinline__ void pf_route_store(const PfRoute &route, void *const &C, size_t o, float v, int out_f16) {
+    if constexpr (RES) v = __fadd_rn(v, out_f16 ? __half2float(reinterpret_cast<const __half *>(route.R)[o]) : reinterpret_cast<const float *>(route.R)[o]);
+    store_out(C, o, v, out_f16);
+}
+template <bool V> struct PfRes { static constexpr bool value = V; };
 template <bool INT_PATH, int QCH, int AGQ>
 __device__ __forceinline__ void lut_tile_rec(const int8_t *qlut, const float *ls, const float *lb, unsigned char *rec, int n, bool live,
                                              int K, int step, int t) {
@@ -278,9 +287,10 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 // warpgroup; when nrsb is odd the last tile's second super-block does not exist and its A rows are zero.
 // fp path: a step is 64 K, two per 128-K window.  INT_PATH: the integer path (see the header); a step is 64 K, p.qch / 4 of them
 // per chunk, and the staging unit is one chunk.
-// ROUTE (routed experts, fp path, prefill_experts_kernel): grid = (row tiles, table entries, count); the CTA of entry k = blockIdx.y
-// and tensor i = blockIdx.z exits at once when the entry is unused, else takes the weights W[i * n_experts + expert] of the pointer
-// table, the records of entry k (lut_tile_gather_kernel) and stores token t's row at row perm[start + t] of C[i * n_experts + expert].
+// ROUTE (routed experts and the dense prefill_* forms, fp path, prefill_experts_kernel): grid = (row tiles, table entries, count);
+// the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the entry is unused, else takes the weights
+// W[i * n_experts + expert] of the pointer table, the records of entry k (lut_tile_gather_kernel) and stores token t's row at row
+// perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one (pf_route_store).
 template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE>
 __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
@@ -484,18 +494,24 @@ __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRou
         }
         if constexpr (ROUTE) {
             void *const Cr = route.C[blockIdx.z * route.n_experts + ent.x];
+            const auto stores = [&](auto res) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row = rt * 128 + r0 + 8 * h;
-                if (row >= p.Mout) continue;
+                for (int h = 0; h < 2; ++h) {
+                    const int row = rt * 128 + r0 + 8 * h;
+                    if (row >= p.Mout) continue;
 #pragma unroll
-                for (int c8 = 0; c8 < 16; ++c8)
+                    for (int c8 = 0; c8 < 16; ++c8)
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int t = 8 * c8 + tc + e;
-                        if (t < ntok) store_out(Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row, accf[4 * c8 + 2 * h + e], p.out_f16);
-                    }
-            }
+                        for (int e = 0; e < 2; ++e) {
+                            const int t = 8 * c8 + tc + e;
+                            if (t < ntok)
+                                pf_route_store<decltype(res)::value>(route, Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row,
+                                                                     accf[4 * c8 + 2 * h + e], p.out_f16);
+                        }
+                }
+            };
+            if (route.R) stores(PfRes<true>{});
+            else stores(PfRes<false>{});
             return;
         }
 #pragma unroll

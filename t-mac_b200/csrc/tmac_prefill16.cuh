@@ -155,10 +155,10 @@ __global__ void __launch_bounds__(256) lut_tile16_gather_kernel(const int8_t *ql
 // threads 0..63 / 64..127 and consumer warpgroups 0 / 1; when nrsb is odd the last tile's second super-block does not exist and
 // its A rows are zero.
 //
-// ROUTE (routed experts, prefill16_experts_kernel): grid = (row tiles, table entries, count), no stream-K.  As in the int8 tile
-// (prefill_body): the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the entry is unused, else runs tile
-// k * nrt + blockIdx.x on the weights W[i * n_experts + expert], the B tiles of entry k, and stores token t's row at row
-// perm[start + t] of C[i * n_experts + expert].
+// ROUTE (routed experts and the dense prefill_* forms, prefill16_experts_kernel): grid = (row tiles, table entries, count), no
+// stream-K.  As in the int8 tile (prefill_body): the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the
+// entry is unused, else runs tile k * nrt + blockIdx.x on the weights W[i * n_experts + expert], the B tiles of entry k, and stores
+// token t's row at row perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one.
 template <int PB, int QCH, int AGQ, bool ROUTE>
 __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
@@ -348,18 +348,23 @@ __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const P
             if constexpr (ROUTE) {                   // one whole tile per CTA
                 void *const Cr = route.C[blockIdx.z * route.n_experts + ent.x];
                 const int row0 = (int)blockIdx.x * 128 + r0;
+                const auto stores = [&](auto res) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int row = row0 + 8 * h;
+                    for (int h = 0; h < 2; ++h) {
+                        const int row = row0 + 8 * h;
 #pragma unroll
-                    for (int c8 = 0; c8 < 32; ++c8)
+                        for (int c8 = 0; c8 < 32; ++c8)
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            const int t = 8 * c8 + tc + e;
-                            if (t < ent.z && row < p.Mout)
-                                store_out(Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row, acc[4 * c8 + 2 * h + e], p.out_f16);
-                        }
-                }
+                            for (int e = 0; e < 2; ++e) {
+                                const int t = 8 * c8 + tc + e;
+                                if (t < ent.z && row < p.Mout)
+                                    pf_route_store<decltype(res)::value>(route, Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row,
+                                                                         acc[4 * c8 + 2 * h + e], p.out_f16);
+                            }
+                    }
+                };
+                if (route.R) stores(PfRes<true>{});
+                else stores(PfRes<false>{});
                 continue;
             }
             const bool whole = fs0[f] == 0 && fs1[f] == nsteps, last = fs1[f] == nsteps;
@@ -425,9 +430,10 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_experts_kernel(const
     prefill16_body<PB, QCH, AGQ, true>(p, route);
 }
 
-// The routed-expert launches (tmac_b200_prefill_experts / _glu): the kernels of one tensor kind (PB) and fp grouping, instantiated
-// in tmac_prefill_experts.cu.  route sorts the slots by expert and writes the tile table; swiglu materialises the GLU form's
-// inputs; combine adds the GLU form's slot rows.
+// The routed launches (tmac_b200_prefill_experts / _glu, and the dense tmac_b200_prefill_rmsnorm / _glu / _residual as one expert):
+// the kernels of one tensor kind (PB) and fp grouping, instantiated in tmac_prefill_experts.cu.  route sorts the slots by expert
+// (or writes the identity routing) and the tile table; swiglu and rmsnorm materialise the GLU and norm inputs; combine adds the
+// GLU experts' slot rows.
 struct PfExpertKernels {
     void (*tile)(const PrefillParams, const PfRoute);
     void (*lut)(const int8_t *, const float *, const float *, unsigned char *, int, const int4 *, const int *, int);
@@ -438,6 +444,7 @@ PfExpertKernels pick_pf_experts(int pb, int qch, int agq);
 void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
                      int out_f16, cudaStream_t st);
 void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st);
+void pf_rmsnorm_launch(const void *H, int f16, const float *w, float eps, int N, int K, float *a, cudaStream_t st);
 void pf_combine_launch(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R, void *C, int N, int Mout,
                        int out_f16, cudaStream_t st);
 

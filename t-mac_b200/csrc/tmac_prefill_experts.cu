@@ -1,7 +1,8 @@
-// tmac_prefill_experts.cu -- the routed-expert launches at prefill sizes (tmac_b200_prefill_experts / _glu): the routing kernel
-// that groups the slots by expert, the routed instantiations of both wgmma tiles and their gathered LUT records (3 bit widths x 6 fp
-// groupings; tmac_prefill.cuh, tmac_prefill16.cuh), the GLU form's input and its combine.  In their own translation unit so that
-// they compile in parallel with tmac_b200.cu.
+// tmac_prefill_experts.cu -- the routed launches at prefill sizes: the routed experts (tmac_b200_prefill_experts / _glu) and the
+// dense transformed-input forms (tmac_b200_prefill_rmsnorm / _glu / _residual), which run as one expert with the identity routing.
+// The routing kernel that groups the slots by expert, the routed instantiations of both wgmma tiles and their gathered LUT records
+// (3 bit widths x 6 fp groupings; tmac_prefill.cuh, tmac_prefill16.cuh), the RMSNorm and GLU inputs and the GLU combine.  In their
+// own translation unit so that they compile in parallel with tmac_b200.cu.
 #include "tmac_prefill16.cuh"
 
 namespace tmac_b200 {
@@ -15,6 +16,7 @@ constexpr int kRouteThreads = 1024, kRouteWarps = kRouteThreads / 32, kRouteMaxE
 // earlier rounds) + (those in earlier warps of the round) + (those in earlier lanes of its warp) -- ascending s inside an expert.
 // Tile table: expert e's rows in runs of T from off[e], entries in expert order, the rest of the cap entries unused (ntok 0).
 // Cnan != null (the plain form): the Mout-wide rows of every invalid slot in C_i = Cnan[i * E] are quiet NaN.
+// ids == null (the dense forms): every slot is expert 0, so with E = 1 the table is {0, q * T, min(T, S - q * T), 0} and perm[s] = s.
 __global__ void __launch_bounds__(kRouteThreads) pf_route_kernel(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm,
                                                                  void *const *Cnan, int count, int ldc, int out_f16) {
     __shared__ int cnt[kRouteMaxE], off[kRouteMaxE], tb[kRouteMaxE], run[kRouteMaxE], wc[kRouteWarps][kRouteMaxE];
@@ -23,7 +25,7 @@ __global__ void __launch_bounds__(kRouteThreads) pf_route_kernel(const int32_t *
     for (int e = tid; e < E; e += kRouteThreads) { cnt[e] = 0; run[e] = 0; }
     __syncthreads();
     for (int s = tid; s < S; s += kRouteThreads) {
-        const int e = ids[s];
+        const int e = ids ? ids[s] : 0;
         if ((unsigned)e < (unsigned)E) atomicAdd(&cnt[e], 1);
     }
     __syncthreads();
@@ -38,7 +40,7 @@ __global__ void __launch_bounds__(kRouteThreads) pf_route_kernel(const int32_t *
     for (int k = used + tid; k < cap; k += kRouteThreads) tiles[k] = make_int4(0, 0, 0, 0);
     for (int base = 0; base < S; base += kRouteThreads) {
         const int s = base + tid;
-        int e = s < S ? ids[s] : -1;
+        int e = s < S ? (ids ? ids[s] : 0) : -1;
         if ((unsigned)e >= (unsigned)E) e = -1;
         for (int i = tid; i < kRouteWarps * E; i += kRouteThreads) wc[i / E][i % E] = 0;
         __syncthreads();
@@ -70,6 +72,26 @@ template <typename T>
 __global__ void __launch_bounds__(256) pf_swiglu_kernel(const T *g, const T *u, size_t n, float *a) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
         a[i] = swiglu(ld_act(g, i), ld_act(u, i));
+}
+
+// a[n][k] = rms_scale(h[n][k], inv_n, w[k]), fp16 inputs widened first: the input the GEMV's norm kind (kInNorm) builds its LUT from.
+// One CTA per row: warp 0 sums the squares in the order rms_sumsq / rms_warp_sum document (lane l: the 4-element groups l, l + 32,
+// ...), then every thread scales its elements.  K % 4 == 0.
+template <typename T>
+__global__ void __launch_bounds__(256) pf_rmsnorm_kernel(const T *h, const float *w, float eps, int K, float *a) {
+    __shared__ float inv;
+    const size_t base = (size_t)blockIdx.x * K;
+    if (threadIdx.x < 32) {
+        float s = 0.f;
+        for (int g = threadIdx.x; g < K / 4; g += 32) {
+            const size_t k = base + 4 * (size_t)g;
+            s = rms_sumsq(s, ld_act(h, k), ld_act(h, k + 1), ld_act(h, k + 2), ld_act(h, k + 3));
+        }
+        s = rms_warp_sum(s);
+        if (threadIdx.x == 0) inv = rms_inv(s, K, eps);
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < K; k += blockDim.x) a[base + k] = rms_scale(ld_act(h, base + k), inv, w[k]);
 }
 
 // C[n][row] = fadd_rn(...fadd_rn(fmul_rn(w_0, y_0), fmul_rn(w_1, y_1))..., fmul_rn(w_{topk-1}, y_{topk-1})) (+ R[n][row]), y_j =
@@ -116,6 +138,11 @@ void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a,
     const int grid = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
     if (f16) pf_swiglu_kernel<__half><<<grid, 256, 0, st>>>((const __half *)G, (const __half *)U, n, a);
     else pf_swiglu_kernel<float><<<grid, 256, 0, st>>>((const float *)G, (const float *)U, n, a);
+}
+
+void pf_rmsnorm_launch(const void *H, int f16, const float *w, float eps, int N, int K, float *a, cudaStream_t st) {
+    if (f16) pf_rmsnorm_kernel<__half><<<N, 256, 0, st>>>((const __half *)H, w, eps, K, a);
+    else pf_rmsnorm_kernel<float><<<N, 256, 0, st>>>((const float *)H, w, eps, K, a);
 }
 
 void pf_combine_launch(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R, void *C, int N, int Mout,

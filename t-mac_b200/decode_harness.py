@@ -8,7 +8,9 @@ layer's FFN (gate, up, SiLU*mul, down) is one decode sequence launch instead (to
 `post_attn_sequence=True` everything after attention -- o-projection, residual add, RMSNorm, FFN and the second residual add -- is
 one; with `fused_ops=True` the seven linears run as four library launches whose inputs and outputs take the RMSNorms, the
 SiLU*mul and the residual adds (tools/layer_bench.py times the four); adding `experts=E` makes the FFN a routed MoE of E experts with
-top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them).
+top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them).  `prompt()` is the
+prompt step: P tokens through every layer, with causal attention over cache positions [0, P) and the linears on the prefill tiles
+(tmac_b200_prefill_*; tools/prompt_bench.py times it).
 
 Not a model implementation: no tokenizer, no sampling, no checkpoint loading (SURVEY 8 f1 scope).  torch is used for device
 memory, streams and the non-matmul ops only; every linear is a library launch.
@@ -44,7 +46,7 @@ class QLinear:
         self.wt = tb.upload_plain(cfg, self.w, self.sc, self.z)
 
     def __call__(self, x, out):
-        tb.gemv(self.wt, 1, x, out)
+        tb.gemv(self.wt, x.shape[0], x, out)      # one row per token: 1 in the token step, P in the prompt step
         return out
 
     def dense(self, torch):
@@ -74,7 +76,9 @@ class DecodeLayer:
         gemv_residual(o, att, x) -> h, gemv_rmsnorm([gate, up], h, norm2), gemv_glu(down, gate, up, h).
         experts > 0 (with fused_ops): the FFN is a MoE with Mixtral's structure -- `experts` gate/up/down triples, a dense fp32 router
         Wr [experts][hidden] on h2 = rmsnorm(h) * norm2, the top `topk` logits and a softmax over them -- run as
-        gemv_experts([gate, up], h2, ids) and gemv_experts_glu(down, gate, up, ids, weights, h), with no host sync."""
+        gemv_experts([gate, up], h2, ids) and gemv_experts_glu(down, gate, up, ids, weights, h), with no host sync.
+        The prompt step (`prompt`) runs the fused_ops launches in their prefill forms (prefill_rmsnorm, prefill_residual,
+        prefill_glu, prefill_experts, prefill_experts_glu); the sequences are decode-only, so those layers run per-linear calls."""
         import torch
         if ffn_sequence and post_attn_sequence:
             raise ValueError("ffn_sequence and post_attn_sequence are alternatives: the second one contains the FFN")
@@ -100,6 +104,7 @@ class DecodeLayer:
             self.router = (0.05 * torch.randn((experts, hidden), generator=g)).cuda()
             self.buf.update(gate=torch.zeros((1, topk, ffn), device="cuda"), up=torch.zeros((1, topk, ffn), device="cuda"),
                             ids=torch.zeros((1, topk), dtype=torch.int32, device="cuda"), wts=torch.zeros((1, topk), device="cuda"))
+        self.pbuf = {}                              # the prompt step's buffers, [P][...], made by its first call
         self.ffn_seq = self.post_seq = None
         if ffn_sequence:
             seq = tb.Sequence()
@@ -134,15 +139,18 @@ class DecodeLayer:
         return x * torch.rsqrt((x * x).mean(dim=-1, keepdim=True) + eps) * w
 
     def rope(self, x, pos_cos, pos_sin):
-        t = x.view(self.heads, self.hd // 2, 2)
+        """x [n, hidden], pos_cos / pos_sin [n, hd / 2]: row i rotated by the angles of its position."""
+        t = x.view(x.shape[0], self.heads, self.hd // 2, 2)
         a, b = t[..., 0], t[..., 1]
-        return self.torch.stack((a * pos_cos - b * pos_sin, a * pos_sin + b * pos_cos), dim=-1).reshape(1, -1)
+        c, s = pos_cos[:, None, :], pos_sin[:, None, :]
+        return self.torch.stack((a * c - b * s, a * s + b * c), dim=-1).reshape(x.shape[0], -1)
 
-    def route(self, h2):
-        """The MoE router on h2 [1, hidden]: the ids (int32) and softmax weights of the top `topk` logits, in the buffers."""
+    def route(self, h2, b=None):
+        """The MoE router on h2 [n, hidden]: the ids (int32) and softmax weights of the top `topk` logits, in the buffers b."""
+        b = self.buf if b is None else b
         vals, idx = self.torch.topk(h2 @ self.router.T, self.topk, dim=-1)
-        self.buf["ids"].copy_(idx.to(self.torch.int32))
-        self.buf["wts"].copy_(self.torch.softmax(vals, dim=-1))
+        b["ids"].copy_(idx.to(self.torch.int32))
+        b["wts"].copy_(self.torch.softmax(vals, dim=-1))
 
     def forward(self, x, kcache, vcache, pos: int, pos_cos, pos_sin, linear=None, routed=None):
         """x [1, hidden] fp32 -> [1, hidden].  kcache / vcache [heads, ctx, hd]; `linear(name, inp, out)` overrides the library call
@@ -166,7 +174,7 @@ class DecodeLayer:
             self.post_seq.launch()                  # o(att) + x, rmsnorm, gate, up, down(silu(gate) * up) + h -> b["out"]
             return b["out"]
         if self.experts:
-            return self.moe(x, linear, routed)
+            return self.moe(x, linear, routed, b, 1)
         if fused:
             tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])                          # h = o(att) + x
             tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
@@ -183,31 +191,85 @@ class DecodeLayer:
             lin("down", b["act"], b["down"])
         return h + b["down"]
 
-    def moe(self, x, linear, routed):
-        """The layer after attention with the routed FFN: h = o(att) + x, h2 = rmsnorm(h) * norm2, out = h + sum_j w_j expert_j(h2)."""
-        torch, b, E = self.torch, self.buf, self.experts
+    def moe(self, x, linear, routed, b, n):
+        """The layer after attention with the routed FFN over the n rows of the buffers b (n = 1: the token step's GEMV forms, else
+        the prompt step's prefill forms): h = o(att) + x, h2 = rmsnorm(h) * norm2, out = h + sum_j w_j expert_j(h2)."""
+        torch, E = self.torch, self.experts
         if linear is None:
-            tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])
+            (tb.gemv_residual if b is self.buf else tb.prefill_residual)(self.lin["o"].wt, n, b["att"], x, b["h"])
         else:
             linear("o", b["att"], b["o"])
             b["h"].copy_(x + b["o"])
         b["h2"].copy_(self.rmsnorm(torch, b["h"], self.norm2))
         if routed is None:
-            self.route(b["h2"])
+            self.route(b["h2"], b)
         else:
             b["ids"].copy_(routed[0]); b["wts"].copy_(routed[1])
         if linear is None:
-            ex = lambda n: [self.lin["%s.%d" % (n, e)].wt for e in range(E)]
-            tb.gemv_experts([ex("gate"), ex("up")], 1, b["h2"], b["ids"], [b["gate"], b["up"]])
-            tb.gemv_experts_glu(ex("down"), 1, b["gate"], b["up"], b["ids"], b["wts"], b["out"], R=b["h"])
+            ex = lambda name: [self.lin["%s.%d" % (name, e)].wt for e in range(E)]
+            decode = b is self.buf
+            (tb.gemv_experts if decode else tb.prefill_experts)([ex("gate"), ex("up")], n, b["h2"], b["ids"], [b["gate"], b["up"]])
+            (tb.gemv_experts_glu if decode else tb.prefill_experts_glu)(ex("down"), n, b["gate"], b["up"], b["ids"], b["wts"], b["out"], R=b["h"])
             return b["out"]
-        ys = torch.zeros((E, self.hidden), device="cuda")                   # every expert, then the chosen ones: no host sync
-        g, u = torch.zeros((1, self.ffn), device="cuda"), torch.zeros((1, self.ffn), device="cuda")
+        ys = torch.zeros((E, n, self.hidden), device="cuda")                # every expert, then the chosen ones: no host sync
+        g, u = torch.zeros((n, self.ffn), device="cuda"), torch.zeros((n, self.ffn), device="cuda")
         for e in range(E):
             linear("gate.%d" % e, b["h2"], g); linear("up.%d" % e, b["h2"], u)
-            linear("down.%d" % e, torch.nn.functional.silu(g) * u, ys[e:e + 1])
-        y = (b["wts"][0, :, None] * ys[b["ids"][0].long()]).sum(dim=0, keepdim=True)
+            linear("down.%d" % e, torch.nn.functional.silu(g) * u, ys[e])
+        sel = ys[b["ids"].long(), torch.arange(n, device="cuda")[:, None]]  # [n][topk][hidden]
+        y = (b["wts"][:, :, None] * sel).sum(dim=1)
         return b["h"] + y
+
+    def prompt_buffers(self, P: int) -> dict:
+        """The prompt step's buffers for P tokens, kept for later calls (and CUDA graphs) at the same P."""
+        if self.pbuf.get("P") != P:
+            torch = self.torch
+            f = lambda *s: torch.zeros(s, device="cuda")
+            H, F = self.hidden, self.ffn
+            self.pbuf = {"P": P, "h1": f(P, H), "q": f(P, H), "k": f(P, H), "v": f(P, H), "att": f(P, H), "o": f(P, H), "h2": f(P, H),
+                         "gate": f(P, F), "up": f(P, F), "act": f(P, F), "down": f(P, H), "out": f(P, H), "h": f(P, H)}
+            if self.experts:
+                self.pbuf.update(gate=f(P, self.topk, F), up=f(P, self.topk, F), wts=f(P, self.topk),
+                                 ids=torch.zeros((P, self.topk), dtype=torch.int32, device="cuda"))
+        return self.pbuf
+
+    def prompt(self, x, kcache, vcache, cos, sin, linear=None, routed=None):
+        """The prompt step: x [P, hidden] fp32 -> [P, hidden] (a buffer of the layer).  Writes cache positions [0, P) and runs causal
+        attention over them; cos / sin [P, hd / 2] are the positions' RoPE angles.  fused_ops layers run their linears as
+        prefill_rmsnorm([q, k, v]), prefill_residual(o), prefill_rmsnorm([gate, up]) and prefill_glu(down, R=h); MoE layers as
+        prefill_rmsnorm([q, k, v]), prefill_residual(o), the torch router over the P tokens, prefill_experts([gate, up]) and
+        prefill_experts_glu(down, R=h); the other layers as one call per linear.  `linear` and `routed` as for forward."""
+        torch, P = self.torch, x.shape[0]
+        b = self.prompt_buffers(P)
+        lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
+        fused = self.fused_ops and linear is None
+        if fused:
+            tb.prefill_rmsnorm([self.lin[n].wt for n in ("q", "k", "v")], P, x, self.norm1, self.EPS, [b["q"], b["k"], b["v"]])
+        else:
+            b["h1"].copy_(self.rmsnorm(torch, x, self.norm1))
+            lin("q", b["h1"], b["q"]); lin("k", b["h1"], b["k"]); lin("v", b["h1"], b["v"])
+        q = self.rope(b["q"], cos, sin).view(P, self.heads, self.hd).transpose(0, 1)
+        kcache[:, :P] = self.rope(b["k"], cos, sin).view(P, self.heads, self.hd).transpose(0, 1)
+        vcache[:, :P] = b["v"].view(P, self.heads, self.hd).transpose(0, 1)
+        s = (q @ kcache[:, :P].transpose(1, 2)) / math.sqrt(self.hd)
+        s = s.masked_fill(torch.ones((P, P), dtype=torch.bool, device="cuda").triu(1), float("-inf"))
+        att = torch.softmax(s, dim=-1) @ vcache[:, :P]                      # [heads][P][hd]
+        b["att"].copy_(att.transpose(0, 1).reshape(P, -1))
+        if self.experts:
+            return self.moe(x, linear, routed, b, P)
+        if fused:
+            tb.prefill_residual(self.lin["o"].wt, P, b["att"], x, b["h"])                       # h = o(att) + x
+            tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
+            tb.prefill_glu(self.lin["down"].wt, P, b["gate"], b["up"], b["out"], R=b["h"])     # down(silu(gate) * up) + h
+            return b["out"]
+        lin("o", b["att"], b["o"])
+        b["h"].copy_(x + b["o"])
+        b["h2"].copy_(self.rmsnorm(torch, b["h"], self.norm2))
+        lin("gate", b["h2"], b["gate"]); lin("up", b["h2"], b["up"])
+        b["act"].copy_(torch.nn.functional.silu(b["gate"]) * b["up"])
+        lin("down", b["act"], b["down"])
+        b["out"].copy_(b["h"] + b["down"])
+        return b["out"]
 
     def free(self):
         for s in (self.ffn_seq, self.post_seq):
@@ -220,10 +282,12 @@ class DecodeLayer:
 
 class DecodeModel:
     """`layers` decoder layers of one shape (synthetic; layers > 0 share one host tensor set but own their HBM copies, so every
-    weight byte of a token streams from HBM), a KV cache of `ctx` positions, one token step per call."""
+    weight byte of a token streams from HBM), a KV cache of `ctx` positions, one token step per call.  prompt_len = P > 0: also a
+    prompt step of P tokens (`prompt()`) that fills cache positions [0, P)."""
 
     def __init__(self, layers: int, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, ctx: int = 512, seed: int = 0,
-                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2):
+                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
+                 prompt_len: int = 0):
         import torch
         self.torch, self.hidden, self.ctx, self.heads, self.hd = torch, hidden, ctx, heads, hidden // heads
         kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk)
@@ -238,7 +302,15 @@ class DecodeModel:
         self.cos, self.sin = torch.cos(ang)[None, :], torch.sin(ang)[None, :]
         self.x = torch.randn((1, hidden), device="cuda")
         self.y = torch.zeros((1, hidden), device="cuda")
-        self.graph = None
+        self.graph = self.prompt_graph = None
+        if not 0 <= prompt_len <= ctx:
+            raise ValueError("prompt_len must lie in [0, ctx]")
+        self.P = prompt_len
+        if prompt_len:
+            ang = torch.arange(prompt_len, device="cuda").float()[:, None] * inv[None, :]
+            self.pcos, self.psin = torch.cos(ang), torch.sin(ang)
+            self.px = torch.randn((prompt_len, hidden), device="cuda")
+            self.py = torch.zeros((prompt_len, hidden), device="cuda")
 
     def step(self):
         h = self.x
@@ -246,19 +318,33 @@ class DecodeModel:
             h = layer.forward(h, self.kc[i], self.vc[i], self.pos, self.cos, self.sin)
         self.y.copy_(h)
 
-    def capture(self, stream):
+    def prompt(self):
+        """The prompt step: the P rows px through every layer into py, cache positions [0, P) written."""
+        h = self.px
+        for i, layer in enumerate(self.layers):
+            h = layer.prompt(h, self.kc[i], self.vc[i], self.pcos, self.psin)
+        self.py.copy_(h)
+
+    def _graph(self, fn, stream):
         torch = self.torch
         with torch.cuda.stream(stream):
-            self.step()                             # eager warm-up: library workspaces, torch allocator
+            fn()                                    # eager warm-up: library workspaces, torch allocator
         torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph, stream=stream):
-            self.step()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, stream=stream):
+            fn()
+        return graph
+
+    def capture(self, stream):
+        self.graph = self._graph(self.step, stream)
         return self
 
-    def tokens_per_s(self, stream, n: int = 10) -> float:
+    def capture_prompt(self, stream):
+        self.prompt_graph = self._graph(self.prompt, stream)
+        return self
+
+    def _per_s(self, run, stream, n):
         torch = self.torch
-        run = self.graph.replay if self.graph is not None else self.step
         with torch.cuda.stream(stream):
             for _ in range(2):
                 run()
@@ -271,7 +357,14 @@ class DecodeModel:
         torch.cuda.synchronize()
         return n / (e0.elapsed_time(e1) * 1e-3)
 
+    def tokens_per_s(self, stream, n: int = 10) -> float:
+        return self._per_s(self.graph.replay if self.graph is not None else self.step, stream, n)
+
+    def prompt_tokens_per_s(self, stream, n: int = 10) -> float:
+        """Prompt tokens per second: P over the time of one prompt step (graphed when capture_prompt was called)."""
+        return self.P * self._per_s(self.prompt_graph.replay if self.prompt_graph is not None else self.prompt, stream, n)
+
     def free(self):
-        self.graph = None
+        self.graph = self.prompt_graph = None
         for l in self.layers:
             l.free()

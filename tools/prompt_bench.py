@@ -1,0 +1,202 @@
+"""The prompt step of the decode harness (DecodeLayer.prompt): P tokens through a stack of decoder layers with causal attention over
+cache positions [0, P), Llama-2-7B (hidden 4096, FFN 11008, 32 heads, `--layers` 32) in W2 g128 zp and W4 g128, P = 16 .. 512, in
+three forms of the linears:
+
+  prefill    the fused_ops layer's prompt step: prefill_rmsnorm([q, k, v]), prefill_residual(o), prefill_rmsnorm([gate, up]),
+             prefill_glu(down, + h) -- the wgmma tiles, one launch for q/k/v and one for gate/up;
+  per_linear the norm, SiLU * mul and residuals as torch ops and one tmac_b200_gemv per tensor (the dense call, which takes a tile
+             from its own threshold);
+  gemv_io    the same four calls in their gemv_* forms (gemv_rmsnorm, gemv_residual, gemv_glu: the GEMV kernel, whose time grows
+             with P), only up to P = --gemv-max.
+
+Each form is captured in one CUDA graph per P and replayed `--reps` times between CUDA events; the forms alternate, best of
+`--rounds`.  Reported per P: ms per prompt step, prompt tokens/s, and for the prefill form the linears' share of the step's kernel
+time (the library's kernels over all kernels, from a torch.profiler run made after the timed runs).  grouped_qkv: prefill_rmsnorm
+of q/k/v in one launch against three single-tensor launches, over all layers, graphed.  Then a Mixtral-8x7B MoE layer stack
+(`--moe-layers`, 8 experts, top-2) at P = 64 and 512: the prefill form (prefill_experts, prefill_experts_glu) against the gemv_* forms
+(gemv_experts, gemv_experts_glu).  The card's name, power limit and SM clocks are read in the same run, before and after.
+
+    python tools/prompt_bench.py [--layers 32] [--moe-layers 8] [--ps 16,32,64,128,512] [--formats w2zp,w4] [--gemv-max 128]
+"""
+import argparse
+import contextlib
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "t-mac_b200"))
+import torch                                    # noqa: E402
+import tmac_b200 as tb                          # noqa: E402
+import decode_harness                           # noqa: E402
+from decode_harness import DecodeModel          # noqa: E402
+
+FORMATS = {"w2zp": (2, True), "w4": (4, False)}
+LLAMA = dict(hidden=4096, ffn=11008, heads=32)
+MIXTRAL = dict(hidden=4096, ffn=14336, heads=32, experts=8, topk=2)
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--layers", type=int, default=32)
+ap.add_argument("--moe-layers", type=int, default=8)
+ap.add_argument("--ps", default="16,32,64,128,512")
+ap.add_argument("--moe-ps", default="64,512")
+ap.add_argument("--formats", default="w2zp,w4")
+ap.add_argument("--gemv-max", type=int, default=128)
+ap.add_argument("--reps", type=int, default=5)
+ap.add_argument("--rounds", type=int, default=3)
+args = ap.parse_args()
+
+if not torch.cuda.is_available():
+    sys.exit("prompt_bench.py needs a CUDA device")
+lib = tb.load(); tb.check(lib.tmac_b200_init(0), "init")
+st = torch.cuda.Stream(); torch.cuda.set_stream(st); tb.check(lib.tmac_b200_set_stream(st.cuda_stream), "set_stream")
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()),
+                            "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as ex:                     # the timing stands without it, but says so
+        q = "nvidia-smi unavailable: %s" % ex
+    return {"device": torch.cuda.get_device_name(), "nvidia_smi": q}
+
+
+@contextlib.contextmanager
+def gemv_forms():
+    """The harness's prefill_* calls swapped for their gemv_* forms, which take the same arguments."""
+    names = {"prefill_rmsnorm": tb.gemv_rmsnorm, "prefill_residual": tb.gemv_residual, "prefill_glu": tb.gemv_glu,
+             "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
+    saved = {n: getattr(decode_harness.tb, n) for n in names}
+    for n, f in names.items():
+        setattr(decode_harness.tb, n, f)
+    try:
+        yield
+    finally:
+        for n, f in saved.items():
+            setattr(decode_harness.tb, n, f)
+
+
+def graph(fn):
+    """A CUDA graph of fn after one eager call (workspaces, pointer tables, the allocator)."""
+    with torch.cuda.stream(st):
+        fn()
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, stream=st):
+        fn()
+    return g
+
+
+def timed(g, n):
+    """ms per replay of g, n replays between CUDA events."""
+    with torch.cuda.stream(st):
+        g.replay()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(st)
+        for _ in range(n):
+            g.replay()
+        e1.record(st)
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / n
+
+
+def best(graphs):
+    """{name: best ms per replay} over the rounds, the graphs alternating."""
+    out = {k: float("inf") for k in graphs}
+    for _ in range(args.rounds):
+        for k, g in graphs.items():
+            out[k] = min(out[k], timed(g, args.reps))
+    return out
+
+
+def library_share(fn):
+    """The library's kernels' share of fn's kernel time, from one profiled call."""
+    from torch.profiler import ProfilerActivity, profile
+    with torch.cuda.stream(st):
+        fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        with torch.cuda.stream(st):
+            fn()
+        torch.cuda.synchronize()
+    lib_us = all_us = 0.0
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None)
+        t = e.cuda_time_total if t is None else t
+        all_us += t
+        if "tmac_b200" in e.key:
+            lib_us += t
+    return lib_us / all_us if all_us else float("nan")
+
+
+def prompt_fn(m, P, x, linear=None):
+    def run():
+        h = x
+        for i, layer in enumerate(m.layers):
+            lin = None if linear is None else (lambda n, inp, out, layer=layer: layer.lin[n](inp, out))
+            h = layer.prompt(h, m.kc[i], m.vc[i], m.pcos[:P], m.psin[:P], linear=lin)
+    return run
+
+
+def dense_model(fmt, ps):
+    bits, zp = FORMATS[fmt]
+    m = DecodeModel(args.layers, bits=bits, zero_point=zp, ctx=512, fused_ops=True, prompt_len=max(ps), **LLAMA)
+    try:
+        for P in ps:
+            x = m.px[:P].contiguous()
+            forms = {"prefill": prompt_fn(m, P, x), "per_linear": prompt_fn(m, P, x, linear=True)}
+            graphs = {k: graph(f) for k, f in forms.items()}
+            if P <= args.gemv_max:
+                with gemv_forms():
+                    graphs["gemv_io"] = graph(forms["prefill"])
+            ms = best(graphs)
+            # q/k/v of every layer: one grouped launch against three single-tensor launches
+            lays = m.layers
+            h1 = torch.randn((P, LLAMA["hidden"]), device="cuda")
+            qkv = [[l.lin[n].wt for n in ("q", "k", "v")] for l in lays]
+            outs = [[l.pbuf[n] for n in ("q", "k", "v")] for l in lays]
+            grouped = graph(lambda: [tb.prefill_rmsnorm(w, P, h1, l.norm1, l.EPS, o) for w, o, l in zip(qkv, outs, lays)])
+            single = graph(lambda: [tb.prefill_rmsnorm([w[i]], P, h1, l.norm1, l.EPS, [o[i]])
+                                    for w, o, l in zip(qkv, outs, lays) for i in range(3)])
+            q = best({"grouped": grouped, "three_launches": single})
+            share = library_share(forms["prefill"])
+            res = {"model": "llama2_7b", "format": fmt, "layers": args.layers, "P": P,
+                   "ms_per_prompt": {k: round(v, 3) for k, v in ms.items()},
+                   "prompt_tokens_per_s": {k: round(P * 1e3 / v, 1) for k, v in ms.items()},
+                   "prefill_linears_share": round(share, 3),
+                   "qkv_us_per_layer": {k: round(v * 1e3 / args.layers, 1) for k, v in q.items()}}
+            print(json.dumps(res), flush=True)
+            del graphs, grouped, single
+            torch.cuda.synchronize()
+    finally:
+        m.free()
+
+
+def moe_model(fmt, ps):
+    bits, zp = FORMATS[fmt]
+    m = DecodeModel(args.moe_layers, bits=bits, zero_point=zp, ctx=512, fused_ops=True, prompt_len=max(ps), **MIXTRAL)
+    try:
+        for P in ps:
+            x = m.px[:P].contiguous()
+            graphs = {"prefill": graph(prompt_fn(m, P, x))}
+            with gemv_forms():
+                graphs["gemv_io"] = graph(prompt_fn(m, P, x))
+            ms = best(graphs)
+            print(json.dumps({"model": "mixtral_8x7b", "format": fmt, "layers": args.moe_layers, "P": P,
+                              "ms_per_prompt": {k: round(v, 3) for k, v in ms.items()},
+                              "prompt_tokens_per_s": {k: round(P * 1e3 / v, 1) for k, v in ms.items()}}), flush=True)
+            del graphs
+            torch.cuda.synchronize()
+    finally:
+        m.free()
+
+
+print(json.dumps({"card": card()}), flush=True)
+for fmt in args.formats.split(","):
+    dense_model(fmt, [int(p) for p in args.ps.split(",")])
+for fmt in args.formats.split(","):
+    if args.moe_layers:
+        moe_model(fmt, [int(p) for p in args.moe_ps.split(",")])
+print(json.dumps({"card_after": card()}), flush=True)
