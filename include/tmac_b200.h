@@ -183,11 +183,19 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
  *                 CTA computes inv_n itself).  w: fp32 [K], 16-byte aligned; eps finite, >= 0.  C[i] [N][Mout].
  *   gemv_glu:     C = gemv(handle, a) (+ R when R != NULL), a = swiglu(G, U) as for seq_add_gemv_glu.  G, U [N][K], R and C [N][Mout].
  *   gemv_residual: C = fadd_rn(gemv(handle, B), R), B [N][K], R and C [N][Mout].
+ *   gemv_subnorm: the two sub-norms of a BitNet b1.58 layer, so that its linears run as four launches too: gemv_rmsnorm(q/k/v, x, w1),
+ *                 gemv_subnorm(o, att, NULL, w_as, x) -> h, gemv_rmsnorm(gate/up, h, w2), gemv_subnorm(down, gate, up, w_fs, h).
+ *                 C = gemv(handle, a) (+ R when R != NULL), a = rmsnorm(X) * w, X = G when U == NULL (attn_sub_norm before wo),
+ *                 X = swiglu(G, U) when U != NULL (ffn_sub_norm before ffn_down).  a[n][k] = fmul_rn(fmul_rn(X[n][k], inv_n), w[k]),
+ *                 X[n][k] in fp32 (swiglu rounded as for seq_add_gemv_glu), inv_n and its sum of squares of X as for gemv_rmsnorm.
+ *                 G, U [N][K], R and C [N][Mout]; w and eps as for gemv_rmsnorm.
  * R may equal C (each element is read and written by the same thread). */
 TMAC_B200_API int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                                          void *const *C);
 TMAC_B200_API int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
+TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                         const void *R, void *C);
 /* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm / gemv_glu /
  * gemv_residual, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
  * which stream each tensor once per 128 or 256 tokens instead of once per token.  They are the routed-expert tiles of

@@ -298,6 +298,7 @@ gemv3_fn pick_gemv3(int pb, bool sym, int qch, int agq, int minb, int in) {
         case kInRow: return pick_gemv3_in<kInRow>(pb, sym, qch, agq, minb);
         case kInNorm: return pick_gemv3_in<kInNorm>(pb, sym, qch, agq, minb);
         case kInGlu: return pick_gemv3_in<kInGlu>(pb, sym, qch, agq, minb);
+        case kInGluNorm: return pick_gemv3_in<kInGluNorm>(pb, sym, qch, agq, minb);
         case kInExperts: return pick_gemv3_in<kInExperts>(pb, sym, qch, agq, minb);
         case kInExpertsGlu: return pick_gemv3_in<kInExpertsGlu>(pb, sym, qch, agq, minb);
         default: return nullptr;
@@ -408,7 +409,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const Gem
     const size_t wregion = std::max((size_t)p.wpc * (p.nbuf * L.blk + (size_t)L.qch * 4 * (sym ? 8 : 16)), (size_t)p.wpc * L.rsb * 4);
     size_t smem = (size_t)p.cs * L.rsb * 4 + ((wregion + 15) & ~(size_t)15) + (size_t)p.wpc * 16;   // + warp-private mbarriers
     if (in.kind != kInTable && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
-    if (in.kind == kInNorm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
+    if (in.kind == kInNorm || in.kind == kInGluNorm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
     if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t wtx, wty;
     plane_weight_regs(L.bits, sym, &wtx, &wty);
@@ -1271,8 +1272,9 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
     return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kInRow, B, dtype == TMAC_B200_F16), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
-// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual and tmac_b200_prefill_rmsnorm
-// / _glu / _residual): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w and R given are device pointers.
+// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm and
+// tmac_b200_prefill_rmsnorm / _glu / _residual): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
+// and R given are device pointers.
 static int io_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *A, const Gemv3Io &io,
                     void *const *C) {
     if (!handles || count <= 0 || count > 65535 || !A || !C || N <= 0 || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
@@ -1283,12 +1285,13 @@ static int io_check(const std::string &what, const int64_t *handles, int count, 
         if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
     return 0;
 }
+// U and R: gemv_subnorm's SwiGLU up rows and residual, or null.
 static int rmsnorm_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
-                         float eps, void *const *C, Gemv3Io *io) {
+                         float eps, void *const *C, Gemv3Io *io, const void *U = nullptr, const void *R = nullptr) {
     if (!w || ((uintptr_t)w & 15)) return fail(what + ": w must be a 16-byte aligned device vector");
     if (!(eps >= 0.f) || !std::isfinite(eps)) return fail(what + ": eps must be finite and >= 0");
     *io = Gemv3Io{};
-    io->nw = w; io->eps = eps;
+    io->nw = w; io->eps = eps; io->act2 = U; io->res = R;
     return io_check(what, handles, count, N, dtype, H, *io, C);
 }
 static int glu_check(const std::string &what, int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C,
@@ -1305,7 +1308,7 @@ static int residual_check(const std::string &what, int64_t handle, int N, int dt
     return io_check(what, &handle, 1, N, dtype, B, *io, &C);
 }
 
-// tmac_b200_gemv_rmsnorm / _glu / _residual: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
+// tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
 // gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.  The arguments are checked.
 static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
                    const Gemv3Io &io, void *const *C) {
@@ -1340,6 +1343,15 @@ int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, con
     Gemv3Io io;
     if (residual_check("gemv_residual", handle, N, dtype, B, R, C, &io)) return -1;
     return gemv_io("gemv_residual", &handle, 1, N, dtype, kInRow, B, io, &C);
+}
+
+int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps, const void *R,
+                           void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    Gemv3Io io;
+    if (rmsnorm_check("gemv_subnorm", &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
+    return gemv_io("gemv_subnorm", &handle, 1, N, dtype, U ? kInGluNorm : kInNorm, G, io, &C);
 }
 
 // The checks both routed-expert call forms share (tmac_b200_gemv_experts / _glu and tmac_b200_prefill_experts / _glu): the

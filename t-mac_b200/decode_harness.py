@@ -8,7 +8,8 @@ layer's FFN (gate, up, SiLU*mul, down) is one decode sequence launch instead (to
 `post_attn_sequence=True` everything after attention -- o-projection, residual add, RMSNorm, FFN and the second residual add -- is
 one; with `fused_ops=True` the seven linears run as four library launches whose inputs and outputs take the RMSNorms, the
 SiLU*mul and the residual adds (tools/layer_bench.py times the four); adding `experts=E` makes the FFN a routed MoE of E experts with
-top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them).  `prompt()` is the
+top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them); `sub_norms=True`
+makes the layer BitNet b1.58's, with an RMSNorm before o and one before down (tools/layer_bench.py --bitnet).  `prompt()` is the
 prompt step: P tokens through every layer, with causal attention over cache positions [0, P) and the linears on the prefill tiles
 (tmac_b200_prefill_*; tools/prompt_bench.py times it).
 
@@ -28,7 +29,9 @@ import tmac_b200 as tb
 class QLinear:
     """One quantised linear resident in HBM: y = gemv(W, x) through tmac_b200_gemv (LUT build fused for the fp path)."""
 
-    def __init__(self, mout: int, k: int, bits: int, group_size: int, zero_point: bool, seed: int, one_scale: bool = False, share: Optional["QLinear"] = None):
+    def __init__(self, mout: int, k: int, bits: int, group_size: int, zero_point: bool, seed: int, one_scale: bool = False, share: Optional["QLinear"] = None,
+                 act_group_size: Optional[int] = None):
+        """act_group_size: K positions per LUT scale; by default the whole row (the integer path) for one_scale tensors, else 64."""
         self.mout, self.k, self.bits, self.gs, self.zp, self.one_scale = mout, k, bits, group_size, zero_point, one_scale
         if share is not None:                       # another layer with the same synthetic tensor: its own HBM copy, one host encode
             self.w, self.sc, self.z, self.wt = share.w, share.sc, share.z, tb.clone(share.wt)
@@ -42,7 +45,9 @@ class QLinear:
             self.sc = (np.abs(rng.standard_normal((mout, k // group_size))) * 0.01 + 1e-4).astype(np.float16).astype(np.float32)
             self.z = (rng.standard_normal((mout, k // group_size)) * 0.01).astype(np.float16).astype(np.float32) if zero_point else None
         bm = next(b for b in ((192, 384, 576, 768) if bits == 3 else (256, 128, 512, 1024, 320, 640)) if (mout * bits) % b == 0)
-        cfg = tb.make_kcfg(mout, k, bits, bm, 16, group_size, k if one_scale else 64, zero_point, one_scale)
+        if act_group_size is None:
+            act_group_size = k if one_scale else 64
+        cfg = tb.make_kcfg(mout, k, bits, bm, 16, group_size, act_group_size, zero_point, one_scale)
         self.wt = tb.upload_plain(cfg, self.w, self.sc, self.z)
 
     def __call__(self, x, out):
@@ -66,7 +71,8 @@ class QLinear:
 
 class DecodeLayer:
     def __init__(self, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, seed: int, share: Optional["DecodeLayer"] = None, group_size: int = 128,
-                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2):
+                 ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
+                 sub_norms: bool = False):
         """ffn_sequence: the FFN (gate, up, SiLU*mul, down) runs as ONE decode sequence whose down op reads the gated activation of
         the gate and up ops (tmac_b200_seq_add_gemv_glu) instead of three launches and a torch op.
         post_attn_sequence: the layer after attention runs as ONE decode sequence [o(att) + x, gate(rmsnorm(h) * w2),
@@ -77,8 +83,13 @@ class DecodeLayer:
         experts > 0 (with fused_ops): the FFN is a MoE with Mixtral's structure -- `experts` gate/up/down triples, a dense fp32 router
         Wr [experts][hidden] on h2 = rmsnorm(h) * norm2, the top `topk` logits and a softmax over them -- run as
         gemv_experts([gate, up], h2, ids) and gemv_experts_glu(down, gate, up, ids, weights, h), with no host sync.
+        sub_norms: a BitNet b1.58 layer -- ternary one-scale tensors (bits = 2) with activation groups of 64, and two more RMSNorms,
+        o(rmsnorm(att) * w_as) and down(rmsnorm(silu(gate) * up) * w_fs) (HF attn inner_attn_ln and mlp ffn_layernorm).  With
+        fused_ops the linears still run as four launches: gemv_rmsnorm([q, k, v], x, norm1), gemv_subnorm(o, att, w_as, R=x) -> h,
+        gemv_rmsnorm([gate, up], h, norm2), gemv_subnorm(down, gate, w_fs, U=up, R=h).
         The prompt step (`prompt`) runs the fused_ops launches in their prefill forms (prefill_rmsnorm, prefill_residual,
-        prefill_glu, prefill_experts, prefill_experts_glu); the sequences are decode-only, so those layers run per-linear calls."""
+        prefill_glu, prefill_experts, prefill_experts_glu); the sequences are decode-only, and the prefill tiles take no one-scale
+        tensor, so sequence and sub_norms layers run per-linear calls."""
         import torch
         if ffn_sequence and post_attn_sequence:
             raise ValueError("ffn_sequence and post_attn_sequence are alternatives: the second one contains the FFN")
@@ -88,12 +99,18 @@ class DecodeLayer:
             raise ValueError("experts > 0 runs the routed FFN with the fused_ops launches; it needs fused_ops and no sequence")
         if experts and not 1 <= topk <= min(experts, 8):
             raise ValueError("topk must lie in [1, min(experts, 8)]")
-        self.fused_ops, self.experts, self.topk = fused_ops, experts, topk
+        if sub_norms and (ffn_sequence or post_attn_sequence or experts):
+            raise ValueError("sub_norms has no sequence op and no routed FFN: it cannot be combined with a sequence or experts")
+        if sub_norms and bits != 2:
+            raise ValueError("sub_norms layers have ternary weights: bits must be 2")
+        self.fused_ops, self.experts, self.topk, self.sub_norms = fused_ops, experts, topk, sub_norms
         self.torch, self.hidden, self.ffn, self.heads, self.hd = torch, hidden, ffn, heads, hidden // heads
         names = [("q", hidden, hidden), ("k", hidden, hidden), ("v", hidden, hidden), ("o", hidden, hidden)]
         ffn_names = [("gate", ffn, hidden), ("up", ffn, hidden), ("down", hidden, ffn)]
         names += ffn_names if not experts else [("%s.%d" % (n, e), m, k) for e in range(experts) for n, m, k in ffn_names]
-        self.lin = {n: QLinear(m, k, bits, group_size, zero_point, seed + i, share=share.lin[n] if share else None) for i, (n, m, k) in enumerate(names)}
+        qkw = dict(zero_point=False, one_scale=True, act_group_size=64) if sub_norms else dict(zero_point=zero_point)
+        self.lin = {n: QLinear(m, k, bits, group_size, seed=seed + i, share=share.lin[n] if share else None, **qkw)
+                    for i, (n, m, k) in enumerate(names)}
         g = torch.Generator(device="cpu").manual_seed(seed)
         self.norm1 = (1.0 + 0.1 * torch.randn(hidden, generator=g)).cuda()
         self.norm2 = (1.0 + 0.1 * torch.randn(hidden, generator=g)).cuda()
@@ -104,6 +121,10 @@ class DecodeLayer:
             self.router = (0.05 * torch.randn((experts, hidden), generator=g)).cuda()
             self.buf.update(gate=torch.zeros((1, topk, ffn), device="cuda"), up=torch.zeros((1, topk, ffn), device="cuda"),
                             ids=torch.zeros((1, topk), dtype=torch.int32, device="cuda"), wts=torch.zeros((1, topk), device="cuda"))
+        if sub_norms:
+            self.w_as = (1.0 + 0.1 * torch.randn(hidden, generator=g)).cuda()
+            self.w_fs = (1.0 + 0.1 * torch.randn(ffn, generator=g)).cuda()
+            self.buf["att_n"] = f(hidden)
         self.pbuf = {}                              # the prompt step's buffers, [P][...], made by its first call
         self.ffn_seq = self.post_seq = None
         if ffn_sequence:
@@ -175,21 +196,38 @@ class DecodeLayer:
             return b["out"]
         if self.experts:
             return self.moe(x, linear, routed, b, 1)
+        if fused and self.sub_norms:
+            tb.gemv_subnorm(self.lin["o"].wt, 1, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
+            tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
+            tb.gemv_subnorm(self.lin["down"].wt, 1, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
+            return b["out"]                                                                   # down(rmsnorm(silu(gate) * up) * w_fs) + h
         if fused:
             tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])                          # h = o(att) + x
             tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
             tb.gemv_glu(self.lin["down"].wt, 1, b["gate"], b["up"], b["out"], R=b["h"])        # down(silu(gate) * up) + h
             return b["out"]
-        lin("o", b["att"], b["o"])
+        lin("o", self.attn_sub_norm(b), b["o"])
         h = x + b["o"]
         b["h2"].copy_(self.rmsnorm(torch, h, self.norm2))
         if self.ffn_seq is not None and linear is None:
             self.ffn_seq.launch()                   # gate(h2), up(h2), down(silu(gate) * up) -> b["down"]
         else:
             lin("gate", b["h2"], b["gate"]); lin("up", b["h2"], b["up"])
-            b["act"].copy_(torch.nn.functional.silu(b["gate"]) * b["up"])
+            self.ffn_act(b)
             lin("down", b["act"], b["down"])
         return h + b["down"]
+
+    def attn_sub_norm(self, b):
+        """The o projection's input from the buffers b: att, or rmsnorm(att) * w_as in a sub_norms layer (torch ops)."""
+        if not self.sub_norms:
+            return b["att"]
+        b["att_n"].copy_(self.rmsnorm(self.torch, b["att"], self.w_as))
+        return b["att_n"]
+
+    def ffn_act(self, b):
+        """b["act"] = silu(gate) * up, then rmsnorm(.) * w_fs in a sub_norms layer (torch ops)."""
+        act = self.torch.nn.functional.silu(b["gate"]) * b["up"]
+        b["act"].copy_(self.rmsnorm(self.torch, act, self.w_fs) if self.sub_norms else act)
 
     def moe(self, x, linear, routed, b, n):
         """The layer after attention with the routed FFN over the n rows of the buffers b (n = 1: the token step's GEMV forms, else
@@ -227,7 +265,7 @@ class DecodeLayer:
             f = lambda *s: torch.zeros(s, device="cuda")
             H, F = self.hidden, self.ffn
             self.pbuf = {"P": P, "h1": f(P, H), "q": f(P, H), "k": f(P, H), "v": f(P, H), "att": f(P, H), "o": f(P, H), "h2": f(P, H),
-                         "gate": f(P, F), "up": f(P, F), "act": f(P, F), "down": f(P, H), "out": f(P, H), "h": f(P, H)}
+                         "gate": f(P, F), "up": f(P, F), "act": f(P, F), "down": f(P, H), "out": f(P, H), "h": f(P, H), "att_n": f(P, H)}
             if self.experts:
                 self.pbuf.update(gate=f(P, self.topk, F), up=f(P, self.topk, F), wts=f(P, self.topk),
                                  ids=torch.zeros((P, self.topk), dtype=torch.int32, device="cuda"))
@@ -238,11 +276,12 @@ class DecodeLayer:
         attention over them; cos / sin [P, hd / 2] are the positions' RoPE angles.  fused_ops layers run their linears as
         prefill_rmsnorm([q, k, v]), prefill_residual(o), prefill_rmsnorm([gate, up]) and prefill_glu(down, R=h); MoE layers as
         prefill_rmsnorm([q, k, v]), prefill_residual(o), the torch router over the P tokens, prefill_experts([gate, up]) and
-        prefill_experts_glu(down, R=h); the other layers as one call per linear.  `linear` and `routed` as for forward."""
+        prefill_experts_glu(down, R=h); the other layers (sub_norms layers too) as one call per linear.  `linear` and `routed` as
+        for forward."""
         torch, P = self.torch, x.shape[0]
         b = self.prompt_buffers(P)
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
-        fused = self.fused_ops and linear is None
+        fused = self.fused_ops and not self.sub_norms and linear is None
         if fused:
             tb.prefill_rmsnorm([self.lin[n].wt for n in ("q", "k", "v")], P, x, self.norm1, self.EPS, [b["q"], b["k"], b["v"]])
         else:
@@ -262,11 +301,11 @@ class DecodeLayer:
             tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
             tb.prefill_glu(self.lin["down"].wt, P, b["gate"], b["up"], b["out"], R=b["h"])     # down(silu(gate) * up) + h
             return b["out"]
-        lin("o", b["att"], b["o"])
+        lin("o", self.attn_sub_norm(b), b["o"])
         b["h"].copy_(x + b["o"])
         b["h2"].copy_(self.rmsnorm(torch, b["h"], self.norm2))
         lin("gate", b["h2"], b["gate"]); lin("up", b["h2"], b["up"])
-        b["act"].copy_(torch.nn.functional.silu(b["gate"]) * b["up"])
+        self.ffn_act(b)
         lin("down", b["act"], b["down"])
         b["out"].copy_(b["h"] + b["down"])
         return b["out"]
@@ -287,10 +326,11 @@ class DecodeModel:
 
     def __init__(self, layers: int, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, ctx: int = 512, seed: int = 0,
                  ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
-                 prompt_len: int = 0):
+                 prompt_len: int = 0, sub_norms: bool = False):
         import torch
         self.torch, self.hidden, self.ctx, self.heads, self.hd = torch, hidden, ctx, heads, hidden // heads
-        kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk)
+        kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk,
+                  sub_norms=sub_norms)
         first = DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, **kw)
         self.layers: List[DecodeLayer] = [first] + [DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, share=first, **kw)
                                                     for _ in range(layers - 1)]

@@ -3,9 +3,12 @@ ways: every linear its own launch ("off"), each FFN one decode sequence ("ffn_se
 o-projection, residual add, RMSNorm, FFN, second residual add -- one decode sequence ("post_attn_sequence"), and the linears as
 four launches that take the RMSNorms, the SiLU*mul and the residual adds into their inputs and outputs ("fused_ops").  The models are
 resident together and timed alternately, best of `--rounds`; the kernel serving each layer's sequence is recorded beside the time,
-and so are the card's name, power limit and max SM clock.
+and so are the card's name, power limit and max SM clock.  With `--bitnet` the layers are BitNet-3B's (26 layers, hidden 3200,
+FFN 8640, 32 heads; ternary one-scale tensors with activation groups of 64, and the attn / ffn sub-norms), timed in the modes
+"off" and "fused_ops".
 
     python tools/layer_bench.py [--layers 32] [--reps 20] [--rounds 3] [--formats w2zp,w4]
+    python tools/layer_bench.py --bitnet [--layers 26] [...]
     python tools/layer_bench.py --profile [...]     # kernels per token of each mode (torch.profiler, one eager step; no timing)
 """
 import argparse
@@ -26,12 +29,20 @@ MODES = {"off": {}, "ffn_sequence": {"ffn_sequence": True}, "post_attn_sequence"
          "fused_ops": {"fused_ops": True}}
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=32)
+ap.add_argument("--layers", type=int, default=None, help="default 32, 26 with --bitnet")
 ap.add_argument("--reps", type=int, default=20)
 ap.add_argument("--rounds", type=int, default=3)
 ap.add_argument("--formats", default="w2zp,w4")
 ap.add_argument("--profile", action="store_true", help="count the kernels of one token step per mode instead of timing")
+ap.add_argument("--bitnet", action="store_true", help="BitNet-3B layers with sub-norms, modes off and fused_ops")
 args = ap.parse_args()
+if args.bitnet:
+    HIDDEN, FFN, HEADS = 3200, 8640, 32
+    FORMATS = {"bitnet": (2, False)}
+    MODES = {"off": {"sub_norms": True}, "fused_ops": {"sub_norms": True, "fused_ops": True}}
+    args.formats = "bitnet"
+if args.layers is None:
+    args.layers = 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("layer_bench.py needs a CUDA device")
@@ -66,7 +77,7 @@ def kernels_per_token(m):
         torch.cuda.synchronize()
     names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
     kern = [n for n in names if not n.startswith(("Memcpy", "Memset"))]
-    return {"kernels": len(kern), "memcpy_memset": len(names) - len(kern)}
+    return {"kernels": len(kern), "library_kernels": sum("tmac_b200::" in n for n in kern), "memcpy_memset": len(names) - len(kern)}
 
 
 def case(fmt):
