@@ -172,7 +172,7 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
 /* tmac_b200_gemv_grouped behind an input transform or before a residual add, so that a decoder layer's linears run as four launches
  * with no other ops between them: gemv_rmsnorm(q/k/v, x, w1), gemv_residual(o, att, x) -> h, gemv_rmsnorm(gate/up, h, w2),
  * gemv_glu(down, gate, up, h).  The rules of tmac_b200_gemv_grouped apply: device pointers only, the LUT built inside the launch,
- * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual below are the prompt-sized forms), and
+ * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm below are the prompt-sized forms), and
  * an armed tmac_b200_peer_outputs makes the call fail.  fp-path tensors with the
  * activation group inside a chunk only.  The transform is applied in fp32 (fp16 inputs widened first) to give the input a, whose
  * LUT is built as for any input.  Each call gives exactly tmac_b200_gemv_grouped(handles, count, N, F32, a, C32) with a
@@ -197,15 +197,17 @@ TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, cons
 TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                          const void *R, void *C);
 /* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm / gemv_glu /
- * gemv_residual, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
+ * gemv_residual / gemv_subnorm, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
  * which stream each tensor once per 128 or 256 tokens instead of once per token.  They are the routed-expert tiles of
  * tmac_b200_prefill_experts run as one expert with the identity routing, written on the device: no host sync, graph-capturable.
  *   Input.  The call builds the input a in fp32 exactly as the gemv_* form does (fp16 inputs widened first): prefill_rmsnorm
  *           a[n][k] = fmul_rn(fmul_rn(H[n][k], inv_n), w[k]) with inv_n and its sum of squares in the order of seq_add_gemv_rmsnorm,
- *           prefill_glu a = swiglu(G, U), prefill_residual a = B.  The preprocessor builds the LUT of each of the N rows once, and all
+ *           prefill_glu a = swiglu(G, U), prefill_residual a = B, prefill_subnorm the a of gemv_subnorm (X = G or swiglu(G, U) in
+ *           fp32, then its RMS norm in the order of gemv_rmsnorm).  The preprocessor builds the LUT of each of the N rows once, and all
  *           count tensors share it.
  *   Per-row equality.  For every tensor i, row n of C[i] equals, bit for bit, row n of tmac_b200_gemv(handles[i], N, F32, a) on the
- *           same tile kind, then y = fadd_rn(that row, R) when there is a residual R (fp16 R widened), rounded once to fp16 when dtype
+ *           same tile kind (a one-scale tensor: that call on its twin, the same codes with per-row scales all equal to its scale,
+ *           no zero points, the same group and act group), then y = fadd_rn(that row, R) when there is a residual R (fp16 R widened), rounded once to fp16 when dtype
  *           is F16.  Against the float oracle: the fp16 tile within 5e-4 of max|C|, the int8 tile within 2e-5.
  *   Tile.   One kind per launch: the fp16 tile when the prefill16 knob is on, N >= 64 and the tensor fits it, else the int8 tile -- the
  *           dense calls' own rule, so without knobs the result is tmac_b200_gemv's wherever that call takes a tile.  prefill,
@@ -215,8 +217,13 @@ TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const
  *                    (row tiles, token tiles, count).  w: fp32 [K], 16-byte aligned; eps finite, >= 0.
  *   prefill_glu:     C = gemv(handle, a) (+ R when R != NULL), G, U [N][K], R and C [N][Mout].
  *   prefill_residual: C = fadd_rn(gemv(handle, B), R), B [N][K], R and C [N][Mout].
- * R may equal C.  Tensors: W2/W3/W4 fp-path tensors (per-row scales with or without zero points, K % 128 == 0, chunk 128/64/32 K, act
- * group inside the chunk), one geometry for all.  -1 with a message, nothing launched: tensors the tiles do not take (the message
+ *   prefill_subnorm: C = gemv(handle, a) (+ R when R != NULL), G, U (or NULL) [N][K], R and C [N][Mout]; w and eps as for
+ *                    prefill_rmsnorm.  A BitNet b1.58 prompt's linears run as prefill_rmsnorm(q/k/v, x, w1),
+ *                    prefill_subnorm(o, att, NULL, w_as, x) -> h, prefill_rmsnorm(gate/up, h, w2), prefill_subnorm(down, gate, up, w_fs, h).
+ * R may equal C.  Tensors: W2/W3/W4 fp-path tensors with the act group inside the chunk: per-row scales with or without zero points,
+ * K % 128 == 0, chunk 128/64/32 K; or one scale with act group 128, 64 or 32 K < K and K % 128 == 0 (chunk 128 K) or K % 128 == 64
+ * (chunk 64 K, e.g. BitNet-3B's down projection, K = 8640: the int8 tile at every N, whatever the prefill16 knob).  One geometry
+ * for all.  -1 with a message, nothing launched: tensors the tiles do not take (the message
  * names the gemv_* form to use), mixed geometry, host pointers, the gemv_* forms' own rejections (w, eps, a null R for
  * prefill_residual), more than 65535 token tiles, an armed tmac_b200_peer_outputs (disarmed).  Workspaces are library buffers that grow
  * with N, K and Mout: make one eager call at the largest of them before capturing a call in a CUDA graph. */
@@ -224,6 +231,8 @@ TMAC_B200_API int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, i
                                             void *const *C);
 TMAC_B200_API int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
+TMAC_B200_API int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                            const void *R, void *C);
 /* Routed MoE experts: the router's top-k choice stays on the device, so a MoE FFN is two launches with no host sync and the token step
  * stays graph-capturable: gemv_experts([gate, up], h2, ids) -> G, U, then gemv_experts_glu(down, G, U, ids, weights, h) -> y.
  *   gemv_experts:     handles [count][n_experts] (host), entry i * n_experts + e = tensor i of expert e (e.g. i = 0 gate, 1 up).
@@ -264,8 +273,8 @@ TMAC_B200_API int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_exper
  *   prefill_experts_glu: C[n] = fadd_rn(...fadd_rn(fmul_rn(w_0, y_0), fmul_rn(w_1, y_1))..., fmul_rn(w_{topk-1}, y_{topk-1}))
  *                        (+ R[n]), y_j the fp32 row of slot n * topk + j; the expression and layouts of gemv_experts_glu (no fma
  *                        contraction, fp16 R widened, rounded once for F16, R may equal C).
- * Tensors: W2/W3/W4 fp-path tensors (per-row scales with or without zero points, K % 128 == 0, chunk 128/64/32 K, act group inside
- * the chunk), one geometry for all.  An id outside [0, n_experts) is dropped from the grouping and nothing is read out of bounds:
+ * Tensors: those of tmac_b200_prefill_rmsnorm (per-row scales with K % 128 == 0, or one scale with act group < K and K % 128 == 0
+ * or 64; a one-scale expert's slot equals the same call on its twin), one geometry for all.  An id outside [0, n_experts) is dropped from the grouping and nothing is read out of bounds:
  * prefill_experts stores quiet NaN in that slot's row, prefill_experts_glu in that token's whole output; other slots and tokens are
  * unaffected.  Repeated ids are independent slots.  -1 with a message, nothing launched: W1, integer-path and other tensors the tiles
  * do not take (gemv_experts is the call for them), host pointers, topk outside 1..8, n_experts outside 1..256,

@@ -456,6 +456,15 @@ static bool tiles_take_fp(const StreamLayout &L) {
     return !L.one_scale && L.K % 128 == 0 && (L.qch == 8 || L.qch == 4 || L.qch == 2) && L.ck % L.act_group_size == 0 && (L.pb == 2 || L.pb == 4);
 }
 
+// The tensors the routed tiles take (the prefill_* forms, tmac_prefill_experts.cu): those of tiles_take_fp, and one-scale fp-path
+// W2/W3/W4 tensors (act group 128, 64 or 32 K < K) with K % 128 == 0 (chunk 128 K, both tiles) or K % 128 == 64 (chunk 64 K, the
+// int8 tile only: TilePlan::fits16 is false).
+static bool routed_tiles_take(const StreamLayout &L) {
+    if (tiles_take_fp(L)) return true;
+    return L.one_scale && !L.int_path() && (L.pb == 2 || L.pb == 4) &&
+           ((L.K % 128 == 0 && L.qch == 8) || (L.K % 128 == 64 && L.qch == 4));
+}
+
 // Whether N activation rows against this tensor take a prefill tile (with a symmetric LUT): N >= tile_min_n, and either an fp-path
 // tensor the tiles take or the integer path (W2 or W3/W4 streams, one scale, act group K, chunk 128 or 64).
 bool takes_prefill_tile(const StreamLayout &L, int N) {
@@ -469,8 +478,9 @@ struct TilePlan {
     size_t rec, smem16, smem8;     // the int8 tile's LUT record bytes; both tiles' dynamic shared memory
     bool fits16, fits8;
     TilePlan(const StreamLayout &L, bool int_path) {
-        // the producers stage a 128-K window of 128 / ck chunk blocks (integer path: one chunk)
-        const size_t rawsz = ((int_path ? 1 : 8 / L.qch) * L.blk + 127) & ~(size_t)127;
+        // the producers stage a 128-K window of 128 / ck chunk blocks (integer path, K % 128 == 64: one chunk)
+        const bool unit1 = int_path || L.K % 128;
+        const size_t rawsz = ((unit1 ? 1 : 8 / L.qch) * L.blk + 127) & ~(size_t)127;
         // a row tile is 128 rows: one W2 super-block, two W3/W4 super-blocks (64 rows each) whose blocks the producers stage together
         const int nsb = 128 / L.rsb;
         const size_t rawall = 2 * (size_t)nsb * rawsz, xtab = (size_t)128 * L.pb * 8;   // + the expansion table (fp16 tile: PB 4 only)
@@ -478,7 +488,7 @@ struct TilePlan {
         rec = pf_rec_bytes(int_path, L.qch, L.agq());
         smem16 = (size_t)kP16NA * kP16SubA + (size_t)kP16NB * kP16SubB + rawall + (L.pb == 4 ? xtab : 0) + (2 * kP16NA + 2 * kP16NB + 2) * 8 + 1024;
         smem8 = (size_t)kPfStages * (kPfStageBytes + rec) + rawall + xtab + (2 * kPfStages + 4) * 8 + 1024;
-        fits16 = smem16 <= kP16MaxSmem; fits8 = smem8 <= kPfMaxSmem;
+        fits16 = smem16 <= kP16MaxSmem && L.K % 128 == 0; fits8 = smem8 <= kPfMaxSmem;
     }
 };
 
@@ -488,6 +498,7 @@ template <class P> static P tile_params(const StreamLayout &L, const TilePlan &t
     P p{};
     p.N = N; p.K = L.K; p.Mout = L.Mout; p.ldc = ldc; p.out_f16 = out_f16;
     p.nchunk = L.nchunk; p.zp = L.zp; p.sd = L.sd; p.blk_bytes = (int)L.blk; p.rsb_stride = L.rsb_stride; p.nrsb = L.nrsb; p.bits = L.bits;
+    p.scale0 = L.scale0;
     if constexpr (std::is_same_v<P, PrefillParams>) p.qch = L.qch;
     else { p.nrt = t.nrt; p.nmain = t.nmain; p.nextra = t.nextra; }
     return p;
@@ -563,7 +574,7 @@ int launch_prefill(const Resident &R, int N, const int8_t *qlut, const float *ls
     else fk.lut<<<dim3(t.nmain, ntile), 128, 0, g.stream()>>>(qlut, ls, lb, (unsigned char *)g.d_tiles.p, N, L.K);
     CUDA_OK(cudaGetLastError());
     auto p = tile_params<PrefillParams>(L, t, N, ldc, out_f16);
-    p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C; p.scale0 = L.scale0;
+    p.W = R.d; p.qlut = qlut; p.lut_scales = ls; p.lut_biases = lb; p.C = C;
     p.lut_tiles = (const unsigned char *)g.d_tiles.p;
     if (g.trace) {
         if (g.d_trace.ensure(8192)) return fail("out of device memory (trace)");
@@ -1273,7 +1284,7 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
 }
 
 // The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm and
-// tmac_b200_prefill_rmsnorm / _glu / _residual): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
+// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
 // and R given are device pointers.
 static int io_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *A, const Gemv3Io &io,
                     void *const *C) {
@@ -1429,7 +1440,7 @@ static int refuse_peer(const std::string &what) {
 // The routed tile launch of the prefill-sized calls, their arguments checked by the caller.  Routed experts (ids != null): route the
 // slots on the device (pf_route_kernel).  The dense forms (ids == null, n_experts = topk = 1): the identity routing, one table entry
 // per token tile.  Then build the LUT of every input row once (B's N rows; U != null: the N * topk rows swiglu(A[s], U[s]); nw != null:
-// the N rows rms_scale(A[n], inv_n, nw), both materialised in fp32), gather each table entry's LUT records and run the routed tile over
+// the N rows rms_scale(A[n], inv_n, nw); both: the RMS norm of the SwiGLU rows, all materialised in fp32), gather each table entry's LUT records and run the routed tile over
 // (row tiles, table entries, count).  wts != null (the GLU experts): the tile stores the slots' fp32 rows and the combine adds them
 // (+ R); otherwise the tile adds R (when not null) in its epilogue.  Everything is checked and every workspace allocated before
 // anything is launched.
@@ -1441,9 +1452,9 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     auto it0 = g.res.find(handles[0]);
     if (it0 == g.res.end()) return fail(what + ": bad weight handle");
     const StreamLayout &L = it0->second.L;
-    if (!tiles_take_fp(L))
-        return fail(what + ": the tiles take W2/W3/W4 fp-path tensors (per-row scales, K % 128 == 0, chunk 128/64/32 K, act group inside "
-                    "the chunk); use " + gemv_name + " for the others");
+    if (!routed_tiles_take(L))
+        return fail(what + ": the tiles take W2/W3/W4 fp-path tensors with the act group inside the chunk: per-row scales with K % 128 "
+                    "== 0 (chunk 128/64/32 K), or one scale with act group < K and K % 128 == 0 or 64; use " + gemv_name + " for the others");
     const int S = N * topk, Mout = L.Mout, K = L.K, f16 = dtype == TMAC_B200_F16;
     // combine: the table's C is the slots' fp32 rows, so the workspace is allocated before the table is built
     if (combine && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
@@ -1451,7 +1462,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     BatchPtrs bp;
     if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : C, &R, &bp, n_experts))
         return -1;
-    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq());
+    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq(), L.one_scale, L.K % 128 != 0);
     if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
     const TilePlan t(L, false);
     // the tile rule: routed experts as experts_take_tile16, the dense forms as the dense calls (launch_prefill)
@@ -1478,7 +1489,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     CUDA_OK(cudaGetLastError());
     if (act) {
         if (U) pf_swiglu_launch(A, U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st);
-        else pf_rmsnorm_launch(A, f16, nw, eps, rows, K, (float *)g.d_moe_act.p, st);
+        if (nw) pf_rmsnorm_launch(U ? g.d_moe_act.p : A, U ? 0 : f16, nw, eps, rows, K, (float *)g.d_moe_act.p, st);   // U: in place
         CUDA_OK(cudaGetLastError());
         if (launch_preprocessor(K, rows, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
     } else if (launch_preprocessor(K, rows, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
@@ -1495,7 +1506,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
         fk.lut<<<dim3(nsteps, (unsigned)cap), 128, 0, st>>>(qlut, ls, lb, recs, K, tiles, perm, div);
         CUDA_OK(cudaGetLastError());
         auto p = tile_params<PrefillParams>(L, t, N, Mout, out_f16);
-        p.lut_tiles = recs;   // qlut, lut_scales, lut_biases and scale0 are read on the integer path only
+        p.lut_tiles = recs;   // qlut, lut_scales and lut_biases are read on the integer path only; scale0 by one-scale tensors
         if (launch_tile(false, fk.tile, grid, t, 1, L, S, p, route)) return -1;
     }
     if (combine) {
@@ -1524,7 +1535,7 @@ int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, 
     return prefill_routed(what, "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, nullptr, 0.f, ids, weights, R, &C);
 }
 
-// tmac_b200_prefill_rmsnorm / _glu / _residual: the arguments and checks of the gemv_* form, the launch of the routed tile as one
+// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm: the arguments and checks of the gemv_* form, the launch of the routed tile as one
 // expert with the identity routing.
 int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                               void *const *C) {
@@ -1552,6 +1563,16 @@ int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, 
     Gemv3Io io;
     if (refuse_peer(what) || residual_check(what, handle, N, dtype, B, R, C, &io)) return -1;
     return prefill_routed(what, "gemv_residual", &handle, 1, 1, N, dtype, 1, B, nullptr, nullptr, 0.f, nullptr, nullptr, R, &C);
+}
+
+int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps, const void *R,
+                              void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_subnorm";
+    Gemv3Io io;
+    if (refuse_peer(what) || rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
+    return prefill_routed(what, "gemv_subnorm", &handle, 1, 1, N, dtype, 1, G, U, w, eps, nullptr, nullptr, R, &C);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

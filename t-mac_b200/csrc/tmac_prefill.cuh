@@ -38,6 +38,10 @@
 //            (32, 32) -- the last is ggml Q4_0 and GPTQ g32.  The producers stage a 128-K window (128 / ck consecutive chunk
 //            blocks, one contiguous run of the stream layout) per two steps, whatever the chunk; or
 //   integer path: one scale, act group = K, chunk = 128 K or 64 K (p.qch at run time; QCH and AGQ are not used).
+// The routed instantiations (ROUTE) also take one-scale fp-path tensors (act group 128, 64 or 32 K < K): their blocks carry no
+// scales (sd == 0), and the fold's weight scale is the tensor's scale0 with no zero point -- the same operations on the same values
+// as a tensor whose per-row scales all equal scale0.  At K % 128 == 0 the chunk is 128 K; at K % 128 == 64 it is 64 K (an odd chunk
+// count is possible), and the producers stage one chunk per unit (UNIT1, QCH 4), as on the integer path.
 // Everything else takes the GEMV kernel once per activation row.
 #pragma once
 #include "tmac_kernels.cuh"
@@ -56,7 +60,7 @@ struct PrefillParams {
     long long *dbg;                // optional trace [role][step][4] (TMAC_ENABLE_TRACE builds)
     int nrsb, bits;                // row super-blocks of the tensor (PB 4: the last row tile may hold only one), bit width
     int qch;                       // quads of 16 K per chunk: 8, or 4 (integer path only)
-    float scale0;                  // integer path: the tensor's one weight scale
+    float scale0;                  // the tensor's one weight scale (integer path; routed tiles: one-scale fp-path tensors)
 };
 #ifdef TMAC_ENABLE_TRACE
 #define PF_TRACE(role, step, k) do { if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && (step) < 32) p.dbg[((role) * 32 + (step)) * 4 + (k)] = clock64(); } while (0)
@@ -290,16 +294,19 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 // ROUTE (routed experts and the dense prefill_* forms, fp path, prefill_experts_kernel): grid = (row tiles, table entries, count);
 // the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the entry is unused, else takes the weights
 // W[i * n_experts + expert] of the pointer table, the records of entry k (lut_tile_gather_kernel) and stores token t's row at row
-// perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one (pf_route_store).
-template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE>
+// perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one (pf_route_store).  A tensor with
+// p.sd == 0 has one scale (see the header).  UNIT1 (ROUTE, QCH 4, one-scale tensors with K % 128 == 64): a staging unit is one
+// 64-K chunk, one step.
+template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE, bool UNIT1 = false>
 __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
     static_assert(!(ROUTE && INT_PATH), "routed experts: fp path only");
+    static_assert(!UNIT1 || (ROUTE && QCH == 4), "one-chunk staging: routed 64-K chunks only");
     using G = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
     constexpr int REC = pf_rec_bytes(INT_PATH, QCH, AGQ);
-    constexpr int WB = INT_PATH ? 1 : G::WB;                               // chunk blocks per staging unit
+    constexpr int WB = (INT_PATH || UNIT1) ? 1 : G::WB;                    // chunk blocks per staging unit
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char *sA = smem;                                              // [S][16 KB]
     unsigned char *sR = sA + kPfStages * kPfStageBytes;                    // [S][REC] B tile (+ lut scales + lut biases)
@@ -327,7 +334,7 @@ __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRou
     __syncthreads();
     // first super-block of the row tile
     const unsigned char *rsb_base = (ROUTE ? route.W[blockIdx.z * route.n_experts + ent.x] : p.W) + (size_t)rt * NSB * p.rsb_stride;
-    const int spc = INT_PATH ? p.qch >> 2 : 2;       // steps (64 K) per staging unit
+    const int spc = INT_PATH ? p.qch >> 2 : UNIT1 ? 1 : 2;   // steps (64 K) per staging unit
     const int nunits = p.nchunk / WB;                // fp path: 128-K windows; integer path: chunks
     const int nsteps = spc * nunits;
 
@@ -389,8 +396,10 @@ __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRou
         // PB 4: the warpgroup's super-block, row r & 63 in it; zero for the missing second super-block of the last tile.
         const unsigned char *wg_base = rsb_base + (size_t)(PB == 4 ? wg : 0) * p.rsb_stride;
         const bool live = PB == 2 || rt * NSB + wg < p.nrsb;
+        // one-scale tensors (routed tiles): scale0, and nothing is read at pf_scale_off (their blocks are codes only)
+        const bool one = ROUTE && (UNIT1 || p.sd == 0);
         auto ld_s = [&](int c, int r) {
-            return live ? 0.5f * load_scale(wg_base + (size_t)c * p.blk_bytes + pf_scale_off(QCH), p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
+            return live ? 0.5f * (one ? p.scale0 : load_scale(wg_base + (size_t)c * p.blk_bytes + pf_scale_off(QCH), p.sd, PB == 2 ? r : r & (RSB - 1))) : 0.f;
         };
         auto ld_z = [&](int c, int r) {
             return (p.zp && live) ? load_scale(wg_base + (size_t)c * p.blk_bytes + pf_scale_off(QCH) + (size_t)RSB * p.sd, p.sd, PB == 2 ? r : r & (RSB - 1)) : 0.f;
@@ -536,9 +545,9 @@ template <int PB, bool INT_PATH, int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillParams p) {
     prefill_body<PB, INT_PATH, QCH, AGQ, false>(p, PfRoute{});
 }
-template <int PB, int QCH, int AGQ>
+template <int PB, int QCH, int AGQ, bool UNIT1 = false>
 __global__ void __launch_bounds__(kPfThreads2, 1) prefill_experts_kernel(const PrefillParams p, const PfRoute route) {
-    prefill_body<PB, false, QCH, AGQ, true>(p, route);
+    prefill_body<PB, false, QCH, AGQ, true, UNIT1>(p, route);
 }
 
 }  // namespace tmac_b200

@@ -19,7 +19,8 @@
 //                     step's 64 KB B tile as one bulk copy (TMA).
 // Supported: W2 (PB 2) and W3/W4 (PB 4: a 128-row tile is two 64-row super-blocks), K % 128 == 0, the int8 tile's fp-path
 // groupings (chunk ck = 128, 64 or 32 K: QCH 8, 4, 2; act group ags = 128, 64 or 32 K <= ck: AGQ 8, 4, 2), per-row scales
-// (+ zero points), symmetric LUT.  The producers take their row, 128-K window staging, code decode, PB 4 table, grouping constants
+// (+ zero points), symmetric LUT; routed instantiations of their own (ONE) also one-scale tensors at K % 128 == 0 (blocks without
+// scales, hs = fp16(0.5 * scale0), no zero point; tmac_prefill.cuh).  The producers take their row, 128-K window staging, code decode, PB 4 table, grouping constants
 // and scale offset from the int8 tile's shared code (tmac_prefill.cuh: PF_PRODUCER_ROW, PF_STAGE_BLOCKS, row_codes, pf_build_xtab,
 // PfGroups, pf_scale_off); the expansion into fp16 A entries is this tile's own.  Each stream-K fragment is staged as one run.
 #pragma once
@@ -47,6 +48,7 @@ struct Prefill16Params {
     int nrt, bits;                                   // row tiles of 128 rows (PB 2: nrsb, PB 4: ceil(nrsb / 2)), bit width
     float *scratch;                                  // [2][grid][256 tokens][128 rows] fp32 partial tiles (stream-K): published parts, finishers' own parts
     int *flags;                                      // [grid] partial tile ready
+    float scale0;                                    // ROUTE, sd == 0: the one-scale tensor's weight scale
 };
 
 #define WG_D128(T, d) WG_D64(T, d), WG_D8(T, d, 64), WG_D8(T, d, 72), WG_D8(T, d, 80), WG_D8(T, d, 88), WG_D8(T, d, 96), WG_D8(T, d, 104), \
@@ -158,10 +160,13 @@ __global__ void __launch_bounds__(256) lut_tile16_gather_kernel(const int8_t *ql
 // ROUTE (routed experts and the dense prefill_* forms, prefill16_experts_kernel): grid = (row tiles, table entries, count), no
 // stream-K.  As in the int8 tile (prefill_body): the CTA of entry k = blockIdx.y and tensor i = blockIdx.z exits at once when the
 // entry is unused, else runs tile k * nrt + blockIdx.x on the weights W[i * n_experts + expert], the B tiles of entry k, and stores
-// token t's row at row perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one.
-template <int PB, int QCH, int AGQ, bool ROUTE>
+// token t's row at row perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one.  ONE (ROUTE, QCH 8): a
+// one-scale tensor, whose blocks carry no scales: hs = fp16(0.5 * scale0), no zero point.  A template parameter rather than a test of
+// p.sd: the run-time test made the producers of the per-row-scale instantiations slower.
+template <int PB, int QCH, int AGQ, bool ROUTE, bool ONE = false>
 __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
+    static_assert(!ONE || (ROUTE && QCH == 8), "one-scale tensors: routed, 128-K chunks");
     using PG = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
@@ -210,6 +215,7 @@ __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const P
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");           // registers go to the consumers' accumulators
         PF_PRODUCER_ROW(PB, tid - kP16ConsWarps * 32);
         const int srow = wl * (8 / PB) + wi;         // row within the super-block = scale index
+        constexpr bool one = ONE;                    // a one-scale tensor: scale0, nothing read at pf_scale_off
         int it = 0;                                  // running step counter over both fragments
         auto stage_in = [&](int f, int u) {          // wait for a free stage, request its B tile; returns the A tile
             const int s = it % kP16NA;
@@ -243,7 +249,7 @@ __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const P
                     // (plane 0) plus +-2hs at entry j1 (plane 1), built in registers: (+-hs) + (+-2hs) is one fp16 rounding of the
                     // exact k * hs.  A step holds the groups of NCS chunks: their hs, c1 = hs, c2 = 2hs (ck 128: once per window).
                     auto hs_of = [&](int b) {
-                        return __float2half_rn(live ? 0.5f * load_scale(blk + (size_t)b * p.blk_bytes + pf_scale_off(QCH), p.sd, srow) : 0.f);
+                        return __float2half_rn(live ? 0.5f * (one ? p.scale0 : load_scale(blk + (size_t)b * p.blk_bytes + pf_scale_off(QCH), p.sd, srow)) : 0.f);
                     };
                     __half hsv[PG::NCS];
                     uint32_t c1[PG::NCS], c2[PG::NCS];
@@ -308,7 +314,7 @@ __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const P
                         float hs = 0.f, zz = 0.f;
                         if (live && wg < p.nchunk) {
                             const unsigned char *sp = sb_base + (size_t)wg * p.blk_bytes + pf_scale_off(QCH);
-                            hs = 0.5f * load_scale(sp, p.sd, srow);
+                            hs = 0.5f * (one ? p.scale0 : load_scale(sp, p.sd, srow));
                             if (p.zp) zz = load_scale(sp + (size_t)RSB * p.sd, p.sd, srow);
                         }
                         const __half2 a = __floats2half2_rn(hs, hs), b = __floats2half2_rn(zz, zz);
@@ -425,13 +431,14 @@ template <int PB, int QCH = 8, int AGQ = 4>
 __global__ void __launch_bounds__(kP16Threads, 1) prefill16_kernel(const Prefill16Params p) {
     prefill16_body<PB, QCH, AGQ, false>(p, PfRoute{});
 }
-template <int PB, int QCH, int AGQ>
+template <int PB, int QCH, int AGQ, bool ONE = false>
 __global__ void __launch_bounds__(kP16Threads, 1) prefill16_experts_kernel(const Prefill16Params p, const PfRoute route) {
-    prefill16_body<PB, QCH, AGQ, true>(p, route);
+    prefill16_body<PB, QCH, AGQ, true, ONE>(p, route);
 }
 
 // The routed launches (tmac_b200_prefill_experts / _glu, and the dense tmac_b200_prefill_rmsnorm / _glu / _residual as one expert):
-// the kernels of one tensor kind (PB) and fp grouping, instantiated in tmac_prefill_experts.cu.  route sorts the slots by expert
+// the kernels of one tensor kind (PB) and fp grouping, instantiated in tmac_prefill_experts.cu (one: a one-scale tensor, whose fp16
+// tile is its own instantiation; unit1: the int8 tile alone, staging one 64-K chunk per unit, for one-scale tensors with K % 128 == 64).  route sorts the slots by expert
 // (or writes the identity routing) and the tile table; swiglu and rmsnorm materialise the GLU and norm inputs; combine adds the
 // GLU experts' slot rows.
 struct PfExpertKernels {
@@ -440,7 +447,7 @@ struct PfExpertKernels {
     void (*tile16)(const Prefill16Params, const PfRoute);
     void (*lut16)(const int8_t *, const float *, const float *, unsigned char *, int, int, int, const int4 *, const int *, int);
 };
-PfExpertKernels pick_pf_experts(int pb, int qch, int agq);
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1);
 void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
                      int out_f16, cudaStream_t st);
 void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st);

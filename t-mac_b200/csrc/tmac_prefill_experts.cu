@@ -1,7 +1,8 @@
 // tmac_prefill_experts.cu -- the routed launches at prefill sizes: the routed experts (tmac_b200_prefill_experts / _glu) and the
 // dense transformed-input forms (tmac_b200_prefill_rmsnorm / _glu / _residual), which run as one expert with the identity routing.
 // The routing kernel that groups the slots by expert, the routed instantiations of both wgmma tiles and their gathered LUT records
-// (3 bit widths x 6 fp groupings; tmac_prefill.cuh, tmac_prefill16.cuh), the RMSNorm and GLU inputs and the GLU combine.  In their
+// (3 bit widths x 6 fp groupings, plus for one-scale tensors the fp16 tile's 128-K-chunk groupings and the int8 tile's 64-K chunk
+// units; tmac_prefill.cuh, tmac_prefill16.cuh), the RMSNorm, GLU and sub-norm inputs and the GLU combine.  In their
 // own translation unit so that they compile in parallel with tmac_b200.cu.
 #include "tmac_prefill16.cuh"
 
@@ -76,7 +77,8 @@ __global__ void __launch_bounds__(256) pf_swiglu_kernel(const T *g, const T *u, 
 
 // a[n][k] = rms_scale(h[n][k], inv_n, w[k]), fp16 inputs widened first: the input the GEMV's norm kind (kInNorm) builds its LUT from.
 // One CTA per row: warp 0 sums the squares in the order rms_sumsq / rms_warp_sum document (lane l: the 4-element groups l, l + 32,
-// ...), then every thread scales its elements.  K % 4 == 0.
+// ...), then every thread scales its elements.  K % 4 == 0.  In place (fp32, h == a) is allowed: a thread writes only elements it has
+// just read, after the sum.
 template <typename T>
 __global__ void __launch_bounds__(256) pf_rmsnorm_kernel(const T *h, const float *w, float eps, int K, float *a) {
     __shared__ float inv;
@@ -114,18 +116,27 @@ __global__ void __launch_bounds__(256) pf_combine_kernel(const float *ys, const 
     store_out(C, i, acc, out_f16);
 }
 
-template <int PB> PfExpertKernels pick_pf_experts_pb(int qch, int agq) {
-    return FpGroupings::find<PfExpertKernels>(qch, agq, [](auto QCH, auto AGQ) -> PfExpertKernels {
+template <int PB> PfExpertKernels pick_pf_experts_pb(int qch, int agq, bool one, bool unit1) {
+    if (unit1) {                                 // one-scale, K % 128 == 64: 64-K chunks staged one per unit, the int8 tile only
+        if (qch == 4 && agq == 4) return {prefill_experts_kernel<PB, 4, 4, true>, lut_tile_gather_kernel<4, 4>, nullptr, nullptr};
+        if (qch == 4 && agq == 2) return {prefill_experts_kernel<PB, 4, 2, true>, lut_tile_gather_kernel<4, 2>, nullptr, nullptr};
+        return PfExpertKernels{};
+    }
+    PfExpertKernels k = FpGroupings::find<PfExpertKernels>(qch, agq, [](auto QCH, auto AGQ) -> PfExpertKernels {
         return {prefill_experts_kernel<PB, QCH, AGQ>, lut_tile_gather_kernel<QCH, AGQ>, prefill16_experts_kernel<PB, QCH, AGQ>,
                 lut_tile16_gather_kernel<QCH, AGQ>};
     });
+    if (one)                                     // one-scale, K % 128 == 0: chunk 128 K, the fp16 tile's own instantiations
+        k.tile16 = qch != 8 ? nullptr : agq == 8 ? prefill16_experts_kernel<PB, 8, 8, true> : agq == 4 ? prefill16_experts_kernel<PB, 8, 4, true>
+                 : agq == 2 ? prefill16_experts_kernel<PB, 8, 2, true> : nullptr;
+    return k;
 }
 
 }  // namespace
 
-PfExpertKernels pick_pf_experts(int pb, int qch, int agq) {
-    if (pb == 4) return pick_pf_experts_pb<4>(qch, agq);
-    if (pb == 2) return pick_pf_experts_pb<2>(qch, agq);
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1) {
+    if (pb == 4) return pick_pf_experts_pb<4>(qch, agq, one, unit1);
+    if (pb == 2) return pick_pf_experts_pb<2>(qch, agq, one, unit1);
     return PfExpertKernels{};
 }
 

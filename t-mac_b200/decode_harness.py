@@ -88,8 +88,8 @@ class DecodeLayer:
         fused_ops the linears still run as four launches: gemv_rmsnorm([q, k, v], x, norm1), gemv_subnorm(o, att, w_as, R=x) -> h,
         gemv_rmsnorm([gate, up], h, norm2), gemv_subnorm(down, gate, w_fs, U=up, R=h).
         The prompt step (`prompt`) runs the fused_ops launches in their prefill forms (prefill_rmsnorm, prefill_residual,
-        prefill_glu, prefill_experts, prefill_experts_glu); the sequences are decode-only, and the prefill tiles take no one-scale
-        tensor, so sequence and sub_norms layers run per-linear calls."""
+        prefill_glu, prefill_subnorm, prefill_experts, prefill_experts_glu); the sequences are decode-only, so sequence layers run
+        per-linear calls."""
         import torch
         if ffn_sequence and post_attn_sequence:
             raise ValueError("ffn_sequence and post_attn_sequence are alternatives: the second one contains the FFN")
@@ -276,12 +276,13 @@ class DecodeLayer:
         attention over them; cos / sin [P, hd / 2] are the positions' RoPE angles.  fused_ops layers run their linears as
         prefill_rmsnorm([q, k, v]), prefill_residual(o), prefill_rmsnorm([gate, up]) and prefill_glu(down, R=h); MoE layers as
         prefill_rmsnorm([q, k, v]), prefill_residual(o), the torch router over the P tokens, prefill_experts([gate, up]) and
-        prefill_experts_glu(down, R=h); the other layers (sub_norms layers too) as one call per linear.  `linear` and `routed` as
-        for forward."""
+        prefill_experts_glu(down, R=h); sub_norms + fused_ops layers as prefill_rmsnorm([q, k, v]), prefill_subnorm(o, att, w_as,
+        R=x), prefill_rmsnorm([gate, up]) and prefill_subnorm(down, gate, w_fs, U=up, R=h); the other layers as one call per linear.
+        `linear` and `routed` as for forward."""
         torch, P = self.torch, x.shape[0]
         b = self.prompt_buffers(P)
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
-        fused = self.fused_ops and not self.sub_norms and linear is None
+        fused = self.fused_ops and linear is None
         if fused:
             tb.prefill_rmsnorm([self.lin[n].wt for n in ("q", "k", "v")], P, x, self.norm1, self.EPS, [b["q"], b["k"], b["v"]])
         else:
@@ -296,6 +297,11 @@ class DecodeLayer:
         b["att"].copy_(att.transpose(0, 1).reshape(P, -1))
         if self.experts:
             return self.moe(x, linear, routed, b, P)
+        if fused and self.sub_norms:
+            tb.prefill_subnorm(self.lin["o"].wt, P, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
+            tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
+            tb.prefill_subnorm(self.lin["down"].wt, P, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
+            return b["out"]                                                                   # down(rmsnorm(silu(gate) * up) * w_fs) + h
         if fused:
             tb.prefill_residual(self.lin["o"].wt, P, b["att"], x, b["h"])                       # h = o(att) + x
             tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])

@@ -44,7 +44,7 @@ EXPORTS = [
     "tmac_b200_find_kcfg", "tmac_b200_clear_kcfg", "tmac_b200_upload_weights", "tmac_b200_upload_plain",
     "tmac_b200_upload_plain_rows", "tmac_b200_debug_encode", "tmac_b200_free_weights", "tmac_b200_clone_weights", "tmac_b200_hint_next_weights",
     "tmac_b200_graph_begin", "tmac_b200_graph_end", "tmac_b200_graph_launch", "tmac_b200_graph_free", "tmac_b200_sync", "tmac_b200_debug_trace", "tmac_b200_debug_last_launch", "tmac_b200_debug_set", "tmac_b200_weights_nbytes", "tmac_b200_preprocessor",
-    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
+    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_prefill_subnorm", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
     "ggml_tmac_init", "ggml_tmac_free", "ggml_tmac_mul_mat_task_init", "ggml_tmac_mul_mat_task_compute",
     "ggml_tmac_set_n_threads", "ggml_tmac_get_type_bits", "ggml_tmac_b200_can_mul_mat",
     "ggml_tmac_b200_mul_mat_get_wsize", "ggml_tmac_b200_get_nbytes", "ggml_tmac_b200_transform_tensor",
@@ -96,6 +96,7 @@ def load() -> C.CDLL:
         "tmac_b200_prefill_experts_glu": (i, [vp, i, i, i, vp, vp, vp, vp, i, vp, vp]),
         "tmac_b200_prefill_rmsnorm": (i, [vp, i, i, i, vp, vp, C.c_float, vp]),
         "tmac_b200_prefill_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_prefill_residual": (i, [i64, i, i, vp, vp, vp]),
+        "tmac_b200_prefill_subnorm": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_gemv": (i, [i64, i, i, vp, vp]), "tmac_b200_cbits": (i, [i64, i, vp, vp]),
         "qgemm_lut_int8": (i, [i, i, i, i, vp, vp, vp, vp, vp, vp]),
         "preprocessor_int8": (i, [i, i, i, i, vp, vp, vp, vp]),
@@ -321,6 +322,12 @@ def prefill_glu(wt: Weights, N, G, U, Cout, R=None, dtype=F32):
 def prefill_residual(wt: Weights, N, B, R, Cout, dtype=F32):
     """gemv_residual's arguments and output, run on the prefill tiles (tmac_b200_prefill_residual)."""
     check(load().tmac_b200_prefill_residual(wt.handle, N, dtype, ptr(B), ptr(R), ptr(Cout)), "tmac_b200_prefill_residual")
+
+
+def prefill_subnorm(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
+    """gemv_subnorm's arguments and output, run on the prefill tiles (tmac_b200_prefill_subnorm)."""
+    check(load().tmac_b200_prefill_subnorm(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
+          "tmac_b200_prefill_subnorm")
 
 
 def gemv(wt: Weights, N, B, Cout, dtype=F32):

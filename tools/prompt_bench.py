@@ -16,7 +16,12 @@ of q/k/v in one launch against three single-tensor launches, over all layers, gr
 (`--moe-layers`, 8 experts, top-2) at P = 64 and 512: the prefill form (prefill_experts, prefill_experts_glu) against the gemv_* forms
 (gemv_experts, gemv_experts_glu).  The card's name, power limit and SM clocks are read in the same run, before and after.
 
+--bitnet: BitNet-3B instead (hidden 3200, FFN 8640, 32 heads, `--layers` 26; ternary one-scale W2 tensors with activation groups of
+64, and the attention and FFN sub-norms) in the same three forms, where prefill is prefill_rmsnorm([q, k, v]), prefill_subnorm(o, + x),
+prefill_rmsnorm([gate, up]), prefill_subnorm(down, + h), and gemv_io their gemv_* forms (gemv_subnorm for prefill_subnorm).
+
     python tools/prompt_bench.py [--layers 32] [--moe-layers 8] [--ps 16,32,64,128,512] [--formats w2zp,w4] [--gemv-max 128]
+    python tools/prompt_bench.py --bitnet [--layers 26] [--ps 16,32,64,128,512] [--gemv-max 128]
 """
 import argparse
 import contextlib
@@ -35,9 +40,11 @@ from decode_harness import DecodeModel          # noqa: E402
 FORMATS = {"w2zp": (2, True), "w4": (4, False)}
 LLAMA = dict(hidden=4096, ffn=11008, heads=32)
 MIXTRAL = dict(hidden=4096, ffn=14336, heads=32, experts=8, topk=2)
+BITNET = dict(hidden=3200, ffn=8640, heads=32, bits=2, zero_point=False, sub_norms=True)
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=32)
+ap.add_argument("--layers", type=int, default=None, help="decoder layers (default 32, BitNet-3B 26)")
+ap.add_argument("--bitnet", action="store_true", help="BitNet-3B's prompt step instead of Llama-2-7B and Mixtral-8x7B")
 ap.add_argument("--moe-layers", type=int, default=8)
 ap.add_argument("--ps", default="16,32,64,128,512")
 ap.add_argument("--moe-ps", default="64,512")
@@ -46,6 +53,8 @@ ap.add_argument("--gemv-max", type=int, default=128)
 ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--rounds", type=int, default=3)
 args = ap.parse_args()
+if args.layers is None:
+    args.layers = 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("prompt_bench.py needs a CUDA device")
@@ -67,7 +76,7 @@ def card():
 def gemv_forms():
     """The harness's prefill_* calls swapped for their gemv_* forms, which take the same arguments."""
     names = {"prefill_rmsnorm": tb.gemv_rmsnorm, "prefill_residual": tb.gemv_residual, "prefill_glu": tb.gemv_glu,
-             "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
+             "prefill_subnorm": tb.gemv_subnorm, "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
     saved = {n: getattr(decode_harness.tb, n) for n in names}
     for n, f in names.items():
         setattr(decode_harness.tb, n, f)
@@ -141,8 +150,11 @@ def prompt_fn(m, P, x, linear=None):
 
 
 def dense_model(fmt, ps):
-    bits, zp = FORMATS[fmt]
-    m = DecodeModel(args.layers, bits=bits, zero_point=zp, ctx=512, fused_ops=True, prompt_len=max(ps), **LLAMA)
+    if fmt == "bitnet":
+        m = DecodeModel(args.layers, ctx=512, fused_ops=True, prompt_len=max(ps), **BITNET)
+    else:
+        bits, zp = FORMATS[fmt]
+        m = DecodeModel(args.layers, bits=bits, zero_point=zp, ctx=512, fused_ops=True, prompt_len=max(ps), **LLAMA)
     try:
         for P in ps:
             x = m.px[:P].contiguous()
@@ -152,6 +164,15 @@ def dense_model(fmt, ps):
                 with gemv_forms():
                     graphs["gemv_io"] = graph(forms["prefill"])
             ms = best(graphs)
+            if fmt == "bitnet":
+                share = library_share(forms["prefill"])
+                print(json.dumps({"model": "bitnet_b1_58_3b", "format": "w2_one_scale_a64", "layers": args.layers, "P": P,
+                                  "ms_per_prompt": {k: round(v, 3) for k, v in ms.items()},
+                                  "prompt_tokens_per_s": {k: round(P * 1e3 / v, 1) for k, v in ms.items()},
+                                  "prefill_linears_share": round(share, 3)}), flush=True)
+                del graphs
+                torch.cuda.synchronize()
+                continue
             # q/k/v of every layer: one grouped launch against three single-tensor launches
             lays = m.layers
             h1 = torch.randn((P, LLAMA["hidden"]), device="cuda")
@@ -194,9 +215,12 @@ def moe_model(fmt, ps):
 
 
 print(json.dumps({"card": card()}), flush=True)
-for fmt in args.formats.split(","):
-    dense_model(fmt, [int(p) for p in args.ps.split(",")])
-for fmt in args.formats.split(","):
-    if args.moe_layers:
-        moe_model(fmt, [int(p) for p in args.moe_ps.split(",")])
+if args.bitnet:
+    dense_model("bitnet", [int(p) for p in args.ps.split(",")])
+else:
+    for fmt in args.formats.split(","):
+        dense_model(fmt, [int(p) for p in args.ps.split(",")])
+    for fmt in args.formats.split(","):
+        if args.moe_layers:
+            moe_model(fmt, [int(p) for p in args.moe_ps.split(",")])
 print(json.dumps({"card_after": card()}), flush=True)
