@@ -172,7 +172,8 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
 /* tmac_b200_gemv_grouped behind an input transform or before a residual add, so that a decoder layer's linears run as four launches
  * with no other ops between them: gemv_rmsnorm(q/k/v, x, w1), gemv_residual(o, att, x) -> h, gemv_rmsnorm(gate/up, h, w2),
  * gemv_glu(down, gate, up, h).  The rules of tmac_b200_gemv_grouped apply: device pointers only, the LUT built inside the launch,
- * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm below are the prompt-sized forms), and
+ * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2 below are the
+ * prompt-sized forms), and
  * an armed tmac_b200_peer_outputs makes the call fail.  fp-path tensors with the
  * activation group inside a chunk only.  The transform is applied in fp32 (fp16 inputs widened first) to give the input a, whose
  * LUT is built as for any input.  Each call gives exactly tmac_b200_gemv_grouped(handles, count, N, F32, a, C32) with a
@@ -189,6 +190,11 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
  *                 X = swiglu(G, U) when U != NULL (ffn_sub_norm before ffn_down).  a[n][k] = fmul_rn(fmul_rn(X[n][k], inv_n), w[k]),
  *                 X[n][k] in fp32 (swiglu rounded as for seq_add_gemv_glu), inv_n and its sum of squares of X as for gemv_rmsnorm.
  *                 G, U [N][K], R and C [N][Mout]; w and eps as for gemv_rmsnorm.
+ *   gemv_subnorm_relu2: gemv_subnorm's ffn_sub_norm for a squared-ReLU FFN (BitNet b1.58 2B4T, HF hidden_act "relu2"):
+ *                 gemv_subnorm_relu2(down, gate, up, w_fs, h).  The arguments, rules and output of gemv_subnorm with U != NULL, but
+ *                 X[n][k] = fmul_rn(fmul_rn(r, r), U[n][k]) with r = G[n][k] when G[n][k] > 0 or is NaN (torch's relu), else +0.
+ *                 U must not be NULL (gemv_subnorm is the attn sub-norm's call).  Decode sequences (seq_add_gemv_glu) and the routed
+ *                 experts' GLU forms stay SiLU-only.
  * R may equal C (each element is read and written by the same thread). */
 TMAC_B200_API int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                                          void *const *C);
@@ -196,14 +202,16 @@ TMAC_B200_API int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const voi
 TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                          const void *R, void *C);
+TMAC_B200_API int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                               const void *R, void *C);
 /* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm / gemv_glu /
- * gemv_residual / gemv_subnorm, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
+ * gemv_residual / gemv_subnorm / gemv_subnorm_relu2, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
  * which stream each tensor once per 128 or 256 tokens instead of once per token.  They are the routed-expert tiles of
  * tmac_b200_prefill_experts run as one expert with the identity routing, written on the device: no host sync, graph-capturable.
  *   Input.  The call builds the input a in fp32 exactly as the gemv_* form does (fp16 inputs widened first): prefill_rmsnorm
  *           a[n][k] = fmul_rn(fmul_rn(H[n][k], inv_n), w[k]) with inv_n and its sum of squares in the order of seq_add_gemv_rmsnorm,
  *           prefill_glu a = swiglu(G, U), prefill_residual a = B, prefill_subnorm the a of gemv_subnorm (X = G or swiglu(G, U) in
- *           fp32, then its RMS norm in the order of gemv_rmsnorm).  The preprocessor builds the LUT of each of the N rows once, and all
+ *           fp32, then its RMS norm in the order of gemv_rmsnorm), prefill_subnorm_relu2 the a of gemv_subnorm_relu2.  The preprocessor builds the LUT of each of the N rows once, and all
  *           count tensors share it.
  *   Per-row equality.  For every tensor i, row n of C[i] equals, bit for bit, row n of tmac_b200_gemv(handles[i], N, F32, a) on the
  *           same tile kind (a one-scale tensor: that call on its twin, the same codes with per-row scales all equal to its scale,
@@ -220,6 +228,8 @@ TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const
  *   prefill_subnorm: C = gemv(handle, a) (+ R when R != NULL), G, U (or NULL) [N][K], R and C [N][Mout]; w and eps as for
  *                    prefill_rmsnorm.  A BitNet b1.58 prompt's linears run as prefill_rmsnorm(q/k/v, x, w1),
  *                    prefill_subnorm(o, att, NULL, w_as, x) -> h, prefill_rmsnorm(gate/up, h, w2), prefill_subnorm(down, gate, up, w_fs, h).
+ *   prefill_subnorm_relu2: prefill_subnorm with gemv_subnorm_relu2's input; U must not be NULL.  A BitNet b1.58 2B4T prompt's down
+ *                    projection: prefill_subnorm_relu2(down, gate, up, w_fs, h).
  * R may equal C.  Tensors: W2/W3/W4 fp-path tensors with the act group inside the chunk: per-row scales with or without zero points,
  * K % 128 == 0, chunk 128/64/32 K; or one scale with act group 128, 64 or 32 K < K and K % 128 == 0 (chunk 128 K) or K % 128 == 64
  * (chunk 64 K, e.g. BitNet-3B's down projection, K = 8640: the int8 tile at every N, whatever the prefill16 knob).  One geometry
@@ -233,6 +243,8 @@ TMAC_B200_API int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const 
 TMAC_B200_API int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
 TMAC_B200_API int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                             const void *R, void *C);
+TMAC_B200_API int tmac_b200_prefill_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w,
+                                                  float eps, const void *R, void *C);
 /* Routed MoE experts: the router's top-k choice stays on the device, so a MoE FFN is two launches with no host sync and the token step
  * stays graph-capturable: gemv_experts([gate, up], h2, ids) -> G, U, then gemv_experts_glu(down, G, U, ids, weights, h) -> y.
  *   gemv_experts:     handles [count][n_experts] (host), entry i * n_experts + e = tensor i of expert e (e.g. i = 0 gate, 1 up).

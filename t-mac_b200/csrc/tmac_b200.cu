@@ -299,6 +299,7 @@ gemv3_fn pick_gemv3(int pb, bool sym, int qch, int agq, int minb, int in) {
         case kInNorm: return pick_gemv3_in<kInNorm>(pb, sym, qch, agq, minb);
         case kInGlu: return pick_gemv3_in<kInGlu>(pb, sym, qch, agq, minb);
         case kInGluNorm: return pick_gemv3_in<kInGluNorm>(pb, sym, qch, agq, minb);
+        case kInRelu2Norm: return pick_gemv3_in<kInRelu2Norm>(pb, sym, qch, agq, minb);
         case kInExperts: return pick_gemv3_in<kInExperts>(pb, sym, qch, agq, minb);
         case kInExpertsGlu: return pick_gemv3_in<kInExpertsGlu>(pb, sym, qch, agq, minb);
         default: return nullptr;
@@ -409,7 +410,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const Gem
     const size_t wregion = std::max((size_t)p.wpc * (p.nbuf * L.blk + (size_t)L.qch * 4 * (sym ? 8 : 16)), (size_t)p.wpc * L.rsb * 4);
     size_t smem = (size_t)p.cs * L.rsb * 4 + ((wregion + 15) & ~(size_t)15) + (size_t)p.wpc * 16;   // + warp-private mbarriers
     if (in.kind != kInTable && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
-    if (in.kind == kInNorm || in.kind == kInGluNorm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
+    if (in.kind == kInNorm || in.kind == kInGluNorm || in.kind == kInRelu2Norm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
     if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t wtx, wty;
     plane_weight_regs(L.bits, sym, &wtx, &wty);
@@ -1283,8 +1284,8 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
     return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kInRow, B, dtype == TMAC_B200_F16), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
-// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm and
-// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
+// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2
+// and tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
 // and R given are device pointers.
 static int io_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *A, const Gemv3Io &io,
                     void *const *C) {
@@ -1296,7 +1297,7 @@ static int io_check(const std::string &what, const int64_t *handles, int count, 
         if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
     return 0;
 }
-// U and R: gemv_subnorm's SwiGLU up rows and residual, or null.
+// U and R: gemv_subnorm's (and gemv_subnorm_relu2's) up rows and residual, or null.
 static int rmsnorm_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
                          float eps, void *const *C, Gemv3Io *io, const void *U = nullptr, const void *R = nullptr) {
     if (!w || ((uintptr_t)w & 15)) return fail(what + ": w must be a 16-byte aligned device vector");
@@ -1319,7 +1320,7 @@ static int residual_check(const std::string &what, int64_t handle, int N, int dt
     return io_check(what, &handle, 1, N, dtype, B, *io, &C);
 }
 
-// tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
+// tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
 // gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.  The arguments are checked.
 static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
                    const Gemv3Io &io, void *const *C) {
@@ -1363,6 +1364,17 @@ int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, cons
     Gemv3Io io;
     if (rmsnorm_check("gemv_subnorm", &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
     return gemv_io("gemv_subnorm", &handle, 1, N, dtype, U ? kInGluNorm : kInNorm, G, io, &C);
+}
+
+int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                 const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "gemv_subnorm_relu2";
+    if (!U) return fail(what + ": U must not be null (gemv_subnorm is the call for the attn sub-norm)");
+    Gemv3Io io;
+    if (rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
+    return gemv_io(what, &handle, 1, N, dtype, kInRelu2Norm, G, io, &C);
 }
 
 // The checks both routed-expert call forms share (tmac_b200_gemv_experts / _glu and tmac_b200_prefill_experts / _glu): the
@@ -1439,14 +1451,15 @@ static int refuse_peer(const std::string &what) {
 
 // The routed tile launch of the prefill-sized calls, their arguments checked by the caller.  Routed experts (ids != null): route the
 // slots on the device (pf_route_kernel).  The dense forms (ids == null, n_experts = topk = 1): the identity routing, one table entry
-// per token tile.  Then build the LUT of every input row once (B's N rows; U != null: the N * topk rows swiglu(A[s], U[s]); nw != null:
+// per token tile.  Then build the LUT of every input row once (B's N rows; U != null: the N * topk rows swiglu(A[s], U[s]), or
+// relu2(A[s], U[s]) when relu2; nw != null:
 // the N rows rms_scale(A[n], inv_n, nw); both: the RMS norm of the SwiGLU rows, all materialised in fp32), gather each table entry's LUT records and run the routed tile over
 // (row tiles, table entries, count).  wts != null (the GLU experts): the tile stores the slots' fp32 rows and the combine adds them
 // (+ R); otherwise the tile adds R (when not null) in its epilogue.  Everything is checked and every workspace allocated before
 // anything is launched.
 static int prefill_routed(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
                           int N, int dtype, int topk, const void *A, const void *U, const float *nw, float eps, const int32_t *ids,
-                          const float *wts, const void *Rres, void *const *C) {
+                          const float *wts, const void *Rres, void *const *C, bool relu2 = false) {
     const bool combine = wts != nullptr, slot_rows = U != nullptr;   // slot_rows: one input row per slot (GLU), else per token
     if (n_experts > 256) return fail(what + ": n_experts must be 1..256");   // the routing kernel's shared arrays
     auto it0 = g.res.find(handles[0]);
@@ -1488,7 +1501,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     pf_route_launch(ids, S, n_experts, T, (int)cap, tiles, perm, ids && !combine ? bp.C : nullptr, count, Mout, f16, st);
     CUDA_OK(cudaGetLastError());
     if (act) {
-        if (U) pf_swiglu_launch(A, U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st);
+        if (U) pf_swiglu_launch(A, U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st, relu2);
         if (nw) pf_rmsnorm_launch(U ? g.d_moe_act.p : A, U ? 0 : f16, nw, eps, rows, K, (float *)g.d_moe_act.p, st);   // U: in place
         CUDA_OK(cudaGetLastError());
         if (launch_preprocessor(K, rows, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
@@ -1535,7 +1548,7 @@ int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, 
     return prefill_routed(what, "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, nullptr, 0.f, ids, weights, R, &C);
 }
 
-// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm: the arguments and checks of the gemv_* form, the launch of the routed tile as one
+// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2: the arguments and checks of the gemv_* form, the launch of the routed tile as one
 // expert with the identity routing.
 int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                               void *const *C) {
@@ -1573,6 +1586,18 @@ int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, c
     Gemv3Io io;
     if (refuse_peer(what) || rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
     return prefill_routed(what, "gemv_subnorm", &handle, 1, 1, N, dtype, 1, G, U, w, eps, nullptr, nullptr, R, &C);
+}
+
+int tmac_b200_prefill_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                    const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_subnorm_relu2";
+    Gemv3Io io;
+    if (refuse_peer(what)) return -1;
+    if (!U) return fail(what + ": U must not be null (prefill_subnorm is the call for the attn sub-norm)");
+    if (rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
+    return prefill_routed(what, "gemv_subnorm_relu2", &handle, 1, 1, N, dtype, 1, G, U, w, eps, nullptr, nullptr, R, &C, true);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

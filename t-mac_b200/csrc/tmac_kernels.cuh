@@ -359,6 +359,13 @@ __device__ __forceinline__ float lut_slice(float x0, float x1, float x2, float x
 // projections): fp32 with exactly this rounding -- expf, not __expf (the build has no fast-math) -- so that the op equals a plain
 // op fed with the vector of these values.  Its LUT is then built with lut_slice / lut_record like any input.
 __device__ __forceinline__ float swiglu(float g, float u) { return __fmul_rn(__fdiv_rn(g, __fadd_rn(1.0f, expf(-g))), u); }
+// The gated activation of a squared-ReLU FFN (BitNet b1.58 2B4T, HF hidden_act "relu2"), relu(g)^2 * u, in fp32 with exactly this
+// rounding: r = g when g > 0 or g is NaN (torch's relu propagates NaN), else +0; then (r * r) * u.  The GEMV's kInRelu2Norm and the
+// prompt form's pf_swiglu_kernel<T, true> both call it, so the two forms build the same input.
+__device__ __forceinline__ float relu2(float g, float u) {
+    const float r = (g > 0.f || isnan(g)) ? g : 0.f;
+    return __fmul_rn(__fmul_rn(r, r), u);
+}
 
 // The RMS norm of a producer's whole output row h[0, K) as the input of a sequence op: a[k] = (h[k] * inv) * w[k] with
 // inv = 1 / sqrt(ss / K + eps).  The sum of squares ss has one order, so that every consumer (a warp of chain_kernel, a CTA of
@@ -507,15 +514,16 @@ struct Gemv3Params {
 // kind builds the LUT from activation rows p.act (the plain row, the norm's h, the GLU's g) with a symmetric table.
 // The routed-expert kinds (kInExperts, kInExpertsGlu) pick each slot's tensor on the device: slot z = i * topk + j of token n
 // (blockIdx.z, blockIdx.y) runs pointer-table entry i * n_experts + ids[n * topk + j].
-// kInGluNorm is the RMS norm of the SwiGLU row (BitNet's ffn_sub_norm before the down projection).
-enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5, kInGluNorm = 6 };
+// kInGluNorm is the RMS norm of the SwiGLU row (BitNet's ffn_sub_norm before the down projection); kInRelu2Norm the RMS norm of
+// the squared-ReLU row (the same sub-norm in BitNet b1.58 2B4T, whose FFN gate is relu2).
+enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5, kInGluNorm = 6, kInRelu2Norm = 7 };
 // The input transform and residual of the row kinds: the kernel's last parameter, so that Gemv3Params, wtx and wty keep their
 // parameter offsets.
 struct Gemv3Io {
-    const void *act2;              // kInGlu, kInGluNorm, kInExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
-    const float *nw;               // kInNorm, kInGluNorm: the norm weight w [K] (16-byte aligned)
-    float eps;                     // kInNorm, kInGluNorm
-    const void *res;               // fp path, kInRow / kInNorm / kInGlu / kInGluNorm / kInExpertsGlu: residual r [N][ldc] of the output's dtype,
+    const void *act2;              // kInGlu, kInGluNorm, kInRelu2Norm, kInExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
+    const float *nw;               // kInNorm, kInGluNorm, kInRelu2Norm: the norm weight w [K] (16-byte aligned)
+    float eps;                     // kInNorm, kInGluNorm, kInRelu2Norm
+    const void *res;               // fp path, kInRow / kInNorm / kInGlu / kInGluNorm / kInRelu2Norm / kInExpertsGlu: residual r [N][ldc] of the output's dtype,
                                    // or null; may equal C
     const int32_t *ids;            // experts: [N][topk], written by earlier work in the stream (read after the dependency wait)
     const float *wts;              // kInExpertsGlu: combine weights [N][topk]
@@ -634,8 +642,8 @@ constexpr int kG3MaxWarps = 8;
 // the row's LUT bias in the reference's order (addv tree per 32 activations, serial over the blocks).
 // The LUT input of row n is the row itself (kInRow) or a transform of the activation rows -- kInNorm a[k] = rms_scale(h[k], inv_n,
 // w[k]), kInGlu a[k] = swiglu(g[k], u[k]), kInGluNorm a[k] = rms_scale(s[k], inv_n, w[k]) with s[k] = swiglu(g[k], u[k]) and inv_n
-// from the sum of squares of s -- built into the chunk's slice with lut_slice as a plain input; on the fp path the leader adds io.res
-// (when not null) to the row sums before the store.
+// from the sum of squares of s, kInRelu2Norm the same with s[k] = relu2(g[k], u[k]) -- built into the chunk's slice with lut_slice as
+// a plain input; on the fp path the leader adds io.res (when not null) to the row sums before the store.
 // Routed experts: slot z = i * topk + j of token n takes its tensor from the pointer table at
 // i * n_experts + ids[n][j], read after the dependency wait, so the slot's first block request waits for it too.  kInExperts reads row
 // n and stores row n * topk + j of C[i]; kInExpertsGlu reads row n * topk + j of g and u, stores its rows into io.ws and counts
@@ -815,11 +823,11 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             if (lane == 0) *bias_out = bias;       // forwarded to the leader with the partial sums below
         }
     }
-    float inv = 0.f;                              // kInNorm, kInGluNorm: 1 / rms of the row
-    if (IN == kInNorm || IN == kInGluNorm) {
-        // Every CTA computes inv itself.  All threads stage the row (kInGluNorm: its swiglu of the row of g and the row of u),
-        // widened to fp32, in shared memory (iscr [K] | inv), with their loads in flight together; warp 0 then sums its squares
-        // in the order of rms_sumsq / rms_warp_sum.
+    float inv = 0.f;                              // kInNorm, kInGluNorm, kInRelu2Norm: 1 / rms of the row
+    if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm) {
+        // Every CTA computes inv itself.  All threads stage the row (kInGluNorm / kInRelu2Norm: its swiglu / relu2 of the row of g
+        // and the row of u), widened to fp32, in shared memory (iscr [K] | inv), with their loads in flight together; warp 0 then
+        // sums its squares in the order of rms_sumsq / rms_warp_sum.
         const int ngrp = p.K >> 2, nth = WPC * 32;
         float4 *hrow = reinterpret_cast<float4 *>(iscr);
         for (int g0 = tid; g0 < ngrp; g0 += 4 * nth) {
@@ -827,7 +835,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 #pragma unroll
             for (int j = 0; j < 4; ++j)
                 if (g0 + j * nth < ngrp) load_group((size_t)(g0 + j * nth) * 4, b[j]);
-            if (IN == kInGluNorm) {
+            if (IN == kInGluNorm || IN == kInRelu2Norm) {
+                const auto act = [](float g, float u) { return IN == kInRelu2Norm ? relu2(g, u) : swiglu(g, u); };
                 float4 u[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j)
@@ -835,7 +844,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 #pragma unroll
                 for (int j = 0; j < 4; ++j)
                     if (g0 + j * nth < ngrp)
-                        b[j] = make_float4(swiglu(b[j].x, u[j].x), swiglu(b[j].y, u[j].y), swiglu(b[j].z, u[j].z), swiglu(b[j].w, u[j].w));
+                        b[j] = make_float4(act(b[j].x, u[j].x), act(b[j].y, u[j].y), act(b[j].z, u[j].z), act(b[j].w, u[j].w));
             }
 #pragma unroll
             for (int j = 0; j < 4; ++j)
@@ -861,7 +870,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         if (IN != kInTable) {
             constexpr int NG = QCH * 4;            // lane = K-group of the chunk
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (IN == kInNorm || IN == kInGluNorm) {
+            if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm) {
                 if (lane < NG) {
                     const size_t g = (size_t)c * NG + lane;
                     const float4 h = reinterpret_cast<const float4 *>(iscr)[g], w = __ldg(reinterpret_cast<const float4 *>(io.nw) + g);
@@ -1005,8 +1014,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 typedef void (*gemv3_fn)(const Gemv3Params, const uint32_t, const uint32_t, const Gemv3Io);
 // gemv3_kernel<PB, SYM, QCH, AGQ, MINB, IN> for a tensor's (pb, qch, agq), the LUT's symmetry (kInTable; the other kinds are
 // symmetric) and minb; null for a grouping that is not instantiated.  Each kind's kernels are compiled in the one translation unit
-// that instantiates pick_gemv3_in for it, so that the kinds compile in parallel: kInTable in tmac_b200.cu, kInRow, kInNorm, kInGlu
-// and kInGluNorm in tmac_gemv_io.cu, kInExperts and kInExpertsGlu in tmac_gemv_experts.cu.
+// that instantiates pick_gemv3_in for it, so that the kinds compile in parallel: kInTable in tmac_b200.cu, kInRow, kInNorm, kInGlu,
+// kInGluNorm and kInRelu2Norm in tmac_gemv_io.cu, kInExperts and kInExpertsGlu in tmac_gemv_experts.cu.
 template <int IN> gemv3_fn pick_gemv3_in(int pb, bool sym, int qch, int agq, int minb) {
     const auto pick = [&](auto SYM, auto MINB) {
         return with_pb<gemv3_fn>(pb, [&](auto PB) {
@@ -1029,6 +1038,7 @@ extern template gemv3_fn pick_gemv3_in<kInRow>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInNorm>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInGlu>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInGluNorm>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInRelu2Norm>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInExperts>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInExpertsGlu>(int, bool, int, int, int);
 

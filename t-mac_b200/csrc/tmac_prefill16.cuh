@@ -439,7 +439,7 @@ __global__ void __launch_bounds__(kP16Threads, 1) prefill16_experts_kernel(const
 // The routed launches (tmac_b200_prefill_experts / _glu, and the dense tmac_b200_prefill_rmsnorm / _glu / _residual as one expert):
 // the kernels of one tensor kind (PB) and fp grouping, instantiated in tmac_prefill_experts.cu (one: a one-scale tensor, whose fp16
 // tile is its own instantiation; unit1: the int8 tile alone, staging one 64-K chunk per unit, for one-scale tensors with K % 128 == 64).  route sorts the slots by expert
-// (or writes the identity routing) and the tile table; swiglu and rmsnorm materialise the GLU and norm inputs; combine adds the
+// (or writes the identity routing) and the tile table; swiglu (or relu2) and rmsnorm materialise the GLU and norm inputs; combine adds the
 // GLU experts' slot rows.
 struct PfExpertKernels {
     void (*tile)(const PrefillParams, const PfRoute);
@@ -450,7 +450,7 @@ struct PfExpertKernels {
 PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1);
 void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
                      int out_f16, cudaStream_t st);
-void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st);
+void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st, bool relu2 = false);
 void pf_rmsnorm_launch(const void *H, int f16, const float *w, float eps, int N, int K, float *a, cudaStream_t st);
 void pf_combine_launch(const float *ys, const int32_t *ids, const float *w, int topk, int E, const void *R, void *C, int N, int Mout,
                        int out_f16, cudaStream_t st);

@@ -68,11 +68,12 @@ __global__ void __launch_bounds__(kRouteThreads) pf_route_kernel(const int32_t *
     }
 }
 
-// a[i] = swiglu(g[i], u[i]) in fp32, fp16 inputs widened first: the input the GEMV's GLU kinds build their LUT from
-template <typename T>
+// a[i] = swiglu(g[i], u[i]) in fp32, fp16 inputs widened first: the input the GEMV's GLU kinds build their LUT from.  RELU2:
+// a[i] = relu2(g[i], u[i]), the squared-ReLU input of kInRelu2Norm (before pf_rmsnorm_kernel in place).
+template <typename T, bool RELU2 = false>
 __global__ void __launch_bounds__(256) pf_swiglu_kernel(const T *g, const T *u, size_t n, float *a) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        a[i] = swiglu(ld_act(g, i), ld_act(u, i));
+        a[i] = RELU2 ? relu2(ld_act(g, i), ld_act(u, i)) : swiglu(ld_act(g, i), ld_act(u, i));
 }
 
 // a[n][k] = rms_scale(h[n][k], inv_n, w[k]), fp16 inputs widened first: the input the GEMV's norm kind (kInNorm) builds its LUT from.
@@ -145,9 +146,11 @@ void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *til
     pf_route_kernel<<<1, kRouteThreads, 0, st>>>(ids, S, E, T, cap, tiles, perm, Cnan, count, ldc, out_f16);
 }
 
-void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st) {
+void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st, bool relu2) {
     const int grid = (int)std::min<size_t>((n + 255) / 256, 132 * 16);
-    if (f16) pf_swiglu_kernel<__half><<<grid, 256, 0, st>>>((const __half *)G, (const __half *)U, n, a);
+    if (relu2 && f16) pf_swiglu_kernel<__half, true><<<grid, 256, 0, st>>>((const __half *)G, (const __half *)U, n, a);
+    else if (relu2) pf_swiglu_kernel<float, true><<<grid, 256, 0, st>>>((const float *)G, (const float *)U, n, a);
+    else if (f16) pf_swiglu_kernel<__half><<<grid, 256, 0, st>>>((const __half *)G, (const __half *)U, n, a);
     else pf_swiglu_kernel<float><<<grid, 256, 0, st>>>((const float *)G, (const float *)U, n, a);
 }
 

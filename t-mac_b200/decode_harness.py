@@ -9,7 +9,8 @@ layer's FFN (gate, up, SiLU*mul, down) is one decode sequence launch instead (to
 one; with `fused_ops=True` the seven linears run as four library launches whose inputs and outputs take the RMSNorms, the
 SiLU*mul and the residual adds (tools/layer_bench.py times the four); adding `experts=E` makes the FFN a routed MoE of E experts with
 top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them); `sub_norms=True`
-makes the layer BitNet b1.58's, with an RMSNorm before o and one before down (tools/layer_bench.py --bitnet).  `prompt()` is the
+makes the layer BitNet b1.58's, with an RMSNorm before o and one before down (tools/layer_bench.py --bitnet; with `ffn_act="relu2"`
+and `kv_heads` < heads, BitNet b1.58 2B4T's, tools/layer_bench.py --bitnet2b).  `prompt()` is the
 prompt step: P tokens through every layer, with causal attention over cache positions [0, P) and the linears on the prefill tiles
 (tmac_b200_prefill_*; tools/prompt_bench.py times it).
 
@@ -72,7 +73,7 @@ class QLinear:
 class DecodeLayer:
     def __init__(self, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, seed: int, share: Optional["DecodeLayer"] = None, group_size: int = 128,
                  ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
-                 sub_norms: bool = False):
+                 sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None):
         """ffn_sequence: the FFN (gate, up, SiLU*mul, down) runs as ONE decode sequence whose down op reads the gated activation of
         the gate and up ops (tmac_b200_seq_add_gemv_glu) instead of three launches and a torch op.
         post_attn_sequence: the layer after attention runs as ONE decode sequence [o(att) + x, gate(rmsnorm(h) * w2),
@@ -87,6 +88,11 @@ class DecodeLayer:
         o(rmsnorm(att) * w_as) and down(rmsnorm(silu(gate) * up) * w_fs) (HF attn inner_attn_ln and mlp ffn_layernorm).  With
         fused_ops the linears still run as four launches: gemv_rmsnorm([q, k, v], x, norm1), gemv_subnorm(o, att, w_as, R=x) -> h,
         gemv_rmsnorm([gate, up], h, norm2), gemv_subnorm(down, gate, w_fs, U=up, R=h).
+        ffn_act: the FFN gate's activation, "silu" (silu(gate) * up) or, with sub_norms only, "relu2" (relu(gate)^2 * up, BitNet b1.58
+        2B4T's), whose fused down projection is gemv_subnorm_relu2 / prefill_subnorm_relu2.
+        kv_heads (default heads): kv_heads < heads is grouped-query attention -- each KV head serves heads / kv_heads consecutive
+        query heads and the KV cache holds kv_heads heads.  q, k and v are then one stacked tensor "qkv" of hidden + 2 * kv_heads * hd
+        rows (one launch, whose output q / k / v are views of), the usual way to group GQA projections.
         The prompt step (`prompt`) runs the fused_ops launches in their prefill forms (prefill_rmsnorm, prefill_residual,
         prefill_glu, prefill_subnorm, prefill_experts, prefill_experts_glu); the sequences are decode-only, so sequence layers run
         per-linear calls."""
@@ -103,9 +109,19 @@ class DecodeLayer:
             raise ValueError("sub_norms has no sequence op and no routed FFN: it cannot be combined with a sequence or experts")
         if sub_norms and bits != 2:
             raise ValueError("sub_norms layers have ternary weights: bits must be 2")
-        self.fused_ops, self.experts, self.topk, self.sub_norms = fused_ops, experts, topk, sub_norms
+        if ffn_act not in ("silu", "relu2"):
+            raise ValueError("ffn_act must be 'silu' or 'relu2'")
+        if ffn_act == "relu2" and not sub_norms:
+            raise ValueError("ffn_act='relu2' is BitNet b1.58 2B4T's FFN: it needs sub_norms")
+        kv_heads = heads if kv_heads is None else kv_heads
+        if not 1 <= kv_heads <= heads or heads % kv_heads:
+            raise ValueError("kv_heads must divide heads")
+        self.fused_ops, self.experts, self.topk, self.sub_norms, self.ffn_act_name = fused_ops, experts, topk, sub_norms, ffn_act
         self.torch, self.hidden, self.ffn, self.heads, self.hd = torch, hidden, ffn, heads, hidden // heads
-        names = [("q", hidden, hidden), ("k", hidden, hidden), ("v", hidden, hidden), ("o", hidden, hidden)]
+        self.kv_heads, kvd = kv_heads, kv_heads * (hidden // heads)
+        self.qkv_names = ("q", "k", "v") if kv_heads == heads else ("qkv",)
+        names = [("q", hidden, hidden), ("k", hidden, hidden), ("v", hidden, hidden)] if kv_heads == heads else [("qkv", hidden + 2 * kvd, hidden)]
+        names += [("o", hidden, hidden)]
         ffn_names = [("gate", ffn, hidden), ("up", ffn, hidden), ("down", hidden, ffn)]
         names += ffn_names if not experts else [("%s.%d" % (n, e), m, k) for e in range(experts) for n, m, k in ffn_names]
         qkw = dict(zero_point=False, one_scale=True, act_group_size=64) if sub_norms else dict(zero_point=zero_point)
@@ -117,6 +133,7 @@ class DecodeLayer:
         f = lambda n: torch.zeros((1, n), device="cuda")
         self.buf = {"h1": f(hidden), "q": f(hidden), "k": f(hidden), "v": f(hidden), "att": f(hidden), "o": f(hidden), "h2": f(hidden),
                     "gate": f(ffn), "up": f(ffn), "act": f(ffn), "down": f(hidden), "x": f(hidden), "out": f(hidden), "h": f(hidden)}
+        self.qkv_views(self.buf, 1)
         if experts:
             self.router = (0.05 * torch.randn((experts, hidden), generator=g)).cuda()
             self.buf.update(gate=torch.zeros((1, topk, ffn), device="cuda"), up=torch.zeros((1, topk, ffn), device="cuda"),
@@ -155,13 +172,24 @@ class DecodeLayer:
 
     EPS = 1e-5
 
+    def qkv_views(self, b, n):
+        """A GQA layer's buffers of n rows: the stacked output qkv [n][hidden + 2 * kv_dim], and q, k and v as views of it."""
+        if self.qkv_names == ("qkv",):
+            H, kvd = self.hidden, self.kv_heads * self.hd
+            qkv = self.torch.zeros((n, H + 2 * kvd), device="cuda")
+            b.update(qkv=qkv, q=qkv[:, :H], k=qkv[:, H:H + kvd], v=qkv[:, H + kvd:])
+
+    def kv(self, c):
+        """The cache positions c [kv_heads, L, hd] repeated over each KV head's query group: [heads, L, hd]."""
+        return c if self.kv_heads == self.heads else c.repeat_interleave(self.heads // self.kv_heads, dim=0)
+
     @staticmethod
     def rmsnorm(torch, x, w, eps=EPS):
         return x * torch.rsqrt((x * x).mean(dim=-1, keepdim=True) + eps) * w
 
     def rope(self, x, pos_cos, pos_sin):
-        """x [n, hidden], pos_cos / pos_sin [n, hd / 2]: row i rotated by the angles of its position."""
-        t = x.view(x.shape[0], self.heads, self.hd // 2, 2)
+        """x [n, heads * hd] (q) or [n, kv_heads * hd] (k), pos_cos / pos_sin [n, hd / 2]: row i rotated by the angles of its position."""
+        t = x.view(x.shape[0], -1, self.hd // 2, 2)
         a, b = t[..., 0], t[..., 1]
         c, s = pos_cos[:, None, :], pos_sin[:, None, :]
         return self.torch.stack((a * c - b * s, a * s + b * c), dim=-1).reshape(x.shape[0], -1)
@@ -174,21 +202,22 @@ class DecodeLayer:
         b["wts"].copy_(self.torch.softmax(vals, dim=-1))
 
     def forward(self, x, kcache, vcache, pos: int, pos_cos, pos_sin, linear=None, routed=None):
-        """x [1, hidden] fp32 -> [1, hidden].  kcache / vcache [heads, ctx, hd]; `linear(name, inp, out)` overrides the library call
+        """x [1, hidden] fp32 -> [1, hidden].  kcache / vcache [kv_heads, ctx, hd]; `linear(name, inp, out)` overrides the library call
         (the dense fp32 reference layer in the tests).  MoE layers: `routed` = (ids, weights) replaces the router's choice, so that a
         reference can follow the choice of the library path; with `linear` every expert runs densely and the chosen ones are combined."""
         torch, b = self.torch, self.buf
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
         fused = self.fused_ops and linear is None
         if fused:
-            tb.gemv_rmsnorm([self.lin[n].wt for n in ("q", "k", "v")], 1, x, self.norm1, self.EPS, [b["q"], b["k"], b["v"]])
+            tb.gemv_rmsnorm([self.lin[n].wt for n in self.qkv_names], 1, x, self.norm1, self.EPS, [b[n] for n in self.qkv_names])
         else:
             b["h1"].copy_(self.rmsnorm(torch, x, self.norm1))
-            lin("q", b["h1"], b["q"]); lin("k", b["h1"], b["k"]); lin("v", b["h1"], b["v"])
+            for n in self.qkv_names:
+                lin(n, b["h1"], b[n])
         q = self.rope(b["q"], pos_cos, pos_sin).view(self.heads, 1, self.hd)
-        kcache[:, pos] = self.rope(b["k"], pos_cos, pos_sin).view(self.heads, self.hd)
-        vcache[:, pos] = b["v"].view(self.heads, self.hd)
-        att = torch.softmax((q @ kcache[:, :pos + 1].transpose(1, 2)) / math.sqrt(self.hd), dim=-1) @ vcache[:, :pos + 1]
+        kcache[:, pos] = self.rope(b["k"], pos_cos, pos_sin).view(self.kv_heads, self.hd)
+        vcache[:, pos] = b["v"].view(self.kv_heads, self.hd)
+        att = torch.softmax((q @ self.kv(kcache[:, :pos + 1]).transpose(1, 2)) / math.sqrt(self.hd), dim=-1) @ self.kv(vcache[:, :pos + 1])
         b["att"].copy_(att.reshape(1, -1))
         if self.post_seq is not None and linear is None:
             b["x"].copy_(x)
@@ -199,8 +228,9 @@ class DecodeLayer:
         if fused and self.sub_norms:
             tb.gemv_subnorm(self.lin["o"].wt, 1, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
             tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            tb.gemv_subnorm(self.lin["down"].wt, 1, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
-            return b["out"]                                                                   # down(rmsnorm(silu(gate) * up) * w_fs) + h
+            down = tb.gemv_subnorm_relu2 if self.ffn_act_name == "relu2" else tb.gemv_subnorm
+            down(self.lin["down"].wt, 1, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
+            return b["out"]                                                                   # down(rmsnorm(act(gate, up)) * w_fs) + h
         if fused:
             tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])                          # h = o(att) + x
             tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
@@ -225,8 +255,11 @@ class DecodeLayer:
         return b["att_n"]
 
     def ffn_act(self, b):
-        """b["act"] = silu(gate) * up, then rmsnorm(.) * w_fs in a sub_norms layer (torch ops)."""
-        act = self.torch.nn.functional.silu(b["gate"]) * b["up"]
+        """b["act"] = silu(gate) * up (relu2 layers: relu(gate)^2 * up), then rmsnorm(.) * w_fs in a sub_norms layer (torch ops)."""
+        if self.ffn_act_name == "relu2":
+            act = self.torch.square(self.torch.relu(b["gate"])) * b["up"]
+        else:
+            act = self.torch.nn.functional.silu(b["gate"]) * b["up"]
         b["act"].copy_(self.rmsnorm(self.torch, act, self.w_fs) if self.sub_norms else act)
 
     def moe(self, x, linear, routed, b, n):
@@ -266,6 +299,7 @@ class DecodeLayer:
             H, F = self.hidden, self.ffn
             self.pbuf = {"P": P, "h1": f(P, H), "q": f(P, H), "k": f(P, H), "v": f(P, H), "att": f(P, H), "o": f(P, H), "h2": f(P, H),
                          "gate": f(P, F), "up": f(P, F), "act": f(P, F), "down": f(P, H), "out": f(P, H), "h": f(P, H), "att_n": f(P, H)}
+            self.qkv_views(self.pbuf, P)
             if self.experts:
                 self.pbuf.update(gate=f(P, self.topk, F), up=f(P, self.topk, F), wts=f(P, self.topk),
                                  ids=torch.zeros((P, self.topk), dtype=torch.int32, device="cuda"))
@@ -277,31 +311,34 @@ class DecodeLayer:
         prefill_rmsnorm([q, k, v]), prefill_residual(o), prefill_rmsnorm([gate, up]) and prefill_glu(down, R=h); MoE layers as
         prefill_rmsnorm([q, k, v]), prefill_residual(o), the torch router over the P tokens, prefill_experts([gate, up]) and
         prefill_experts_glu(down, R=h); sub_norms + fused_ops layers as prefill_rmsnorm([q, k, v]), prefill_subnorm(o, att, w_as,
-        R=x), prefill_rmsnorm([gate, up]) and prefill_subnorm(down, gate, w_fs, U=up, R=h); the other layers as one call per linear.
+        R=x), prefill_rmsnorm([gate, up]) and prefill_subnorm(down, gate, w_fs, U=up, R=h) (relu2 layers: prefill_subnorm_relu2);
+        GQA layers run [qkv] in place of [q, k, v]; the other layers as one call per linear.
         `linear` and `routed` as for forward."""
         torch, P = self.torch, x.shape[0]
         b = self.prompt_buffers(P)
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
         fused = self.fused_ops and linear is None
         if fused:
-            tb.prefill_rmsnorm([self.lin[n].wt for n in ("q", "k", "v")], P, x, self.norm1, self.EPS, [b["q"], b["k"], b["v"]])
+            tb.prefill_rmsnorm([self.lin[n].wt for n in self.qkv_names], P, x, self.norm1, self.EPS, [b[n] for n in self.qkv_names])
         else:
             b["h1"].copy_(self.rmsnorm(torch, x, self.norm1))
-            lin("q", b["h1"], b["q"]); lin("k", b["h1"], b["k"]); lin("v", b["h1"], b["v"])
+            for n in self.qkv_names:
+                lin(n, b["h1"], b[n])
         q = self.rope(b["q"], cos, sin).view(P, self.heads, self.hd).transpose(0, 1)
-        kcache[:, :P] = self.rope(b["k"], cos, sin).view(P, self.heads, self.hd).transpose(0, 1)
-        vcache[:, :P] = b["v"].view(P, self.heads, self.hd).transpose(0, 1)
-        s = (q @ kcache[:, :P].transpose(1, 2)) / math.sqrt(self.hd)
+        kcache[:, :P] = self.rope(b["k"], cos, sin).view(P, self.kv_heads, self.hd).transpose(0, 1)
+        vcache[:, :P] = b["v"].view(P, self.kv_heads, self.hd).transpose(0, 1)
+        s = (q @ self.kv(kcache[:, :P]).transpose(1, 2)) / math.sqrt(self.hd)
         s = s.masked_fill(torch.ones((P, P), dtype=torch.bool, device="cuda").triu(1), float("-inf"))
-        att = torch.softmax(s, dim=-1) @ vcache[:, :P]                      # [heads][P][hd]
+        att = torch.softmax(s, dim=-1) @ self.kv(vcache[:, :P])             # [heads][P][hd]
         b["att"].copy_(att.transpose(0, 1).reshape(P, -1))
         if self.experts:
             return self.moe(x, linear, routed, b, P)
         if fused and self.sub_norms:
             tb.prefill_subnorm(self.lin["o"].wt, P, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
             tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            tb.prefill_subnorm(self.lin["down"].wt, P, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
-            return b["out"]                                                                   # down(rmsnorm(silu(gate) * up) * w_fs) + h
+            down = tb.prefill_subnorm_relu2 if self.ffn_act_name == "relu2" else tb.prefill_subnorm
+            down(self.lin["down"].wt, P, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
+            return b["out"]                                                                   # down(rmsnorm(act(gate, up)) * w_fs) + h
         if fused:
             tb.prefill_residual(self.lin["o"].wt, P, b["att"], x, b["h"])                       # h = o(att) + x
             tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
@@ -332,16 +369,17 @@ class DecodeModel:
 
     def __init__(self, layers: int, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, ctx: int = 512, seed: int = 0,
                  ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
-                 prompt_len: int = 0, sub_norms: bool = False):
+                 prompt_len: int = 0, sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None):
         import torch
         self.torch, self.hidden, self.ctx, self.heads, self.hd = torch, hidden, ctx, heads, hidden // heads
         kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk,
-                  sub_norms=sub_norms)
+                  sub_norms=sub_norms, ffn_act=ffn_act, kv_heads=kv_heads)
         first = DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, **kw)
         self.layers: List[DecodeLayer] = [first] + [DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, share=first, **kw)
                                                     for _ in range(layers - 1)]
-        self.kc = [torch.randn((heads, ctx, self.hd), device="cuda") * 0.1 for _ in range(layers)]
-        self.vc = [torch.randn((heads, ctx, self.hd), device="cuda") * 0.1 for _ in range(layers)]
+        kvh = first.kv_heads
+        self.kc = [torch.randn((kvh, ctx, self.hd), device="cuda") * 0.1 for _ in range(layers)]
+        self.vc = [torch.randn((kvh, ctx, self.hd), device="cuda") * 0.1 for _ in range(layers)]
         inv = 1.0 / (10000.0 ** (torch.arange(0, self.hd, 2, device="cuda").float() / self.hd))
         self.pos = ctx - 1                          # decode at the last cache position: attention over the whole context
         ang = self.pos * inv

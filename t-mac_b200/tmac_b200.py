@@ -44,7 +44,7 @@ EXPORTS = [
     "tmac_b200_find_kcfg", "tmac_b200_clear_kcfg", "tmac_b200_upload_weights", "tmac_b200_upload_plain",
     "tmac_b200_upload_plain_rows", "tmac_b200_debug_encode", "tmac_b200_free_weights", "tmac_b200_clone_weights", "tmac_b200_hint_next_weights",
     "tmac_b200_graph_begin", "tmac_b200_graph_end", "tmac_b200_graph_launch", "tmac_b200_graph_free", "tmac_b200_sync", "tmac_b200_debug_trace", "tmac_b200_debug_last_launch", "tmac_b200_debug_set", "tmac_b200_weights_nbytes", "tmac_b200_preprocessor",
-    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_prefill_subnorm", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
+    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_subnorm_relu2", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_prefill_subnorm", "tmac_b200_prefill_subnorm_relu2", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
     "ggml_tmac_init", "ggml_tmac_free", "ggml_tmac_mul_mat_task_init", "ggml_tmac_mul_mat_task_compute",
     "ggml_tmac_set_n_threads", "ggml_tmac_get_type_bits", "ggml_tmac_b200_can_mul_mat",
     "ggml_tmac_b200_mul_mat_get_wsize", "ggml_tmac_b200_get_nbytes", "ggml_tmac_b200_transform_tensor",
@@ -90,6 +90,7 @@ def load() -> C.CDLL:
         "tmac_b200_gemv_rmsnorm": (i, [vp, i, i, i, vp, vp, C.c_float, vp]),
         "tmac_b200_gemv_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_gemv_residual": (i, [i64, i, i, vp, vp, vp]),
         "tmac_b200_gemv_subnorm": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
+        "tmac_b200_gemv_subnorm_relu2": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_gemv_experts": (i, [vp, i, i, i, i, vp, vp, i, vp]),
         "tmac_b200_gemv_experts_glu": (i, [vp, i, i, i, vp, vp, vp, vp, i, vp, vp]),
         "tmac_b200_prefill_experts": (i, [vp, i, i, i, i, vp, vp, i, vp]),
@@ -97,6 +98,7 @@ def load() -> C.CDLL:
         "tmac_b200_prefill_rmsnorm": (i, [vp, i, i, i, vp, vp, C.c_float, vp]),
         "tmac_b200_prefill_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_prefill_residual": (i, [i64, i, i, vp, vp, vp]),
         "tmac_b200_prefill_subnorm": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
+        "tmac_b200_prefill_subnorm_relu2": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_gemv": (i, [i64, i, i, vp, vp]), "tmac_b200_cbits": (i, [i64, i, vp, vp]),
         "qgemm_lut_int8": (i, [i, i, i, i, vp, vp, vp, vp, vp, vp]),
         "preprocessor_int8": (i, [i, i, i, i, vp, vp, vp, vp]),
@@ -264,6 +266,13 @@ def gemv_subnorm(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
           "tmac_b200_gemv_subnorm")
 
 
+def gemv_subnorm_relu2(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
+    """Cout = gemv(wt, rmsnorm(relu(G)^2 * U) * w) (+ R): the down projection of a squared-ReLU BitNet FFN (b1.58 2B4T) behind its
+    ffn_sub_norm (tmac_b200_gemv_subnorm_relu2; gemv_subnorm's argument order, U required; device tensors, R may be Cout)."""
+    check(load().tmac_b200_gemv_subnorm_relu2(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
+          "tmac_b200_gemv_subnorm_relu2")
+
+
 def gemv_experts(tables, N, B, ids, outs, dtype=F32):
     """Routed experts: tables[i][e] is tensor i of expert e (e.g. i = 0 gate, 1 up).  outs[i] [N][topk][Mout] gets
     gemv(tables[i][ids[n][j]], B[n]) in row (n, j); ids: device int32 [N][topk], read only on the device."""
@@ -328,6 +337,12 @@ def prefill_subnorm(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
     """gemv_subnorm's arguments and output, run on the prefill tiles (tmac_b200_prefill_subnorm)."""
     check(load().tmac_b200_prefill_subnorm(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
           "tmac_b200_prefill_subnorm")
+
+
+def prefill_subnorm_relu2(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
+    """gemv_subnorm_relu2's arguments and output, run on the prefill tiles (tmac_b200_prefill_subnorm_relu2)."""
+    check(load().tmac_b200_prefill_subnorm_relu2(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
+          "tmac_b200_prefill_subnorm_relu2")
 
 
 def gemv(wt: Weights, N, B, Cout, dtype=F32):

@@ -5,10 +5,12 @@ four launches that take the RMSNorms, the SiLU*mul and the residual adds into th
 resident together and timed alternately, best of `--rounds`; the kernel serving each layer's sequence is recorded beside the time,
 and so are the card's name, power limit and max SM clock.  With `--bitnet` the layers are BitNet-3B's (26 layers, hidden 3200,
 FFN 8640, 32 heads; ternary one-scale tensors with activation groups of 64, and the attn / ffn sub-norms), timed in the modes
-"off" and "fused_ops".
+"off" and "fused_ops".  With `--bitnet2b` they are BitNet b1.58 2B4T's (30 layers, hidden 2560, FFN 6912, 20 query heads and 5 KV
+heads of 128, the squared-ReLU FFN: ffn_act="relu2", kv_heads=5), in the same two modes.
 
     python tools/layer_bench.py [--layers 32] [--reps 20] [--rounds 3] [--formats w2zp,w4]
     python tools/layer_bench.py --bitnet [--layers 26] [...]
+    python tools/layer_bench.py --bitnet2b [--layers 30] [...]
     python tools/layer_bench.py --profile [...]     # kernels per token of each mode (torch.profiler, one eager step; no timing)
 """
 import argparse
@@ -29,20 +31,22 @@ MODES = {"off": {}, "ffn_sequence": {"ffn_sequence": True}, "post_attn_sequence"
          "fused_ops": {"fused_ops": True}}
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=None, help="default 32, 26 with --bitnet")
+ap.add_argument("--layers", type=int, default=None, help="default 32, 26 with --bitnet, 30 with --bitnet2b")
 ap.add_argument("--reps", type=int, default=20)
 ap.add_argument("--rounds", type=int, default=3)
 ap.add_argument("--formats", default="w2zp,w4")
 ap.add_argument("--profile", action="store_true", help="count the kernels of one token step per mode instead of timing")
 ap.add_argument("--bitnet", action="store_true", help="BitNet-3B layers with sub-norms, modes off and fused_ops")
+ap.add_argument("--bitnet2b", action="store_true", help="BitNet b1.58 2B4T layers (relu2 FFN, 5 KV heads), modes off and fused_ops")
 args = ap.parse_args()
-if args.bitnet:
-    HIDDEN, FFN, HEADS = 3200, 8640, 32
-    FORMATS = {"bitnet": (2, False)}
-    MODES = {"off": {"sub_norms": True}, "fused_ops": {"sub_norms": True, "fused_ops": True}}
-    args.formats = "bitnet"
+if args.bitnet or args.bitnet2b:
+    sub = dict(sub_norms=True, ffn_act="relu2", kv_heads=5) if args.bitnet2b else dict(sub_norms=True)
+    HIDDEN, FFN, HEADS = (2560, 6912, 20) if args.bitnet2b else (3200, 8640, 32)
+    args.formats = "bitnet2b" if args.bitnet2b else "bitnet"
+    FORMATS = {args.formats: (2, False)}
+    MODES = {"off": sub, "fused_ops": dict(sub, fused_ops=True)}
 if args.layers is None:
-    args.layers = 26 if args.bitnet else 32
+    args.layers = 30 if args.bitnet2b else 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("layer_bench.py needs a CUDA device")

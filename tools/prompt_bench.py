@@ -21,7 +21,11 @@ of q/k/v in one launch against three single-tensor launches, over all layers, gr
 prefill_rmsnorm([gate, up]), prefill_subnorm(down, + h), and gemv_io their gemv_* forms (gemv_subnorm for prefill_subnorm).
 
     python tools/prompt_bench.py [--layers 32] [--moe-layers 8] [--ps 16,32,64,128,512] [--formats w2zp,w4] [--gemv-max 128]
+--bitnet2b: BitNet b1.58 2B4T instead (hidden 2560, FFN 6912, 20 query heads and 5 KV heads of 128, `--layers` 30, the squared-ReLU
+FFN), in the same three forms: q/k/v are one stacked tensor, and the down projection is prefill_subnorm_relu2 (gemv_subnorm_relu2).
+
     python tools/prompt_bench.py --bitnet [--layers 26] [--ps 16,32,64,128,512] [--gemv-max 128]
+    python tools/prompt_bench.py --bitnet2b [--layers 30] [--ps 16,32,64,128,512] [--gemv-max 128]
 """
 import argparse
 import contextlib
@@ -41,10 +45,12 @@ FORMATS = {"w2zp": (2, True), "w4": (4, False)}
 LLAMA = dict(hidden=4096, ffn=11008, heads=32)
 MIXTRAL = dict(hidden=4096, ffn=14336, heads=32, experts=8, topk=2)
 BITNET = dict(hidden=3200, ffn=8640, heads=32, bits=2, zero_point=False, sub_norms=True)
+BITNET2B = dict(hidden=2560, ffn=6912, heads=20, kv_heads=5, bits=2, zero_point=False, sub_norms=True, ffn_act="relu2")
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=None, help="decoder layers (default 32, BitNet-3B 26)")
+ap.add_argument("--layers", type=int, default=None, help="decoder layers (default 32, BitNet-3B 26, BitNet b1.58 2B4T 30)")
 ap.add_argument("--bitnet", action="store_true", help="BitNet-3B's prompt step instead of Llama-2-7B and Mixtral-8x7B")
+ap.add_argument("--bitnet2b", action="store_true", help="BitNet b1.58 2B4T's prompt step instead of Llama-2-7B and Mixtral-8x7B")
 ap.add_argument("--moe-layers", type=int, default=8)
 ap.add_argument("--ps", default="16,32,64,128,512")
 ap.add_argument("--moe-ps", default="64,512")
@@ -54,7 +60,7 @@ ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--rounds", type=int, default=3)
 args = ap.parse_args()
 if args.layers is None:
-    args.layers = 26 if args.bitnet else 32
+    args.layers = 30 if args.bitnet2b else 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("prompt_bench.py needs a CUDA device")
@@ -76,7 +82,7 @@ def card():
 def gemv_forms():
     """The harness's prefill_* calls swapped for their gemv_* forms, which take the same arguments."""
     names = {"prefill_rmsnorm": tb.gemv_rmsnorm, "prefill_residual": tb.gemv_residual, "prefill_glu": tb.gemv_glu,
-             "prefill_subnorm": tb.gemv_subnorm, "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
+             "prefill_subnorm": tb.gemv_subnorm, "prefill_subnorm_relu2": tb.gemv_subnorm_relu2, "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
     saved = {n: getattr(decode_harness.tb, n) for n in names}
     for n, f in names.items():
         setattr(decode_harness.tb, n, f)
@@ -150,8 +156,8 @@ def prompt_fn(m, P, x, linear=None):
 
 
 def dense_model(fmt, ps):
-    if fmt == "bitnet":
-        m = DecodeModel(args.layers, ctx=512, fused_ops=True, prompt_len=max(ps), **BITNET)
+    if fmt in ("bitnet", "bitnet2b"):
+        m = DecodeModel(args.layers, ctx=512, fused_ops=True, prompt_len=max(ps), **(BITNET2B if fmt == "bitnet2b" else BITNET))
     else:
         bits, zp = FORMATS[fmt]
         m = DecodeModel(args.layers, bits=bits, zero_point=zp, ctx=512, fused_ops=True, prompt_len=max(ps), **LLAMA)
@@ -164,9 +170,9 @@ def dense_model(fmt, ps):
                 with gemv_forms():
                     graphs["gemv_io"] = graph(forms["prefill"])
             ms = best(graphs)
-            if fmt == "bitnet":
+            if fmt in ("bitnet", "bitnet2b"):
                 share = library_share(forms["prefill"])
-                print(json.dumps({"model": "bitnet_b1_58_3b", "format": "w2_one_scale_a64", "layers": args.layers, "P": P,
+                print(json.dumps({"model": "bitnet_b1_58_2b4t" if fmt == "bitnet2b" else "bitnet_b1_58_3b", "format": "w2_one_scale_a64", "layers": args.layers, "P": P,
                                   "ms_per_prompt": {k: round(v, 3) for k, v in ms.items()},
                                   "prompt_tokens_per_s": {k: round(P * 1e3 / v, 1) for k, v in ms.items()},
                                   "prefill_linears_share": round(share, 3)}), flush=True)
@@ -215,8 +221,8 @@ def moe_model(fmt, ps):
 
 
 print(json.dumps({"card": card()}), flush=True)
-if args.bitnet:
-    dense_model("bitnet", [int(p) for p in args.ps.split(",")])
+if args.bitnet or args.bitnet2b:
+    dense_model("bitnet2b" if args.bitnet2b else "bitnet", [int(p) for p in args.ps.split(",")])
 else:
     for fmt in args.formats.split(","):
         dense_model(fmt, [int(p) for p in args.ps.split(",")])
