@@ -172,8 +172,8 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
 /* tmac_b200_gemv_grouped behind an input transform or before a residual add, so that a decoder layer's linears run as four launches
  * with no other ops between them: gemv_rmsnorm(q/k/v, x, w1), gemv_residual(o, att, x) -> h, gemv_rmsnorm(gate/up, h, w2),
  * gemv_glu(down, gate, up, h).  The rules of tmac_b200_gemv_grouped apply: device pointers only, the LUT built inside the launch,
- * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2 below are the
- * prompt-sized forms), and
+ * the GEMV kernel at every N (no prefill tile: tmac_b200_prefill_rmsnorm / _rmsnorm_bias / _glu / _residual / _subnorm /
+ * _subnorm_relu2 below are the prompt-sized forms), and
  * an armed tmac_b200_peer_outputs makes the call fail.  fp-path tensors with the
  * activation group inside a chunk only.  The transform is applied in fp32 (fp16 inputs widened first) to give the input a, whose
  * LUT is built as for any input.  Each call gives exactly tmac_b200_gemv_grouped(handles, count, N, F32, a, C32) with a
@@ -195,17 +195,26 @@ TMAC_B200_API int tmac_b200_gemv_grouped(const int64_t *handles, int count, int 
  *                 X[n][k] = fmul_rn(fmul_rn(r, r), U[n][k]) with r = G[n][k] when G[n][k] > 0 or is NaN (torch's relu), else +0.
  *                 U must not be NULL (gemv_subnorm is the attn sub-norm's call).  Decode sequences (seq_add_gemv_glu) and the routed
  *                 experts' GLU forms stay SiLU-only.
+ *   gemv_rmsnorm_bias: gemv_rmsnorm for projections that carry a bias (Qwen2's q_proj, k_proj and v_proj; HF Qwen2Attention has
+ *                 bias=True there and nowhere else): gemv_rmsnorm_bias(q/k/v, x, w1, b).  The arguments, rules, decomposition and
+ *                 rejections of gemv_rmsnorm, plus bias: a host array of count device pointers, bias[i] fp32 [Mout], non-null, 16-byte
+ *                 aligned, overlapping no C[j].  C[i][n][row] = fadd_rn(y, bias[i][row]), y the fp32 value gemv_rmsnorm gives that row,
+ *                 rounded once to fp16 when dtype is F16 (so with F32 it equals gemv_rmsnorm followed by a float32 add of the bias, bit
+ *                 for bit).  GQA models pass the stacked q/k/v tensor (count 1, bias [hidden + 2 * kv_dim]); MHA models three tensors
+ *                 and three biases.  tmac_b200_debug_last_launch reports what gemv_rmsnorm reports.
  * R may equal C (each element is read and written by the same thread). */
 TMAC_B200_API int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                                          void *const *C);
+TMAC_B200_API int tmac_b200_gemv_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
+                                              float eps, const float *const *bias, void *const *C);
 TMAC_B200_API int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                          const void *R, void *C);
 TMAC_B200_API int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                                const void *R, void *C);
-/* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm / gemv_glu /
- * gemv_residual / gemv_subnorm / gemv_subnorm_relu2, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
+/* The transformed-input calls at prefill sizes (a prompt): exactly the arguments and output layouts of gemv_rmsnorm /
+ * gemv_rmsnorm_bias / gemv_glu / gemv_residual / gemv_subnorm / gemv_subnorm_relu2, so a caller switches between the two forms by N (DESIGN.md 3.3), but the linears run on the prefill tiles (wgmma),
  * which stream each tensor once per 128 or 256 tokens instead of once per token.  They are the routed-expert tiles of
  * tmac_b200_prefill_experts run as one expert with the identity routing, written on the device: no host sync, graph-capturable.
  *   Input.  The call builds the input a in fp32 exactly as the gemv_* form does (fp16 inputs widened first): prefill_rmsnorm
@@ -230,6 +239,10 @@ TMAC_B200_API int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype,
  *                    prefill_subnorm(o, att, NULL, w_as, x) -> h, prefill_rmsnorm(gate/up, h, w2), prefill_subnorm(down, gate, up, w_fs, h).
  *   prefill_subnorm_relu2: prefill_subnorm with gemv_subnorm_relu2's input; U must not be NULL.  A BitNet b1.58 2B4T prompt's down
  *                    projection: prefill_subnorm_relu2(down, gate, up, w_fs, h).
+ *   prefill_rmsnorm_bias: prefill_rmsnorm with gemv_rmsnorm_bias's bias: C[i][n][row] = fadd_rn(y, bias[i][row]), y the fp32 value
+ *                    prefill_rmsnorm gives that row on the same tile kind, rounded once to fp16 when dtype is F16.  The tile choice,
+ *                    workspaces and rejections are prefill_rmsnorm's, plus the bias checks of gemv_rmsnorm_bias.  A Qwen2 prompt's
+ *                    q/k/v: prefill_rmsnorm_bias(q/k/v, x, w1, b).
  * R may equal C.  Tensors: W2/W3/W4 fp-path tensors with the act group inside the chunk: per-row scales with or without zero points,
  * K % 128 == 0, chunk 128/64/32 K; or one scale with act group 128, 64 or 32 K < K and K % 128 == 0 (chunk 128 K) or K % 128 == 64
  * (chunk 64 K, e.g. BitNet-3B's down projection, K = 8640: the int8 tile at every N, whatever the prefill16 knob).  One geometry
@@ -239,6 +252,8 @@ TMAC_B200_API int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype,
  * with N, K and Mout: make one eager call at the largest of them before capturing a call in a CUDA graph. */
 TMAC_B200_API int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                                             void *const *C);
+TMAC_B200_API int tmac_b200_prefill_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
+                                                 float eps, const float *const *bias, void *const *C);
 TMAC_B200_API int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C);
 TMAC_B200_API int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C);
 TMAC_B200_API int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,

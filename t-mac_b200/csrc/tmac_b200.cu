@@ -300,6 +300,7 @@ gemv3_fn pick_gemv3(int pb, bool sym, int qch, int agq, int minb, int in) {
         case kInGlu: return pick_gemv3_in<kInGlu>(pb, sym, qch, agq, minb);
         case kInGluNorm: return pick_gemv3_in<kInGluNorm>(pb, sym, qch, agq, minb);
         case kInRelu2Norm: return pick_gemv3_in<kInRelu2Norm>(pb, sym, qch, agq, minb);
+        case kInNormBias: return pick_gemv3_in<kInNormBias>(pb, sym, qch, agq, minb);
         case kInExperts: return pick_gemv3_in<kInExperts>(pb, sym, qch, agq, minb);
         case kInExpertsGlu: return pick_gemv3_in<kInExpertsGlu>(pb, sym, qch, agq, minb);
         default: return nullptr;
@@ -331,7 +332,7 @@ void choose_decomposition(int nrsb, int nchunk, int N, int *cs_out, int *wpc_out
 
 // Production launch: clusters + DSMEM reduction + PDL (gemv3_kernel).
 struct BatchPtrs { int n = 0; const unsigned char *const *W = nullptr; const int8_t *const *q = nullptr; const float *const *ls = nullptr,
-                   *const *lb = nullptr; void *const *C = nullptr; };
+                   *const *lb = nullptr; void *const *C = nullptr; const float *const *bias = nullptr; };
 
 // What a launch reads: LUT tables (kInTable; a grouped launch takes them from its pointer table), or activation rows [N][K] from
 // which the kernel builds a symmetric LUT (the other kinds), with the kind's Gemv3Io.
@@ -410,7 +411,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const Gem
     const size_t wregion = std::max((size_t)p.wpc * (p.nbuf * L.blk + (size_t)L.qch * 4 * (sym ? 8 : 16)), (size_t)p.wpc * L.rsb * 4);
     size_t smem = (size_t)p.cs * L.rsb * 4 + ((wregion + 15) & ~(size_t)15) + (size_t)p.wpc * 16;   // + warp-private mbarriers
     if (in.kind != kInTable && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
-    if (in.kind == kInNorm || in.kind == kInGluNorm || in.kind == kInRelu2Norm) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
+    if (in.kind == kInNorm || in.kind == kInGluNorm || in.kind == kInRelu2Norm || in.kind == kInNormBias) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
     if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t wtx, wty;
     plane_weight_regs(L.bits, sym, &wtx, &wty);
@@ -1209,11 +1210,13 @@ int tmac_b200_qgemm_lut(int64_t handle, int row0, int rows, int N, int dtype, co
 }
 
 // The setup both grouped launches share: the tensors of `handles`, which must share one geometry (*first: the first of them), and the
-// device pointer table {W, QLUT, LUT_Scales, LUT_Biases, C[i / per_c]}[count] of the call (null q / ls / lb: null entries).  Pointer
-// tables: one device allocation per distinct call signature (stable under graph capture), at most 256.
+// device pointer table {W, QLUT, LUT_Scales, LUT_Biases, C[i / per_c]}[count] of the call (null q / ls / lb: null entries), followed
+// by {bias[i / per_c]}[count] when bias is given.  Pointer tables: one device allocation per distinct call signature (stable under
+// graph capture), at most 256.
 static int grouped_setup(const char *what, const int64_t *handles, int count, const void *const *q, const void *const *ls,
-                         const void *const *lb, void *const *C, const Resident **first, BatchPtrs *bp, int per_c = 1) {
-    std::vector<const void *> tab(5 * (size_t)count, nullptr);
+                         const void *const *lb, void *const *C, const Resident **first, BatchPtrs *bp, int per_c = 1,
+                         const float *const *bias = nullptr) {
+    std::vector<const void *> tab((bias ? 6 : 5) * (size_t)count, nullptr);
     for (int i = 0; i < count; ++i) {
         auto it = g.res.find(handles[i]);
         if (it == g.res.end()) return fail(std::string(what) + ": bad weight handle");
@@ -1223,6 +1226,7 @@ static int grouped_setup(const char *what, const int64_t *handles, int count, co
             a.one_scale != b.one_scale || a.sd != b.sd || a.act_group_size != b.act_group_size || a.scale0 != b.scale0)
             return fail(std::string(what) + ": all tensors must share one geometry");
         tab[i] = it->second.d; tab[4 * count + i] = C[i / per_c];
+        if (bias) tab[5 * count + i] = bias[i / per_c];
         if (q) { tab[count + i] = q[i]; tab[2 * count + i] = ls[i]; tab[3 * count + i] = lb[i]; }
     }
     void *dtab = nullptr;
@@ -1242,6 +1246,7 @@ static int grouped_setup(const char *what, const int64_t *handles, int count, co
     bp->n = count;
     bp->W = (const unsigned char *const *)dt; bp->q = (const int8_t *const *)(dt + count);
     bp->ls = (const float *const *)(dt + 2 * count); bp->lb = (const float *const *)(dt + 3 * count); bp->C = (void *const *)(dt + 4 * count);
+    if (bias) bp->bias = (const float *const *)(dt + 5 * count);
     return 0;
 }
 
@@ -1319,14 +1324,33 @@ static int residual_check(const std::string &what, int64_t handle, int N, int dt
     io->res = R;
     return io_check(what, &handle, 1, N, dtype, B, *io, &C);
 }
+// The biases of tmac_b200_gemv_rmsnorm_bias / tmac_b200_prefill_rmsnorm_bias, after rmsnorm_check: count 16-byte aligned device
+// vectors fp32 [Mout] (Mout of handles[0]; the geometry check follows) that overlap no C[i] ([N][Mout] of dtype).
+static int bias_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const float *const *bias, void *const *C) {
+    if (!bias) return fail(what + ": bias must not be null");
+    auto it = g.res.find(handles[0]);
+    if (it == g.res.end()) return fail(what + ": bad weight handle");
+    const size_t bb = (size_t)it->second.L.Mout * sizeof(float), cb = (size_t)N * it->second.L.Mout * (dtype == TMAC_B200_F16 ? 2 : 4);
+    for (int i = 0; i < count; ++i) {
+        if (!bias[i] || ((uintptr_t)bias[i] & 15) || !is_device_ptr(bias[i])) return fail(what + ": each bias must be a 16-byte aligned device vector");
+        const uintptr_t b0 = (uintptr_t)bias[i];
+        for (int j = 0; j < count; ++j) {
+            const uintptr_t c0 = (uintptr_t)C[j];
+            if (b0 < c0 + cb && c0 < b0 + bb) return fail(what + ": a bias must not overlap an output");
+        }
+    }
+    return 0;
+}
 
 // tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
-// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res.  The arguments are checked.
+// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res, or (kInNormBias) the biases
+// bias[count] through the pointer table.  The arguments are checked.
 static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
-                   const Gemv3Io &io, void *const *C) {
+                   Gemv3Io io, void *const *C, const float *const *bias = nullptr) {
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count, nullptr, nullptr, nullptr, C, &R, &bp)) return -1;
+    if (grouped_setup(what.c_str(), handles, count, nullptr, nullptr, nullptr, C, &R, &bp, 1, bias)) return -1;
+    io.biasv = bp.bias;
     const StreamLayout &L = R->L;
     if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
     return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kind, A, dtype == TMAC_B200_F16, io), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
@@ -1339,6 +1363,16 @@ int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, 
     Gemv3Io io;
     if (rmsnorm_check("gemv_rmsnorm", handles, count, N, dtype, H, w, eps, C, &io)) return -1;
     return gemv_io("gemv_rmsnorm", handles, count, N, dtype, kInNorm, H, io, C);
+}
+
+int tmac_b200_gemv_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                                const float *const *bias, void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "gemv_rmsnorm_bias";
+    Gemv3Io io;
+    if (rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io) || bias_check(what, handles, count, N, dtype, bias, C)) return -1;
+    return gemv_io(what, handles, count, N, dtype, kInNormBias, H, io, C, bias);
 }
 
 int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
@@ -1455,11 +1489,11 @@ static int refuse_peer(const std::string &what) {
 // relu2(A[s], U[s]) when relu2; nw != null:
 // the N rows rms_scale(A[n], inv_n, nw); both: the RMS norm of the SwiGLU rows, all materialised in fp32), gather each table entry's LUT records and run the routed tile over
 // (row tiles, table entries, count).  wts != null (the GLU experts): the tile stores the slots' fp32 rows and the combine adds them
-// (+ R); otherwise the tile adds R (when not null) in its epilogue.  Everything is checked and every workspace allocated before
-// anything is launched.
+// (+ R); otherwise the tile adds R (when not null) in its epilogue.  bias != null (prefill_rmsnorm_bias; no R, no wts): the BIAS
+// tiles add bias[i] to tensor i's outputs.  Everything is checked and every workspace allocated before anything is launched.
 static int prefill_routed(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
                           int N, int dtype, int topk, const void *A, const void *U, const float *nw, float eps, const int32_t *ids,
-                          const float *wts, const void *Rres, void *const *C, bool relu2 = false) {
+                          const float *wts, const void *Rres, void *const *C, bool relu2 = false, const float *const *bias = nullptr) {
     const bool combine = wts != nullptr, slot_rows = U != nullptr;   // slot_rows: one input row per slot (GLU), else per token
     if (n_experts > 256) return fail(what + ": n_experts must be 1..256");   // the routing kernel's shared arrays
     auto it0 = g.res.find(handles[0]);
@@ -1473,9 +1507,10 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     if (combine && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : C, &R, &bp, n_experts))
+    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : C, &R, &bp, n_experts,
+                      bias))
         return -1;
-    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq(), L.one_scale, L.K % 128 != 0);
+    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq(), L.one_scale, L.K % 128 != 0, bias != nullptr);
     if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
     const TilePlan t(L, false);
     // the tile rule: routed experts as experts_take_tile16, the dense forms as the dense calls (launch_prefill)
@@ -1506,7 +1541,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
         CUDA_OK(cudaGetLastError());
         if (launch_preprocessor(K, rows, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
     } else if (launch_preprocessor(K, rows, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
-    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts, combine ? nullptr : Rres};
+    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts, combine ? nullptr : Rres, bp.bias};
     const int div = slot_rows ? 1 : topk, out_f16 = combine ? 0 : f16;
     const dim3 grid(t.nrt, (unsigned)cap, count);
     if (t16) {
@@ -1558,6 +1593,19 @@ int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtyp
     Gemv3Io io;
     if (refuse_peer(what) || rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io)) return -1;
     return prefill_routed(what, "gemv_rmsnorm", handles, count, 1, N, dtype, 1, H, nullptr, w, eps, nullptr, nullptr, nullptr, C);
+}
+
+int tmac_b200_prefill_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                                   const float *const *bias, void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    const std::string what = "prefill_rmsnorm_bias";
+    Gemv3Io io;
+    if (refuse_peer(what) || rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io) ||
+        bias_check(what, handles, count, N, dtype, bias, C))
+        return -1;
+    return prefill_routed(what, "gemv_rmsnorm_bias", handles, count, 1, N, dtype, 1, H, nullptr, w, eps, nullptr, nullptr, nullptr, C,
+                          false, bias);
 }
 
 int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {

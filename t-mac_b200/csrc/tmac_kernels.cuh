@@ -515,14 +515,16 @@ struct Gemv3Params {
 // The routed-expert kinds (kInExperts, kInExpertsGlu) pick each slot's tensor on the device: slot z = i * topk + j of token n
 // (blockIdx.z, blockIdx.y) runs pointer-table entry i * n_experts + ids[n * topk + j].
 // kInGluNorm is the RMS norm of the SwiGLU row (BitNet's ffn_sub_norm before the down projection); kInRelu2Norm the RMS norm of
-// the squared-ReLU row (the same sub-norm in BitNet b1.58 2B4T, whose FFN gate is relu2).
-enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5, kInGluNorm = 6, kInRelu2Norm = 7 };
+// the squared-ReLU row (the same sub-norm in BitNet b1.58 2B4T, whose FFN gate is relu2).  kInNormBias is kInNorm whose outputs
+// take a per-tensor bias (Qwen2's q/k/v projections).
+enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5, kInGluNorm = 6, kInRelu2Norm = 7,
+             kInNormBias = 8 };
 // The input transform and residual of the row kinds: the kernel's last parameter, so that Gemv3Params, wtx and wty keep their
 // parameter offsets.
 struct Gemv3Io {
     const void *act2;              // kInGlu, kInGluNorm, kInRelu2Norm, kInExpertsGlu: u [N][K] / [N][topk][K], dtype of p.act
-    const float *nw;               // kInNorm, kInGluNorm, kInRelu2Norm: the norm weight w [K] (16-byte aligned)
-    float eps;                     // kInNorm, kInGluNorm, kInRelu2Norm
+    const float *nw;               // kInNorm, kInGluNorm, kInRelu2Norm, kInNormBias: the norm weight w [K] (16-byte aligned)
+    float eps;                     // kInNorm, kInGluNorm, kInRelu2Norm, kInNormBias
     const void *res;               // fp path, kInRow / kInNorm / kInGlu / kInGluNorm / kInRelu2Norm / kInExpertsGlu: residual r [N][ldc] of the output's dtype,
                                    // or null; may equal C
     const int32_t *ids;            // experts: [N][topk], written by earlier work in the stream (read after the dependency wait)
@@ -530,6 +532,7 @@ struct Gemv3Io {
     float *ws;                     // kInExpertsGlu: the slots' fp32 rows [N][topk][ldc]
     unsigned *cnt;                 // kInExpertsGlu: arrivals per (token, row super-block) [N][nrsb], 0 between launches
     int topk, n_experts;           // experts
+    const float *const *biasv;     // kInNormBias: bias[z] fp32 [Mout] of the grouped launch's tensor z (device pointer table)
 };
 __device__ __forceinline__ long long globaltimer_ns() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 #ifdef TMAC_ENABLE_TRACE
@@ -642,8 +645,9 @@ constexpr int kG3MaxWarps = 8;
 // the row's LUT bias in the reference's order (addv tree per 32 activations, serial over the blocks).
 // The LUT input of row n is the row itself (kInRow) or a transform of the activation rows -- kInNorm a[k] = rms_scale(h[k], inv_n,
 // w[k]), kInGlu a[k] = swiglu(g[k], u[k]), kInGluNorm a[k] = rms_scale(s[k], inv_n, w[k]) with s[k] = swiglu(g[k], u[k]) and inv_n
-// from the sum of squares of s, kInRelu2Norm the same with s[k] = relu2(g[k], u[k]) -- built into the chunk's slice with lut_slice as
-// a plain input; on the fp path the leader adds io.res (when not null) to the row sums before the store.
+// from the sum of squares of s, kInRelu2Norm the same with s[k] = relu2(g[k], u[k]), kInNormBias kInNorm's -- built into the chunk's
+// slice with lut_slice as a plain input; on the fp path the leader adds io.res (when not null) to the row sums before the store, and
+// kInNormBias adds its tensor's bias there instead: C = fadd_rn(row sum, bias[z][row]), rounded once at the store.
 // Routed experts: slot z = i * topk + j of token n takes its tensor from the pointer table at
 // i * n_experts + ids[n][j], read after the dependency wait, so the slot's first block request waits for it too.  kInExperts reads row
 // n and stores row n * topk + j of C[i]; kInExpertsGlu reads row n * topk + j of g and u, stores its rows into io.ws and counts
@@ -823,8 +827,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             if (lane == 0) *bias_out = bias;       // forwarded to the leader with the partial sums below
         }
     }
-    float inv = 0.f;                              // kInNorm, kInGluNorm, kInRelu2Norm: 1 / rms of the row
-    if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm) {
+    float inv = 0.f;                              // kInNorm, kInGluNorm, kInRelu2Norm, kInNormBias: 1 / rms of the row
+    if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm || IN == kInNormBias) {
         // Every CTA computes inv itself.  All threads stage the row (kInGluNorm / kInRelu2Norm: its swiglu / relu2 of the row of g
         // and the row of u), widened to fp32, in shared memory (iscr [K] | inv), with their loads in flight together; warp 0 then
         // sums its squares in the order of rms_sumsq / rms_warp_sum.
@@ -870,7 +874,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         if (IN != kInTable) {
             constexpr int NG = QCH * 4;            // lane = K-group of the chunk
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm) {
+            if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm || IN == kInNormBias) {
                 if (lane < NG) {
                     const size_t g = (size_t)c * NG + lane;
                     const float4 h = reinterpret_cast<const float4 *>(iscr)[g], w = __ldg(reinterpret_cast<const float4 *>(io.nw) + g);
@@ -974,6 +978,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
                 const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
                 if (IN != kInTable && !INT_PATH && io.res)   // read, then written by this thread: the residual may be C itself
                     out = __fadd_rn(out, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
+                if (IN == kInNormBias) out = __fadd_rn(out, __ldg(io.biasv[blockIdx.z] + (row - p.c_row0)));
                 store_out(Cb, o, out, p.out_f16);
                 for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
                     store_out(p.Cpeer[q], o, out, p.out_f16);
@@ -1015,7 +1020,7 @@ typedef void (*gemv3_fn)(const Gemv3Params, const uint32_t, const uint32_t, cons
 // gemv3_kernel<PB, SYM, QCH, AGQ, MINB, IN> for a tensor's (pb, qch, agq), the LUT's symmetry (kInTable; the other kinds are
 // symmetric) and minb; null for a grouping that is not instantiated.  Each kind's kernels are compiled in the one translation unit
 // that instantiates pick_gemv3_in for it, so that the kinds compile in parallel: kInTable in tmac_b200.cu, kInRow, kInNorm, kInGlu,
-// kInGluNorm and kInRelu2Norm in tmac_gemv_io.cu, kInExperts and kInExpertsGlu in tmac_gemv_experts.cu.
+// kInGluNorm, kInRelu2Norm and kInNormBias in tmac_gemv_io.cu, kInExperts and kInExpertsGlu in tmac_gemv_experts.cu.
 template <int IN> gemv3_fn pick_gemv3_in(int pb, bool sym, int qch, int agq, int minb) {
     const auto pick = [&](auto SYM, auto MINB) {
         return with_pb<gemv3_fn>(pb, [&](auto PB) {
@@ -1039,6 +1044,7 @@ extern template gemv3_fn pick_gemv3_in<kInNorm>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInGlu>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInGluNorm>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInRelu2Norm>(int, bool, int, int, int);
+extern template gemv3_fn pick_gemv3_in<kInNormBias>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInExperts>(int, bool, int, int, int);
 extern template gemv3_fn pick_gemv3_in<kInExpertsGlu>(int, bool, int, int, int);
 

@@ -146,6 +146,7 @@ struct PfRoute {
     void *const *C;                      // C[i * n_experts + e]: where tensor i stores slot s's row, at row s of [N * topk][Mout]
     int n_experts;
     const void *R;                       // null, or the residual added to every output: R[s][row] of C's type (the dense forms)
+    const float *const *bias;            // the BIAS tiles (prefill_rmsnorm_bias): bias[i * n_experts + e] fp32 [Mout], indexed like C
 };
 // A routed tile's output element C[o] = v (RES: + R[o], fp16 R widened).  R is read, then C written, by the same thread: R may be C.
 // The epilogues branch on route.R once and run a store loop per case, so the experts' loop (no R) stores as it did without it.
@@ -155,6 +156,13 @@ __device__ __forceinline__ void pf_route_store(const PfRoute &route, void *const
     store_out(C, o, v, out_f16);
 }
 template <bool V> struct PfRes { static constexpr bool value = V; };
+// The BIAS tiles' case: no residual, and every output of tensor i is fadd_rn(v, b[row]) with b its bias, rounded once at the store.
+struct PfBias { static constexpr bool value = false; const float *b; };
+// The epilogues' output value of (row, v): v, or PfBias's sum.
+template <typename E> __device__ __forceinline__ float pf_bias_add(const E &e, int row, float v) {
+    if constexpr (std::is_same_v<E, PfBias>) return __fadd_rn(v, __ldg(e.b + row));
+    else return v;
+}
 template <bool INT_PATH, int QCH, int AGQ>
 __device__ __forceinline__ void lut_tile_rec(const int8_t *qlut, const float *ls, const float *lb, unsigned char *rec, int n, bool live,
                                              int K, int step, int t) {
@@ -296,12 +304,13 @@ __device__ __forceinline__ void pf_build_xtab(uint64_t *xtab, int bits, bool bia
 // W[i * n_experts + expert] of the pointer table, the records of entry k (lut_tile_gather_kernel) and stores token t's row at row
 // perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one (pf_route_store).  A tensor with
 // p.sd == 0 has one scale (see the header).  UNIT1 (ROUTE, QCH 4, one-scale tensors with K % 128 == 64): a staging unit is one
-// 64-K chunk, one step.
-template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE, bool UNIT1 = false>
+// 64-K chunk, one step.  BIAS (ROUTE, prefill_bias_kernel): no residual; each output takes route.bias's row (PfBias).
+template <int PB, bool INT_PATH, int QCH, int AGQ, bool ROUTE, bool UNIT1 = false, bool BIAS = false>
 __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
     static_assert(!(ROUTE && INT_PATH), "routed experts: fp path only");
     static_assert(!UNIT1 || (ROUTE && QCH == 4), "one-chunk staging: routed 64-K chunks only");
+    static_assert(!BIAS || ROUTE, "biases: routed tiles only");
     using G = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
@@ -515,11 +524,12 @@ __device__ __forceinline__ void prefill_body(const PrefillParams &p, const PfRou
                             const int t = 8 * c8 + tc + e;
                             if (t < ntok)
                                 pf_route_store<decltype(res)::value>(route, Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row,
-                                                                     accf[4 * c8 + 2 * h + e], p.out_f16);
+                                                                     pf_bias_add(res, row, accf[4 * c8 + 2 * h + e]), p.out_f16);
                         }
                 }
             };
-            if (route.R) stores(PfRes<true>{});
+            if constexpr (BIAS) stores(PfBias{route.bias[blockIdx.z * route.n_experts + ent.x]});
+            else if (route.R) stores(PfRes<true>{});
             else stores(PfRes<false>{});
             return;
         }
@@ -548,6 +558,12 @@ __global__ void __launch_bounds__(kPfThreads2, 1) prefill_kernel(const PrefillPa
 template <int PB, int QCH, int AGQ, bool UNIT1 = false>
 __global__ void __launch_bounds__(kPfThreads2, 1) prefill_experts_kernel(const PrefillParams p, const PfRoute route) {
     prefill_body<PB, false, QCH, AGQ, true, UNIT1>(p, route);
+}
+// prefill_experts_kernel with a bias on every output (tmac_b200_prefill_rmsnorm_bias): kernels of their own, so that the routed
+// kernels' epilogues are not touched
+template <int PB, int QCH, int AGQ, bool UNIT1 = false>
+__global__ void __launch_bounds__(kPfThreads2, 1) prefill_bias_kernel(const PrefillParams p, const PfRoute route) {
+    prefill_body<PB, false, QCH, AGQ, true, UNIT1, true>(p, route);
 }
 
 }  // namespace tmac_b200

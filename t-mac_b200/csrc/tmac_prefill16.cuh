@@ -162,11 +162,13 @@ __global__ void __launch_bounds__(256) lut_tile16_gather_kernel(const int8_t *ql
 // entry is unused, else runs tile k * nrt + blockIdx.x on the weights W[i * n_experts + expert], the B tiles of entry k, and stores
 // token t's row at row perm[start + t] of C[i * n_experts + expert], plus the residual route.R when there is one.  ONE (ROUTE, QCH 8): a
 // one-scale tensor, whose blocks carry no scales: hs = fp16(0.5 * scale0), no zero point.  A template parameter rather than a test of
-// p.sd: the run-time test made the producers of the per-row-scale instantiations slower.
-template <int PB, int QCH, int AGQ, bool ROUTE, bool ONE = false>
+// p.sd: the run-time test made the producers of the per-row-scale instantiations slower.  BIAS (ROUTE, prefill16_bias_kernel): no
+// residual; each output takes route.bias's row (PfBias).
+template <int PB, int QCH, int AGQ, bool ROUTE, bool ONE = false, bool BIAS = false>
 __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const PfRoute &route) {
     static_assert(PB == 2 || PB == 4, "prefill tile: W2 or W3/W4 stream layout");
     static_assert(!ONE || (ROUTE && QCH == 8), "one-scale tensors: routed, 128-K chunks");
+    static_assert(!BIAS || ROUTE, "biases: routed tiles only");
     using PG = PfGroups<QCH, AGQ>;
     constexpr int RSB = 32 * (8 / PB);                                     // rows per super-block
     constexpr int NSB = 128 / RSB;                                         // super-blocks per row tile
@@ -365,11 +367,12 @@ __device__ __forceinline__ void prefill16_body(const Prefill16Params &p, const P
                                 const int t = 8 * c8 + tc + e;
                                 if (t < ent.z && row < p.Mout)
                                     pf_route_store<decltype(res)::value>(route, Cr, (size_t)__ldg(route.perm + ent.y + t) * p.ldc + row,
-                                                                         acc[4 * c8 + 2 * h + e], p.out_f16);
+                                                                         pf_bias_add(res, row, acc[4 * c8 + 2 * h + e]), p.out_f16);
                             }
                     }
                 };
-                if (route.R) stores(PfRes<true>{});
+                if constexpr (BIAS) stores(PfBias{route.bias[blockIdx.z * route.n_experts + ent.x]});
+                else if (route.R) stores(PfRes<true>{});
                 else stores(PfRes<false>{});
                 continue;
             }
@@ -435,6 +438,11 @@ template <int PB, int QCH, int AGQ, bool ONE = false>
 __global__ void __launch_bounds__(kP16Threads, 1) prefill16_experts_kernel(const Prefill16Params p, const PfRoute route) {
     prefill16_body<PB, QCH, AGQ, true, ONE>(p, route);
 }
+// prefill16_experts_kernel with a bias on every output (tmac_b200_prefill_rmsnorm_bias), as prefill_bias_kernel
+template <int PB, int QCH, int AGQ, bool ONE = false>
+__global__ void __launch_bounds__(kP16Threads, 1) prefill16_bias_kernel(const Prefill16Params p, const PfRoute route) {
+    prefill16_body<PB, QCH, AGQ, true, ONE, true>(p, route);
+}
 
 // The routed launches (tmac_b200_prefill_experts / _glu, and the dense tmac_b200_prefill_rmsnorm / _glu / _residual as one expert):
 // the kernels of one tensor kind (PB) and fp grouping, instantiated in tmac_prefill_experts.cu (one: a one-scale tensor, whose fp16
@@ -447,7 +455,8 @@ struct PfExpertKernels {
     void (*tile16)(const Prefill16Params, const PfRoute);
     void (*lut16)(const int8_t *, const float *, const float *, unsigned char *, int, int, int, const int4 *, const int *, int);
 };
-PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1);
+// bias: the tiles are prefill_bias_kernel / prefill16_bias_kernel (tmac_b200_prefill_rmsnorm_bias)
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1, bool bias = false);
 void pf_route_launch(const int32_t *ids, int S, int E, int T, int cap, int4 *tiles, int *perm, void *const *Cnan, int count, int ldc,
                      int out_f16, cudaStream_t st);
 void pf_swiglu_launch(const void *G, const void *U, int f16, size_t n, float *a, cudaStream_t st, bool relu2 = false);

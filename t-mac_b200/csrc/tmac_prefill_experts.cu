@@ -2,7 +2,8 @@
 // dense transformed-input forms (tmac_b200_prefill_rmsnorm / _glu / _residual), which run as one expert with the identity routing.
 // The routing kernel that groups the slots by expert, the routed instantiations of both wgmma tiles and their gathered LUT records
 // (3 bit widths x 6 fp groupings, plus for one-scale tensors the fp16 tile's 128-K-chunk groupings and the int8 tile's 64-K chunk
-// units; tmac_prefill.cuh, tmac_prefill16.cuh), the RMSNorm, GLU and sub-norm inputs and the GLU combine.  In their
+// units; tmac_prefill.cuh, tmac_prefill16.cuh), the same tiles once more with a bias on the outputs (tmac_b200_prefill_rmsnorm_bias),
+// the RMSNorm, GLU and sub-norm inputs and the GLU combine.  In their
 // own translation unit so that they compile in parallel with tmac_b200.cu.
 #include "tmac_prefill16.cuh"
 
@@ -117,27 +118,41 @@ __global__ void __launch_bounds__(256) pf_combine_kernel(const float *ys, const 
     store_out(C, i, acc, out_f16);
 }
 
-template <int PB> PfExpertKernels pick_pf_experts_pb(int qch, int agq, bool one, bool unit1) {
+// BIAS: the same tiles with a bias on the outputs (prefill_bias_kernel, prefill16_bias_kernel)
+template <int PB, bool BIAS> PfExpertKernels pick_pf_experts_pb(int qch, int agq, bool one, bool unit1) {
+    using Tile = void (*)(const PrefillParams, const PfRoute);
+    using Tile16 = void (*)(const Prefill16Params, const PfRoute);
+    const auto tile = [](auto QCH, auto AGQ, auto UNIT1) -> Tile {
+        if constexpr (BIAS) return prefill_bias_kernel<PB, QCH, AGQ, UNIT1>;
+        else return prefill_experts_kernel<PB, QCH, AGQ, UNIT1>;
+    };
+    const auto tile16 = [](auto QCH, auto AGQ, auto ONE) -> Tile16 {
+        if constexpr (BIAS) return prefill16_bias_kernel<PB, QCH, AGQ, ONE>;
+        else return prefill16_experts_kernel<PB, QCH, AGQ, ONE>;
+    };
+    using I4 = std::integral_constant<int, 4>;
+    using I8 = std::integral_constant<int, 8>;
+    using I2 = std::integral_constant<int, 2>;
     if (unit1) {                                 // one-scale, K % 128 == 64: 64-K chunks staged one per unit, the int8 tile only
-        if (qch == 4 && agq == 4) return {prefill_experts_kernel<PB, 4, 4, true>, lut_tile_gather_kernel<4, 4>, nullptr, nullptr};
-        if (qch == 4 && agq == 2) return {prefill_experts_kernel<PB, 4, 2, true>, lut_tile_gather_kernel<4, 2>, nullptr, nullptr};
+        if (qch == 4 && agq == 4) return {tile(I4{}, I4{}, std::true_type{}), lut_tile_gather_kernel<4, 4>, nullptr, nullptr};
+        if (qch == 4 && agq == 2) return {tile(I4{}, I2{}, std::true_type{}), lut_tile_gather_kernel<4, 2>, nullptr, nullptr};
         return PfExpertKernels{};
     }
-    PfExpertKernels k = FpGroupings::find<PfExpertKernels>(qch, agq, [](auto QCH, auto AGQ) -> PfExpertKernels {
-        return {prefill_experts_kernel<PB, QCH, AGQ>, lut_tile_gather_kernel<QCH, AGQ>, prefill16_experts_kernel<PB, QCH, AGQ>,
+    PfExpertKernels k = FpGroupings::find<PfExpertKernels>(qch, agq, [&](auto QCH, auto AGQ) -> PfExpertKernels {
+        return {tile(QCH, AGQ, std::false_type{}), lut_tile_gather_kernel<QCH, AGQ>, tile16(QCH, AGQ, std::false_type{}),
                 lut_tile16_gather_kernel<QCH, AGQ>};
     });
     if (one)                                     // one-scale, K % 128 == 0: chunk 128 K, the fp16 tile's own instantiations
-        k.tile16 = qch != 8 ? nullptr : agq == 8 ? prefill16_experts_kernel<PB, 8, 8, true> : agq == 4 ? prefill16_experts_kernel<PB, 8, 4, true>
-                 : agq == 2 ? prefill16_experts_kernel<PB, 8, 2, true> : nullptr;
+        k.tile16 = qch != 8 ? nullptr : agq == 8 ? tile16(I8{}, I8{}, std::true_type{}) : agq == 4 ? tile16(I8{}, I4{}, std::true_type{})
+                 : agq == 2 ? tile16(I8{}, I2{}, std::true_type{}) : nullptr;
     return k;
 }
 
 }  // namespace
 
-PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1) {
-    if (pb == 4) return pick_pf_experts_pb<4>(qch, agq, one, unit1);
-    if (pb == 2) return pick_pf_experts_pb<2>(qch, agq, one, unit1);
+PfExpertKernels pick_pf_experts(int pb, int qch, int agq, bool one, bool unit1, bool bias) {
+    if (pb == 4) return bias ? pick_pf_experts_pb<4, true>(qch, agq, one, unit1) : pick_pf_experts_pb<4, false>(qch, agq, one, unit1);
+    if (pb == 2) return bias ? pick_pf_experts_pb<2, true>(qch, agq, one, unit1) : pick_pf_experts_pb<2, false>(qch, agq, one, unit1);
     return PfExpertKernels{};
 }
 

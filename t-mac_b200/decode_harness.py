@@ -10,7 +10,8 @@ one; with `fused_ops=True` the seven linears run as four library launches whose 
 SiLU*mul and the residual adds (tools/layer_bench.py times the four); adding `experts=E` makes the FFN a routed MoE of E experts with
 top-k routing, run as two library launches that pick the experts on the device (tools/moe_bench.py times them); `sub_norms=True`
 makes the layer BitNet b1.58's, with an RMSNorm before o and one before down (tools/layer_bench.py --bitnet; with `ffn_act="relu2"`
-and `kv_heads` < heads, BitNet b1.58 2B4T's, tools/layer_bench.py --bitnet2b).  `prompt()` is the
+and `kv_heads` < heads, BitNet b1.58 2B4T's, tools/layer_bench.py --bitnet2b); `qkv_bias=True` gives q/k/v a bias, as Qwen2's
+(tools/layer_bench.py --qwen2).  `prompt()` is the
 prompt step: P tokens through every layer, with causal attention over cache positions [0, P) and the linears on the prefill tiles
 (tmac_b200_prefill_*; tools/prompt_bench.py times it).
 
@@ -73,7 +74,7 @@ class QLinear:
 class DecodeLayer:
     def __init__(self, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, seed: int, share: Optional["DecodeLayer"] = None, group_size: int = 128,
                  ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
-                 sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None):
+                 sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None, qkv_bias: bool = False):
         """ffn_sequence: the FFN (gate, up, SiLU*mul, down) runs as ONE decode sequence whose down op reads the gated activation of
         the gate and up ops (tmac_b200_seq_add_gemv_glu) instead of three launches and a torch op.
         post_attn_sequence: the layer after attention runs as ONE decode sequence [o(att) + x, gate(rmsnorm(h) * w2),
@@ -93,6 +94,9 @@ class DecodeLayer:
         kv_heads (default heads): kv_heads < heads is grouped-query attention -- each KV head serves heads / kv_heads consecutive
         query heads and the KV cache holds kv_heads heads.  q, k and v are then one stacked tensor "qkv" of hidden + 2 * kv_heads * hd
         rows (one launch, whose output q / k / v are views of), the usual way to group GQA projections.
+        qkv_bias: q, k and v (or the stacked qkv) carry a seeded fp32 bias, as Qwen2's (HF Qwen2Attention, bias=True on q_proj,
+        k_proj and v_proj only).  fused_ops layers run gemv_rmsnorm_bias / prefill_rmsnorm_bias for them; the other layers and the
+        dense reference (`linear`) add the bias with torch after each projection.
         The prompt step (`prompt`) runs the fused_ops launches in their prefill forms (prefill_rmsnorm, prefill_residual,
         prefill_glu, prefill_subnorm, prefill_experts, prefill_experts_glu); the sequences are decode-only, so sequence layers run
         per-linear calls."""
@@ -142,6 +146,8 @@ class DecodeLayer:
             self.w_as = (1.0 + 0.1 * torch.randn(hidden, generator=g)).cuda()
             self.w_fs = (1.0 + 0.1 * torch.randn(ffn, generator=g)).cuda()
             self.buf["att_n"] = f(hidden)
+        # drawn last, so that every other tensor of the layer is the one it has without biases
+        self.qkv_b = {n: (0.5 * torch.randn(self.lin[n].mout, generator=g)).cuda() for n in self.qkv_names} if qkv_bias else None
         self.pbuf = {}                              # the prompt step's buffers, [P][...], made by its first call
         self.ffn_seq = self.post_seq = None
         if ffn_sequence:
@@ -208,12 +214,7 @@ class DecodeLayer:
         torch, b = self.torch, self.buf
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
         fused = self.fused_ops and linear is None
-        if fused:
-            tb.gemv_rmsnorm([self.lin[n].wt for n in self.qkv_names], 1, x, self.norm1, self.EPS, [b[n] for n in self.qkv_names])
-        else:
-            b["h1"].copy_(self.rmsnorm(torch, x, self.norm1))
-            for n in self.qkv_names:
-                lin(n, b["h1"], b[n])
+        self.qkv(x, b, 1, fused, lin)
         q = self.rope(b["q"], pos_cos, pos_sin).view(self.heads, 1, self.hd)
         kcache[:, pos] = self.rope(b["k"], pos_cos, pos_sin).view(self.kv_heads, self.hd)
         vcache[:, pos] = b["v"].view(self.kv_heads, self.hd)
@@ -246,6 +247,23 @@ class DecodeLayer:
             self.ffn_act(b)
             lin("down", b["act"], b["down"])
         return h + b["down"]
+
+    def qkv(self, x, b, n, fused, lin):
+        """The q/k/v projections of rmsnorm(x) * norm1 into the buffers b (n rows: the token step's GEMV forms at n = 1, else the
+        prompt step's prefill forms), plus their biases in a qkv_bias layer."""
+        wts, outs = [self.lin[m].wt for m in self.qkv_names], [b[m] for m in self.qkv_names]
+        decode = b is self.buf
+        if fused and self.qkv_b is not None:
+            bias = [self.qkv_b[m] for m in self.qkv_names]
+            (tb.gemv_rmsnorm_bias if decode else tb.prefill_rmsnorm_bias)(wts, n, x, self.norm1, self.EPS, bias, outs)
+        elif fused:
+            (tb.gemv_rmsnorm if decode else tb.prefill_rmsnorm)(wts, n, x, self.norm1, self.EPS, outs)
+        else:
+            b["h1"].copy_(self.rmsnorm(self.torch, x, self.norm1))
+            for m in self.qkv_names:
+                lin(m, b["h1"], b[m])
+                if self.qkv_b is not None:
+                    b[m].add_(self.qkv_b[m])
 
     def attn_sub_norm(self, b):
         """The o projection's input from the buffers b: att, or rmsnorm(att) * w_as in a sub_norms layer (torch ops)."""
@@ -312,18 +330,14 @@ class DecodeLayer:
         prefill_rmsnorm([q, k, v]), prefill_residual(o), the torch router over the P tokens, prefill_experts([gate, up]) and
         prefill_experts_glu(down, R=h); sub_norms + fused_ops layers as prefill_rmsnorm([q, k, v]), prefill_subnorm(o, att, w_as,
         R=x), prefill_rmsnorm([gate, up]) and prefill_subnorm(down, gate, w_fs, U=up, R=h) (relu2 layers: prefill_subnorm_relu2);
-        GQA layers run [qkv] in place of [q, k, v]; the other layers as one call per linear.
+        GQA layers run [qkv] in place of [q, k, v], qkv_bias layers prefill_rmsnorm_bias in place of prefill_rmsnorm for them; the
+        other layers as one call per linear.
         `linear` and `routed` as for forward."""
         torch, P = self.torch, x.shape[0]
         b = self.prompt_buffers(P)
         lin = linear or (lambda n, inp, out: self.lin[n](inp, out))
         fused = self.fused_ops and linear is None
-        if fused:
-            tb.prefill_rmsnorm([self.lin[n].wt for n in self.qkv_names], P, x, self.norm1, self.EPS, [b[n] for n in self.qkv_names])
-        else:
-            b["h1"].copy_(self.rmsnorm(torch, x, self.norm1))
-            for n in self.qkv_names:
-                lin(n, b["h1"], b[n])
+        self.qkv(x, b, P, fused, lin)
         q = self.rope(b["q"], cos, sin).view(P, self.heads, self.hd).transpose(0, 1)
         kcache[:, :P] = self.rope(b["k"], cos, sin).view(P, self.kv_heads, self.hd).transpose(0, 1)
         vcache[:, :P] = b["v"].view(P, self.kv_heads, self.hd).transpose(0, 1)
@@ -369,11 +383,12 @@ class DecodeModel:
 
     def __init__(self, layers: int, hidden: int, ffn: int, heads: int, bits: int, zero_point: bool, ctx: int = 512, seed: int = 0,
                  ffn_sequence: bool = False, post_attn_sequence: bool = False, fused_ops: bool = False, experts: int = 0, topk: int = 2,
-                 prompt_len: int = 0, sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None):
+                 prompt_len: int = 0, sub_norms: bool = False, ffn_act: str = "silu", kv_heads: Optional[int] = None,
+                 qkv_bias: bool = False):
         import torch
         self.torch, self.hidden, self.ctx, self.heads, self.hd = torch, hidden, ctx, heads, hidden // heads
         kw = dict(ffn_sequence=ffn_sequence, post_attn_sequence=post_attn_sequence, fused_ops=fused_ops, experts=experts, topk=topk,
-                  sub_norms=sub_norms, ffn_act=ffn_act, kv_heads=kv_heads)
+                  sub_norms=sub_norms, ffn_act=ffn_act, kv_heads=kv_heads, qkv_bias=qkv_bias)
         first = DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, **kw)
         self.layers: List[DecodeLayer] = [first] + [DecodeLayer(hidden, ffn, heads, bits, zero_point, seed, share=first, **kw)
                                                     for _ in range(layers - 1)]

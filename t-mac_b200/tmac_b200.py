@@ -44,7 +44,7 @@ EXPORTS = [
     "tmac_b200_find_kcfg", "tmac_b200_clear_kcfg", "tmac_b200_upload_weights", "tmac_b200_upload_plain",
     "tmac_b200_upload_plain_rows", "tmac_b200_debug_encode", "tmac_b200_free_weights", "tmac_b200_clone_weights", "tmac_b200_hint_next_weights",
     "tmac_b200_graph_begin", "tmac_b200_graph_end", "tmac_b200_graph_launch", "tmac_b200_graph_free", "tmac_b200_sync", "tmac_b200_debug_trace", "tmac_b200_debug_last_launch", "tmac_b200_debug_set", "tmac_b200_weights_nbytes", "tmac_b200_preprocessor",
-    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_subnorm_relu2", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_prefill_subnorm", "tmac_b200_prefill_subnorm_relu2", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
+    "tmac_b200_qgemm_lut", "tmac_b200_qgemm_lut_grouped", "tmac_b200_gemv", "tmac_b200_gemv_grouped", "tmac_b200_gemv_rmsnorm", "tmac_b200_gemv_rmsnorm_bias", "tmac_b200_gemv_glu", "tmac_b200_gemv_residual", "tmac_b200_gemv_subnorm", "tmac_b200_gemv_subnorm_relu2", "tmac_b200_gemv_experts", "tmac_b200_gemv_experts_glu", "tmac_b200_prefill_experts", "tmac_b200_prefill_experts_glu", "tmac_b200_prefill_rmsnorm", "tmac_b200_prefill_rmsnorm_bias", "tmac_b200_prefill_glu", "tmac_b200_prefill_residual", "tmac_b200_prefill_subnorm", "tmac_b200_prefill_subnorm_relu2", "tmac_b200_cbits", "qgemm_lut_int8", "preprocessor_int8",
     "ggml_tmac_init", "ggml_tmac_free", "ggml_tmac_mul_mat_task_init", "ggml_tmac_mul_mat_task_compute",
     "ggml_tmac_set_n_threads", "ggml_tmac_get_type_bits", "ggml_tmac_b200_can_mul_mat",
     "ggml_tmac_b200_mul_mat_get_wsize", "ggml_tmac_b200_get_nbytes", "ggml_tmac_b200_transform_tensor",
@@ -88,6 +88,7 @@ def load() -> C.CDLL:
         "tmac_b200_qgemm_lut_grouped": (i, [vp, i, i, i, vp, vp, vp, vp]),
         "tmac_b200_gemv_grouped": (i, [vp, i, i, i, vp, vp]),
         "tmac_b200_gemv_rmsnorm": (i, [vp, i, i, i, vp, vp, C.c_float, vp]),
+        "tmac_b200_gemv_rmsnorm_bias": (i, [vp, i, i, i, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_gemv_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_gemv_residual": (i, [i64, i, i, vp, vp, vp]),
         "tmac_b200_gemv_subnorm": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_gemv_subnorm_relu2": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
@@ -96,6 +97,7 @@ def load() -> C.CDLL:
         "tmac_b200_prefill_experts": (i, [vp, i, i, i, i, vp, vp, i, vp]),
         "tmac_b200_prefill_experts_glu": (i, [vp, i, i, i, vp, vp, vp, vp, i, vp, vp]),
         "tmac_b200_prefill_rmsnorm": (i, [vp, i, i, i, vp, vp, C.c_float, vp]),
+        "tmac_b200_prefill_rmsnorm_bias": (i, [vp, i, i, i, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_prefill_glu": (i, [i64, i, i, vp, vp, vp, vp]), "tmac_b200_prefill_residual": (i, [i64, i, i, vp, vp, vp]),
         "tmac_b200_prefill_subnorm": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
         "tmac_b200_prefill_subnorm_relu2": (i, [i64, i, i, vp, vp, vp, C.c_float, vp, vp]),
@@ -249,6 +251,16 @@ def gemv_rmsnorm(wts, N, H, w, eps, outs, dtype=F32):
     check(load().tmac_b200_gemv_rmsnorm(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), O), "tmac_b200_gemv_rmsnorm")
 
 
+def gemv_rmsnorm_bias(wts, N, H, w, eps, bias, outs, dtype=F32):
+    """gemv_rmsnorm plus a bias on each tensor's outputs, outs[i] = gemv_rmsnorm's row + bias[i] rounded once (Qwen2's q/k/v;
+    tmac_b200_gemv_rmsnorm_bias).  bias: len(wts) device fp32 [Mout] vectors, 16-byte aligned."""
+    n = len(wts)
+    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
+    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
+    Bs = None if bias is None else (C.c_void_p * n)(*[ptr(b) for b in bias])
+    check(load().tmac_b200_gemv_rmsnorm_bias(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), Bs, O), "tmac_b200_gemv_rmsnorm_bias")
+
+
 def gemv_glu(wt: Weights, N, G, U, Cout, R=None, dtype=F32):
     """Cout = gemv(wt, silu(G) * U) (+ R), the down projection of a SwiGLU FFN and its residual add (device tensors)."""
     check(load().tmac_b200_gemv_glu(wt.handle, N, dtype, ptr(G), ptr(U), ptr(R), ptr(Cout)), "tmac_b200_gemv_glu")
@@ -321,6 +333,15 @@ def prefill_rmsnorm(wts, N, H, w, eps, outs, dtype=F32):
     Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
     O = (C.c_void_p * n)(*[ptr(x) for x in outs])
     check(load().tmac_b200_prefill_rmsnorm(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), O), "tmac_b200_prefill_rmsnorm")
+
+
+def prefill_rmsnorm_bias(wts, N, H, w, eps, bias, outs, dtype=F32):
+    """gemv_rmsnorm_bias's arguments and output, run on the prefill tiles (tmac_b200_prefill_rmsnorm_bias)."""
+    n = len(wts)
+    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
+    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
+    Bs = None if bias is None else (C.c_void_p * n)(*[ptr(b) for b in bias])
+    check(load().tmac_b200_prefill_rmsnorm_bias(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), Bs, O), "tmac_b200_prefill_rmsnorm_bias")
 
 
 def prefill_glu(wt: Weights, N, G, U, Cout, R=None, dtype=F32):

@@ -6,11 +6,15 @@ resident together and timed alternately, best of `--rounds`; the kernel serving 
 and so are the card's name, power limit and max SM clock.  With `--bitnet` the layers are BitNet-3B's (26 layers, hidden 3200,
 FFN 8640, 32 heads; ternary one-scale tensors with activation groups of 64, and the attn / ffn sub-norms), timed in the modes
 "off" and "fused_ops".  With `--bitnet2b` they are BitNet b1.58 2B4T's (30 layers, hidden 2560, FFN 6912, 20 query heads and 5 KV
-heads of 128, the squared-ReLU FFN: ffn_act="relu2", kv_heads=5), in the same two modes.
+heads of 128, the squared-ReLU FFN: ffn_act="relu2", kv_heads=5), in the same two modes.  With `--qwen2` they are Qwen2-7B's (28
+layers, hidden 3584, FFN 18944, 28 query heads and 4 KV heads of 128, W4 g128 with zero points, a bias on q/k/v: kv_heads=4,
+qkv_bias=True), in the same two modes, plus one line that times the stacked q/k/v tensor (4608 x 3584) of every layer at N = 1 as
+gemv_rmsnorm followed by a torch add of the bias against gemv_rmsnorm_bias (CUDA-graphed, alternated, us per layer).
 
     python tools/layer_bench.py [--layers 32] [--reps 20] [--rounds 3] [--formats w2zp,w4]
     python tools/layer_bench.py --bitnet [--layers 26] [...]
     python tools/layer_bench.py --bitnet2b [--layers 30] [...]
+    python tools/layer_bench.py --qwen2 [--layers 28] [...]
     python tools/layer_bench.py --profile [...]     # kernels per token of each mode (torch.profiler, one eager step; no timing)
 """
 import argparse
@@ -31,22 +35,29 @@ MODES = {"off": {}, "ffn_sequence": {"ffn_sequence": True}, "post_attn_sequence"
          "fused_ops": {"fused_ops": True}}
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=None, help="default 32, 26 with --bitnet, 30 with --bitnet2b")
+ap.add_argument("--layers", type=int, default=None, help="default 32, 26 with --bitnet, 30 with --bitnet2b, 28 with --qwen2")
 ap.add_argument("--reps", type=int, default=20)
 ap.add_argument("--rounds", type=int, default=3)
 ap.add_argument("--formats", default="w2zp,w4")
 ap.add_argument("--profile", action="store_true", help="count the kernels of one token step per mode instead of timing")
 ap.add_argument("--bitnet", action="store_true", help="BitNet-3B layers with sub-norms, modes off and fused_ops")
 ap.add_argument("--bitnet2b", action="store_true", help="BitNet b1.58 2B4T layers (relu2 FFN, 5 KV heads), modes off and fused_ops")
+ap.add_argument("--qwen2", action="store_true", help="Qwen2-7B layers (W4 g128 zp, 4 KV heads, q/k/v biases), modes off and fused_ops")
 args = ap.parse_args()
-if args.bitnet or args.bitnet2b:
+if args.qwen2:
+    qwen = dict(kv_heads=4, qkv_bias=True)
+    HIDDEN, FFN, HEADS = 3584, 18944, 28
+    args.formats = "qwen2_w4g128zp"
+    FORMATS = {args.formats: (4, True)}
+    MODES = {"off": qwen, "fused_ops": dict(qwen, fused_ops=True)}
+elif args.bitnet or args.bitnet2b:
     sub = dict(sub_norms=True, ffn_act="relu2", kv_heads=5) if args.bitnet2b else dict(sub_norms=True)
     HIDDEN, FFN, HEADS = (2560, 6912, 20) if args.bitnet2b else (3200, 8640, 32)
     args.formats = "bitnet2b" if args.bitnet2b else "bitnet"
     FORMATS = {args.formats: (2, False)}
     MODES = {"off": sub, "fused_ops": dict(sub, fused_ops=True)}
 if args.layers is None:
-    args.layers = 30 if args.bitnet2b else 26 if args.bitnet else 32
+    args.layers = 28 if args.qwen2 else 30 if args.bitnet2b else 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("layer_bench.py needs a CUDA device")
@@ -84,6 +95,30 @@ def kernels_per_token(m):
     return {"kernels": len(kern), "library_kernels": sum("tmac_b200::" in n for n in kern), "memcpy_memset": len(names) - len(kern)}
 
 
+def qkv_bias_pair(m):
+    """Every layer's stacked q/k/v tensor at N = 1: gemv_rmsnorm then a torch add of the bias, against gemv_rmsnorm_bias; each a CUDA
+    graph over the layers, alternated, best of --rounds.  The two outputs of the last layer must be equal bit for bit (F32)."""
+    lays = m.layers
+    x = torch.randn((1, HIDDEN), device="cuda")
+    outs = {k: torch.zeros((1, lays[0].lin["qkv"].mout), device="cuda") for k in ("add", "bias")}
+
+    def add():
+        for l in lays:
+            tb.gemv_rmsnorm([l.lin["qkv"].wt], 1, x, l.norm1, l.EPS, [outs["add"]])
+            outs["add"].add_(l.qkv_b["qkv"])
+
+    def bias():
+        for l in lays:
+            tb.gemv_rmsnorm_bias([l.lin["qkv"].wt], 1, x, l.norm1, l.EPS, [l.qkv_b["qkv"]], [outs["bias"]])
+    graphs = {"gemv_rmsnorm_plus_add": m._graph(add, st), "gemv_rmsnorm_bias": m._graph(bias, st)}
+    us = {k: float("inf") for k in graphs}
+    for _ in range(args.rounds):
+        for k, g in graphs.items():
+            us[k] = min(us[k], 1e6 / m._per_s(g.replay, st, args.reps) / len(lays))
+    return {"qkv_bias_N1": {"rows": lays[0].lin["qkv"].mout, "K": HIDDEN, "us_per_layer": {k: round(v, 2) for k, v in us.items()},
+                            "bit_equal": bool(torch.equal(outs["add"], outs["bias"]))}}
+
+
 def case(fmt):
     bits, zp = FORMATS[fmt]
     res = {"format": fmt, "layers": args.layers, "ctx": CTX}
@@ -96,6 +131,8 @@ def case(fmt):
         if args.profile:
             res["per_token"] = {mode: kernels_per_token(m) for mode, m in models.items()}
             return res
+        if args.qwen2:
+            res.update(qkv_bias_pair(models["fused_ops"]))
         for m in models.values():
             m.capture(st)
         runs = {mode: [] for mode in models}

@@ -24,8 +24,14 @@ prefill_rmsnorm([gate, up]), prefill_subnorm(down, + h), and gemv_io their gemv_
 --bitnet2b: BitNet b1.58 2B4T instead (hidden 2560, FFN 6912, 20 query heads and 5 KV heads of 128, `--layers` 30, the squared-ReLU
 FFN), in the same three forms: q/k/v are one stacked tensor, and the down projection is prefill_subnorm_relu2 (gemv_subnorm_relu2).
 
+--qwen2: Qwen2-7B instead (hidden 3584, FFN 18944, 28 query heads and 4 KV heads of 128, W4 g128 with zero points, `--layers` 28,
+a bias on q/k/v), in the same three forms: q/k/v are one stacked tensor (4608 rows) run by prefill_rmsnorm_bias (gemv_rmsnorm_bias).
+Then one line timing that tensor of every layer at N = 256 as prefill_rmsnorm followed by a torch add of the bias against
+prefill_rmsnorm_bias (graphed, alternated).
+
     python tools/prompt_bench.py --bitnet [--layers 26] [--ps 16,32,64,128,512] [--gemv-max 128]
     python tools/prompt_bench.py --bitnet2b [--layers 30] [--ps 16,32,64,128,512] [--gemv-max 128]
+    python tools/prompt_bench.py --qwen2 [--layers 28] [--ps 16,32,64,128,512] [--gemv-max 128]
 """
 import argparse
 import contextlib
@@ -46,11 +52,13 @@ LLAMA = dict(hidden=4096, ffn=11008, heads=32)
 MIXTRAL = dict(hidden=4096, ffn=14336, heads=32, experts=8, topk=2)
 BITNET = dict(hidden=3200, ffn=8640, heads=32, bits=2, zero_point=False, sub_norms=True)
 BITNET2B = dict(hidden=2560, ffn=6912, heads=20, kv_heads=5, bits=2, zero_point=False, sub_norms=True, ffn_act="relu2")
+QWEN2 = dict(hidden=3584, ffn=18944, heads=28, kv_heads=4, bits=4, zero_point=True, qkv_bias=True)
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--layers", type=int, default=None, help="decoder layers (default 32, BitNet-3B 26, BitNet b1.58 2B4T 30)")
+ap.add_argument("--layers", type=int, default=None, help="decoder layers (default 32, BitNet-3B 26, BitNet b1.58 2B4T 30, Qwen2-7B 28)")
 ap.add_argument("--bitnet", action="store_true", help="BitNet-3B's prompt step instead of Llama-2-7B and Mixtral-8x7B")
 ap.add_argument("--bitnet2b", action="store_true", help="BitNet b1.58 2B4T's prompt step instead of Llama-2-7B and Mixtral-8x7B")
+ap.add_argument("--qwen2", action="store_true", help="Qwen2-7B's prompt step instead of Llama-2-7B and Mixtral-8x7B")
 ap.add_argument("--moe-layers", type=int, default=8)
 ap.add_argument("--ps", default="16,32,64,128,512")
 ap.add_argument("--moe-ps", default="64,512")
@@ -60,7 +68,7 @@ ap.add_argument("--reps", type=int, default=5)
 ap.add_argument("--rounds", type=int, default=3)
 args = ap.parse_args()
 if args.layers is None:
-    args.layers = 30 if args.bitnet2b else 26 if args.bitnet else 32
+    args.layers = 28 if args.qwen2 else 30 if args.bitnet2b else 26 if args.bitnet else 32
 
 if not torch.cuda.is_available():
     sys.exit("prompt_bench.py needs a CUDA device")
@@ -81,7 +89,7 @@ def card():
 @contextlib.contextmanager
 def gemv_forms():
     """The harness's prefill_* calls swapped for their gemv_* forms, which take the same arguments."""
-    names = {"prefill_rmsnorm": tb.gemv_rmsnorm, "prefill_residual": tb.gemv_residual, "prefill_glu": tb.gemv_glu,
+    names = {"prefill_rmsnorm": tb.gemv_rmsnorm, "prefill_rmsnorm_bias": tb.gemv_rmsnorm_bias, "prefill_residual": tb.gemv_residual, "prefill_glu": tb.gemv_glu,
              "prefill_subnorm": tb.gemv_subnorm, "prefill_subnorm_relu2": tb.gemv_subnorm_relu2, "prefill_experts": tb.gemv_experts, "prefill_experts_glu": tb.gemv_experts_glu}
     saved = {n: getattr(decode_harness.tb, n) for n in names}
     for n, f in names.items():
@@ -155,8 +163,31 @@ def prompt_fn(m, P, x, linear=None):
     return run
 
 
+def qkv_bias_pair(m, P):
+    """Every layer's stacked q/k/v tensor at N = P: prefill_rmsnorm then a torch add of the bias, against prefill_rmsnorm_bias, graphed
+    and alternated.  The two outputs of the last layer must be equal bit for bit (F32, the same tile)."""
+    lays = m.layers
+    x = torch.randn((P, m.hidden), device="cuda")
+    outs = {k: torch.zeros((P, lays[0].lin["qkv"].mout), device="cuda") for k in ("add", "bias")}
+
+    def add():
+        for l in lays:
+            tb.prefill_rmsnorm([l.lin["qkv"].wt], P, x, l.norm1, l.EPS, [outs["add"]])
+            outs["add"].add_(l.qkv_b["qkv"])
+
+    def bias():
+        for l in lays:
+            tb.prefill_rmsnorm_bias([l.lin["qkv"].wt], P, x, l.norm1, l.EPS, [l.qkv_b["qkv"]], [outs["bias"]])
+    ms = best({"prefill_rmsnorm_plus_add": graph(add), "prefill_rmsnorm_bias": graph(bias)})
+    print(json.dumps({"model": "qwen2_7b", "qkv_bias_P": P, "rows": lays[0].lin["qkv"].mout, "K": m.hidden,
+                      "us_per_layer": {k: round(v * 1e3 / len(lays), 2) for k, v in ms.items()},
+                      "bit_equal": bool(torch.equal(outs["add"], outs["bias"]))}), flush=True)
+
+
 def dense_model(fmt, ps):
-    if fmt in ("bitnet", "bitnet2b"):
+    if fmt == "qwen2":
+        m = DecodeModel(args.layers, ctx=512, fused_ops=True, prompt_len=max(ps), **QWEN2)
+    elif fmt in ("bitnet", "bitnet2b"):
         m = DecodeModel(args.layers, ctx=512, fused_ops=True, prompt_len=max(ps), **(BITNET2B if fmt == "bitnet2b" else BITNET))
     else:
         bits, zp = FORMATS[fmt]
@@ -170,9 +201,10 @@ def dense_model(fmt, ps):
                 with gemv_forms():
                     graphs["gemv_io"] = graph(forms["prefill"])
             ms = best(graphs)
-            if fmt in ("bitnet", "bitnet2b"):
+            if fmt in ("bitnet", "bitnet2b", "qwen2"):
                 share = library_share(forms["prefill"])
-                print(json.dumps({"model": "bitnet_b1_58_2b4t" if fmt == "bitnet2b" else "bitnet_b1_58_3b", "format": "w2_one_scale_a64", "layers": args.layers, "P": P,
+                model = {"bitnet2b": "bitnet_b1_58_2b4t", "bitnet": "bitnet_b1_58_3b", "qwen2": "qwen2_7b"}[fmt]
+                print(json.dumps({"model": model, "format": "w4_g128_zp" if fmt == "qwen2" else "w2_one_scale_a64", "layers": args.layers, "P": P,
                                   "ms_per_prompt": {k: round(v, 3) for k, v in ms.items()},
                                   "prompt_tokens_per_s": {k: round(P * 1e3 / v, 1) for k, v in ms.items()},
                                   "prefill_linears_share": round(share, 3)}), flush=True)
@@ -197,6 +229,8 @@ def dense_model(fmt, ps):
             print(json.dumps(res), flush=True)
             del graphs, grouped, single
             torch.cuda.synchronize()
+        if fmt == "qwen2":
+            qkv_bias_pair(m, 256)
     finally:
         m.free()
 
@@ -221,8 +255,8 @@ def moe_model(fmt, ps):
 
 
 print(json.dumps({"card": card()}), flush=True)
-if args.bitnet or args.bitnet2b:
-    dense_model("bitnet2b" if args.bitnet2b else "bitnet", [int(p) for p in args.ps.split(",")])
+if args.qwen2 or args.bitnet or args.bitnet2b:
+    dense_model("qwen2" if args.qwen2 else "bitnet2b" if args.bitnet2b else "bitnet", [int(p) for p in args.ps.split(",")])
 else:
     for fmt in args.formats.split(","):
         dense_model(fmt, [int(p) for p in args.ps.split(",")])
