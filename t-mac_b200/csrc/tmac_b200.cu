@@ -411,7 +411,7 @@ int launch_gemv3(const Resident &R, int row_begin, int row_end, int N, const Gem
     const size_t wregion = std::max((size_t)p.wpc * (p.nbuf * L.blk + (size_t)L.qch * 4 * (sym ? 8 : 16)), (size_t)p.wpc * L.rsb * 4);
     size_t smem = (size_t)p.cs * L.rsb * 4 + ((wregion + 15) & ~(size_t)15) + (size_t)p.wpc * 16;   // + warp-private mbarriers
     if (in.kind != kInTable && L.int_path()) { p.ioff = (int)smem; smem += (size_t)(L.K / 32 + kG3MaxWarps + 4 + 8) * 4; }   // row scan: block sums, warp maxima, bias, cluster maxima
-    if (in.kind == kInNorm || in.kind == kInGluNorm || in.kind == kInRelu2Norm || in.kind == kInNormBias) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
+    if (in_norm(in.kind)) { p.ioff = (int)smem; smem += (size_t)(L.K + 4) * 4; }   // the norm's row in fp32, then inv
     if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     uint32_t wtx, wty;
     plane_weight_regs(L.bits, sym, &wtx, &wty);
@@ -1289,186 +1289,181 @@ int tmac_b200_gemv_grouped(const int64_t *handles, int count, int N, int dtype, 
     return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kInRow, B, dtype == TMAC_B200_F16), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
 }
 
-// The checks both forms of the transformed-input calls share (tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2
-// and tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2): the arguments, the call's own (io_call_check), then that A, C[count] and every U, w
-// and R given are device pointers.
-static int io_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *A, const Gemv3Io &io,
-                    void *const *C) {
-    if (!handles || count <= 0 || count > 65535 || !A || !C || N <= 0 || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
+// What a transformed-input call computes (tmac_b200_gemv_* and tmac_b200_prefill_* of rmsnorm, rmsnorm_bias, glu, residual,
+// subnorm and subnorm_relu2, and of the routed experts), filled in by its entry points and read by both of its forms: the input row
+// is A, or gate(A, U) when the call has a gate; then its RMS norm with w and eps when it has a norm.  Its output C[i] takes R when R
+// is given (required when needs_R), or bias[i] when it has a bias.  Routed calls pick each slot's tensor from the count * n_experts
+// tensors of handles by ids, topk slots per token; the GLU form combines the slots' rows with wts.
+struct IoCall {
+    const char *name;                              // the call without its form, as messages name it
+    const int64_t *handles;
+    int count, N, dtype;
+    const void *A;
+    void *const *C;
+    int gate = kGateNone;                          // kGateSilu / kGateRelu2: gate(A, U) with the second input U
+    const void *U = nullptr;
+    bool norm = false;
+    const float *w = nullptr;                      // norm: fp32 [K], 16-byte aligned
+    float eps = 0.f;
+    bool needs_R = false;
+    const void *R = nullptr;
+    bool bias = false;
+    const float *const *biasv = nullptr;           // bias: count fp32 [Mout], 16-byte aligned
+    bool routed = false;
+    const int32_t *ids = nullptr;                  // routed: [N][topk]
+    const float *wts = nullptr;                    // routed with a gate: [N][topk]
+    int topk = 1, n_experts = 1;
+    IoCall(const char *name, const int64_t *handles, int count, int N, int dtype, const void *A, void *const *C)
+        : name(name), handles(handles), count(count), N(N), dtype(dtype), A(A), C(C) {}
+};
+
+// Every argument check of both forms of the calls IoCall describes (form: "gemv" or "prefill").
+static int io_check(const std::string &form, const IoCall &c) {
+    const std::string what = form + "_" + c.name;
+    if (c.gate == kGateRelu2 && !c.U) return fail(what + ": U must not be null (" + form + "_subnorm is the call for the attn sub-norm)");
+    if (c.needs_R && !c.R) return fail(what + ": R must not be null");
+    if (c.norm) {
+        if (!c.w || ((uintptr_t)c.w & 15)) return fail(what + ": w must be a 16-byte aligned device vector");
+        if (!(c.eps >= 0.f) || !std::isfinite(c.eps)) return fail(what + ": eps must be finite and >= 0");
+    }
+    if (!c.handles || c.count <= 0 || c.N <= 0 || !c.A || !c.C || (c.gate != kGateNone && !c.U) ||
+        (c.dtype != TMAC_B200_F32 && c.dtype != TMAC_B200_F16) ||
+        (c.routed ? c.n_experts <= 0 || !c.ids || (c.gate != kGateNone && (!c.wts || !c.C[0])) : c.count > 65535))
         return fail(what + ": bad arguments");
-    if (!is_device_ptr(A) || (io.act2 && !is_device_ptr(io.act2)) || (io.nw && !is_device_ptr(io.nw)) || (io.res && !is_device_ptr(io.res)))
+    if (c.routed) {
+        if (c.topk < 1 || c.topk > 8) return fail(what + ": topk must be 1..8");
+        if ((long long)c.count * c.n_experts > 65535) return fail(what + ": count * n_experts must be <= 65535");
+    }
+    if (!is_device_ptr(c.A) || (c.U && !is_device_ptr(c.U)) || (c.w && !is_device_ptr(c.w)) || (c.R && !is_device_ptr(c.R)) ||
+        (c.ids && !is_device_ptr(c.ids)) || (c.wts && !is_device_ptr(c.wts)))
         return fail(what + ": device pointers only");
-    for (int i = 0; i < count; ++i)
-        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
-    return 0;
-}
-// U and R: gemv_subnorm's (and gemv_subnorm_relu2's) up rows and residual, or null.
-static int rmsnorm_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const void *H, const float *w,
-                         float eps, void *const *C, Gemv3Io *io, const void *U = nullptr, const void *R = nullptr) {
-    if (!w || ((uintptr_t)w & 15)) return fail(what + ": w must be a 16-byte aligned device vector");
-    if (!(eps >= 0.f) || !std::isfinite(eps)) return fail(what + ": eps must be finite and >= 0");
-    *io = Gemv3Io{};
-    io->nw = w; io->eps = eps; io->act2 = U; io->res = R;
-    return io_check(what, handles, count, N, dtype, H, *io, C);
-}
-static int glu_check(const std::string &what, int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C,
-                     Gemv3Io *io) {
-    if (!U) return fail(what + ": bad arguments");
-    *io = Gemv3Io{};
-    io->act2 = U; io->res = R;
-    return io_check(what, &handle, 1, N, dtype, G, *io, &C);
-}
-static int residual_check(const std::string &what, int64_t handle, int N, int dtype, const void *B, const void *R, void *C, Gemv3Io *io) {
-    if (!R) return fail(what + ": R must not be null");
-    *io = Gemv3Io{};
-    io->res = R;
-    return io_check(what, &handle, 1, N, dtype, B, *io, &C);
-}
-// The biases of tmac_b200_gemv_rmsnorm_bias / tmac_b200_prefill_rmsnorm_bias, after rmsnorm_check: count 16-byte aligned device
-// vectors fp32 [Mout] (Mout of handles[0]; the geometry check follows) that overlap no C[i] ([N][Mout] of dtype).
-static int bias_check(const std::string &what, const int64_t *handles, int count, int N, int dtype, const float *const *bias, void *const *C) {
-    if (!bias) return fail(what + ": bias must not be null");
-    auto it = g.res.find(handles[0]);
+    for (int i = 0; i < c.count; ++i)
+        if (!is_device_ptr(c.C[i])) return fail(what + ": device pointers only");
+    if (!c.bias) return 0;
+    // count fp32 [Mout] vectors (Mout of handles[0]; grouped_setup checks the geometry) that overlap no C[j] ([N][Mout] of dtype)
+    if (!c.biasv) return fail(what + ": bias must not be null");
+    auto it = g.res.find(c.handles[0]);
     if (it == g.res.end()) return fail(what + ": bad weight handle");
-    const size_t bb = (size_t)it->second.L.Mout * sizeof(float), cb = (size_t)N * it->second.L.Mout * (dtype == TMAC_B200_F16 ? 2 : 4);
-    for (int i = 0; i < count; ++i) {
-        if (!bias[i] || ((uintptr_t)bias[i] & 15) || !is_device_ptr(bias[i])) return fail(what + ": each bias must be a 16-byte aligned device vector");
-        const uintptr_t b0 = (uintptr_t)bias[i];
-        for (int j = 0; j < count; ++j) {
-            const uintptr_t c0 = (uintptr_t)C[j];
+    const size_t bb = (size_t)it->second.L.Mout * sizeof(float), cb = (size_t)c.N * it->second.L.Mout * (c.dtype == TMAC_B200_F16 ? 2 : 4);
+    for (int i = 0; i < c.count; ++i) {
+        if (!c.biasv[i] || ((uintptr_t)c.biasv[i] & 15) || !is_device_ptr(c.biasv[i]))
+            return fail(what + ": each bias must be a 16-byte aligned device vector");
+        const uintptr_t b0 = (uintptr_t)c.biasv[i];
+        for (int j = 0; j < c.count; ++j) {
+            const uintptr_t c0 = (uintptr_t)c.C[j];
             if (b0 < c0 + cb && c0 < b0 + bb) return fail(what + ": a bias must not overlap an output");
         }
     }
     return 0;
 }
 
-// tmac_b200_gemv_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the
-// gemv3_kernel whose input A is transformed in the LUT build (kind) and whose output takes io.res, or (kInNormBias) the biases
-// bias[count] through the pointer table.  The arguments are checked.
-static int gemv_io(const std::string &what, const int64_t *handles, int count, int N, int dtype, int kind, const void *A,
-                   Gemv3Io io, void *const *C, const float *const *bias = nullptr) {
+// The gemv3_kernel input kind of a call: the one whose properties are the call's.
+static int io_kind(const IoCall &c) {
+    for (int k = kInRow; k <= kInNormBias; ++k)
+        if (in_experts(k) == c.routed && in_gate(k) == c.gate && in_norm(k) == c.norm && in_bias(k) == c.bias) return k;
+    return -1;
+}
+
+// The gemv_* form: tmac_b200_gemv_grouped's launch (same decomposition, so the same sums) of the gemv3_kernel of the call's kind, whose
+// input is built in the LUT build.  Routed calls launch count * topk slots (so each slot's sums are those of gemv_grouped at
+// N * count * topk) with a pointer table of every tensor, count * n_experts entries.  Everything is checked before anything is launched.
+static int gemv_io(const IoCall &c) {
+    const std::string what = std::string("gemv_") + c.name;
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count, nullptr, nullptr, nullptr, C, &R, &bp, 1, bias)) return -1;
-    io.biasv = bp.bias;
-    const StreamLayout &L = R->L;
-    if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
-    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kind, A, dtype == TMAC_B200_F16, io), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
-}
-
-int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
-                           void *const *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    Gemv3Io io;
-    if (rmsnorm_check("gemv_rmsnorm", handles, count, N, dtype, H, w, eps, C, &io)) return -1;
-    return gemv_io("gemv_rmsnorm", handles, count, N, dtype, kInNorm, H, io, C);
-}
-
-int tmac_b200_gemv_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
-                                const float *const *bias, void *const *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    const std::string what = "gemv_rmsnorm_bias";
-    Gemv3Io io;
-    if (rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io) || bias_check(what, handles, count, N, dtype, bias, C)) return -1;
-    return gemv_io(what, handles, count, N, dtype, kInNormBias, H, io, C, bias);
-}
-
-int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    Gemv3Io io;
-    if (glu_check("gemv_glu", handle, N, dtype, G, U, R, C, &io)) return -1;
-    return gemv_io("gemv_glu", &handle, 1, N, dtype, kInGlu, G, io, &C);
-}
-
-int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    Gemv3Io io;
-    if (residual_check("gemv_residual", handle, N, dtype, B, R, C, &io)) return -1;
-    return gemv_io("gemv_residual", &handle, 1, N, dtype, kInRow, B, io, &C);
-}
-
-int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps, const void *R,
-                           void *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    Gemv3Io io;
-    if (rmsnorm_check("gemv_subnorm", &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
-    return gemv_io("gemv_subnorm", &handle, 1, N, dtype, U ? kInGluNorm : kInNorm, G, io, &C);
-}
-
-int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
-                                 const void *R, void *C) {
-    std::unique_lock<std::shared_mutex> lk(g_mu);
-    if (ensure_init()) return -1;
-    const std::string what = "gemv_subnorm_relu2";
-    if (!U) return fail(what + ": U must not be null (gemv_subnorm is the call for the attn sub-norm)");
-    Gemv3Io io;
-    if (rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
-    return gemv_io(what, &handle, 1, N, dtype, kInRelu2Norm, G, io, &C);
-}
-
-// The checks both routed-expert call forms share (tmac_b200_gemv_experts / _glu and tmac_b200_prefill_experts / _glu): the
-// arguments, then that A, ids, C[count] and every U, weights and R given are device pointers.
-static int experts_check(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
-                         const void *A, const void *U, const int32_t *ids, const float *wts, const void *R, void *const *C) {
-    if (!handles || count <= 0 || n_experts <= 0 || N <= 0 || !A || !ids || !C || (dtype != TMAC_B200_F32 && dtype != TMAC_B200_F16))
-        return fail(what + ": bad arguments");
-    if (topk < 1 || topk > 8) return fail(what + ": topk must be 1..8");
-    if ((long long)count * n_experts > 65535) return fail(what + ": count * n_experts must be <= 65535");
-    if (!is_device_ptr(A) || !is_device_ptr(ids) || (U && !is_device_ptr(U)) || (wts && !is_device_ptr(wts)) || (R && !is_device_ptr(R)))
-        return fail(what + ": device pointers only");
-    for (int i = 0; i < count; ++i)
-        if (!is_device_ptr(C[i])) return fail(what + ": device pointers only");
-    return 0;
-}
-
-// tmac_b200_gemv_experts / _glu: the launch of tmac_b200_gemv_grouped over count * topk slots (so each slot's sums are those of
-// gemv_grouped at N * count * topk), with a pointer table of every tensor, count * n_experts entries, from which each slot picks its
-// tensor by the id it reads on the device.  Everything is checked before anything is launched.
-static int gemv_experts(const std::string &what, const int64_t *handles, int count, int n_experts, int N, int dtype, int topk,
-                        int kind, const void *A, Gemv3Io io, void *const *C) {
-    const Resident *R = nullptr;
-    BatchPtrs bp;
-    if (experts_check(what, handles, count, n_experts, N, dtype, topk, A, io.act2, io.ids, io.wts, io.res, C) ||
-        grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, C, &R, &bp, n_experts))
+    if (io_check("gemv", c) ||
+        grouped_setup(what.c_str(), c.handles, c.count * c.n_experts, nullptr, nullptr, nullptr, c.C, &R, &bp, c.n_experts, c.biasv))
         return -1;
     const StreamLayout &L = R->L;
     if (L.int_path() || L.act_group_size > L.ck) return fail(what + ": fp-path tensors with the activation group inside a chunk only");
-    bp.n = count * topk;                           // grid.z: the slots
-    io.topk = topk; io.n_experts = n_experts;
+    const int kind = io_kind(c);
+    Gemv3Io io{};
+    io.act2 = c.U; io.nw = c.w; io.eps = c.eps; io.res = c.R; io.ids = c.ids; io.wts = c.wts; io.biasv = bp.bias;
+    if (c.routed) {
+        bp.n = c.count * c.topk;                   // grid.z: the slots
+        io.topk = c.topk; io.n_experts = c.n_experts;
+    }
     if (kind == kInExpertsGlu) {
-        const size_t cnt_bytes = (size_t)N * ((L.Mout + L.rsb - 1) / L.rsb) * sizeof(unsigned);
-        if (g.d_moe_ws.ensure((size_t)N * topk * L.Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
+        const size_t cnt_bytes = (size_t)c.N * ((L.Mout + L.rsb - 1) / L.rsb) * sizeof(unsigned);
+        if (g.d_moe_ws.ensure((size_t)c.N * c.topk * L.Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
         if (g.d_moe_cnt.cap < cnt_bytes) {
             if (g.d_moe_cnt.ensure(cnt_bytes)) return fail(what + ": out of device memory (workspace)");
             CUDA_OK(cudaMemsetAsync(g.d_moe_cnt.p, 0, g.d_moe_cnt.cap, g.stream()));
         }
         io.ws = (float *)g.d_moe_ws.p; io.cnt = (unsigned *)g.d_moe_cnt.p;
     }
-    return launch_gemv3(*R, 0, L.Mout, N, Gemv3In::rows(kind, A, dtype == TMAC_B200_F16, io), nullptr, L.Mout, 0, dtype == TMAC_B200_F16, &bp);
+    const int f16 = c.dtype == TMAC_B200_F16;
+    return launch_gemv3(*R, 0, L.Mout, c.N, Gemv3In::rows(kind, c.A, f16, io), nullptr, L.Mout, 0, f16, &bp);
+}
+
+int tmac_b200_gemv_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                           void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("rmsnorm", handles, count, N, dtype, H, C);
+    c.norm = true; c.w = w; c.eps = eps;
+    return gemv_io(c);
+}
+
+int tmac_b200_gemv_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
+                                const float *const *bias, void *const *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("rmsnorm_bias", handles, count, N, dtype, H, C);
+    c.norm = true; c.w = w; c.eps = eps; c.bias = true; c.biasv = bias;
+    return gemv_io(c);
+}
+
+int tmac_b200_gemv_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("glu", &handle, 1, N, dtype, G, &C);
+    c.gate = kGateSilu; c.U = U; c.R = R;
+    return gemv_io(c);
+}
+
+int tmac_b200_gemv_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("residual", &handle, 1, N, dtype, B, &C);
+    c.needs_R = true; c.R = R;
+    return gemv_io(c);
+}
+
+int tmac_b200_gemv_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps, const void *R,
+                           void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("subnorm", &handle, 1, N, dtype, G, &C);
+    c.gate = U ? kGateSilu : kGateNone; c.U = U; c.norm = true; c.w = w; c.eps = eps; c.R = R;
+    return gemv_io(c);
+}
+
+int tmac_b200_gemv_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
+                                 const void *R, void *C) {
+    std::unique_lock<std::shared_mutex> lk(g_mu);
+    if (ensure_init()) return -1;
+    IoCall c("subnorm_relu2", &handle, 1, N, dtype, G, &C);
+    c.gate = kGateRelu2; c.U = U; c.norm = true; c.w = w; c.eps = eps; c.R = R;
+    return gemv_io(c);
 }
 
 int tmac_b200_gemv_experts(const int64_t *handles, int count, int n_experts, int N, int dtype, const void *B, const int32_t *ids,
                            int topk, void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    Gemv3Io io{};
-    io.ids = ids;
-    return gemv_experts("gemv_experts", handles, count, n_experts, N, dtype, topk, kInExperts, B, io, C);
+    IoCall c("experts", handles, count, N, dtype, B, C);
+    c.routed = true; c.ids = ids; c.topk = topk; c.n_experts = n_experts;
+    return gemv_io(c);
 }
 
 int tmac_b200_gemv_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
                                const int32_t *ids, const float *weights, int topk, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    if (!U || !weights || !C) return fail("gemv_experts_glu: bad arguments");
-    Gemv3Io io{};
-    io.act2 = U; io.ids = ids; io.wts = weights; io.res = R;
-    return gemv_experts("gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, kInExpertsGlu, G, io, &C);
+    IoCall c("experts_glu", handles, 1, N, dtype, G, &C);
+    c.routed = true; c.gate = kGateSilu; c.U = U; c.ids = ids; c.wts = weights; c.topk = topk; c.n_experts = n_experts; c.R = R;
+    return gemv_io(c);
 }
 
 // The tile of a routed launch: the fp16 tile when it is on and the average expert fills one of its 256-token tiles,
@@ -1483,44 +1478,44 @@ static int refuse_peer(const std::string &what) {
     return fail(what + ": peer outputs are for N = 1 single-tensor launches");
 }
 
-// The routed tile launch of the prefill-sized calls, their arguments checked by the caller.  Routed experts (ids != null): route the
-// slots on the device (pf_route_kernel).  The dense forms (ids == null, n_experts = topk = 1): the identity routing, one table entry
-// per token tile.  Then build the LUT of every input row once (B's N rows; U != null: the N * topk rows swiglu(A[s], U[s]), or
-// relu2(A[s], U[s]) when relu2; nw != null:
-// the N rows rms_scale(A[n], inv_n, nw); both: the RMS norm of the SwiGLU rows, all materialised in fp32), gather each table entry's LUT records and run the routed tile over
-// (row tiles, table entries, count).  wts != null (the GLU experts): the tile stores the slots' fp32 rows and the combine adds them
-// (+ R); otherwise the tile adds R (when not null) in its epilogue.  bias != null (prefill_rmsnorm_bias; no R, no wts): the BIAS
-// tiles add bias[i] to tensor i's outputs.  Everything is checked and every workspace allocated before anything is launched.
-static int prefill_routed(const std::string &what, const std::string &gemv_name, const int64_t *handles, int count, int n_experts,
-                          int N, int dtype, int topk, const void *A, const void *U, const float *nw, float eps, const int32_t *ids,
-                          const float *wts, const void *Rres, void *const *C, bool relu2 = false, const float *const *bias = nullptr) {
-    const bool combine = wts != nullptr, slot_rows = U != nullptr;   // slot_rows: one input row per slot (GLU), else per token
+// The prefill_* form: the routed tile launch.  Routed calls: route the slots on the device (pf_route_kernel).  The others: the
+// identity routing (one expert, topk = 1), one table entry per token tile.  Then build the LUT of every input row once (A's N rows;
+// a gate: the N * topk rows gate(A[s], U[s]), swiglu or relu2; a norm: the N rows rms_scale(A[n], inv_n, w); both: the RMS norm of
+// the gated rows, all materialised in fp32), gather each table entry's LUT records and run the routed tile over (row tiles, table
+// entries, count).  wts (the routed GLU form): the tile stores the slots' fp32 rows and the combine adds them (+ R); otherwise the
+// tile adds R (when not null) in its epilogue, or with a bias the BIAS tiles add bias[i] to tensor i's outputs.  Everything is
+// checked and every workspace allocated before anything is launched.
+static int prefill_io(const IoCall &c) {
+    const std::string what = std::string("prefill_") + c.name;
+    if (refuse_peer(what) || io_check("prefill", c)) return -1;
+    const bool combine = c.wts != nullptr, slot_rows = c.gate != kGateNone;   // slot_rows: one input row per slot (GLU), else per token
+    const int N = c.N, topk = c.topk, n_experts = c.n_experts, count = c.count;
     if (n_experts > 256) return fail(what + ": n_experts must be 1..256");   // the routing kernel's shared arrays
-    auto it0 = g.res.find(handles[0]);
+    auto it0 = g.res.find(c.handles[0]);
     if (it0 == g.res.end()) return fail(what + ": bad weight handle");
     const StreamLayout &L = it0->second.L;
     if (!routed_tiles_take(L))
         return fail(what + ": the tiles take W2/W3/W4 fp-path tensors with the act group inside the chunk: per-row scales with K % 128 "
-                    "== 0 (chunk 128/64/32 K), or one scale with act group < K and K % 128 == 0 or 64; use " + gemv_name + " for the others");
-    const int S = N * topk, Mout = L.Mout, K = L.K, f16 = dtype == TMAC_B200_F16;
+                    "== 0 (chunk 128/64/32 K), or one scale with act group < K and K % 128 == 0 or 64; use gemv_" + c.name + " for the others");
+    const int S = N * topk, Mout = L.Mout, K = L.K, f16 = c.dtype == TMAC_B200_F16;
     // combine: the table's C is the slots' fp32 rows, so the workspace is allocated before the table is built
     if (combine && g.d_moe_ws.ensure((size_t)S * Mout * sizeof(float))) return fail(what + ": out of device memory (workspace)");
     const Resident *R = nullptr;
     BatchPtrs bp;
-    if (grouped_setup(what.c_str(), handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : C, &R, &bp, n_experts,
-                      bias))
+    if (grouped_setup(what.c_str(), c.handles, count * n_experts, nullptr, nullptr, nullptr, combine ? &g.d_moe_ws.p : c.C, &R, &bp, n_experts,
+                      c.biasv))
         return -1;
-    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq(), L.one_scale, L.K % 128 != 0, bias != nullptr);
+    const PfExpertKernels fk = pick_pf_experts(L.pb, L.qch, L.agq(), L.one_scale, L.K % 128 != 0, c.bias);
     if (!fk.tile) return fail(what + ": no tile for chunk " + std::to_string(L.ck) + ", act group " + std::to_string(L.act_group_size));
     const TilePlan t(L, false);
     // the tile rule: routed experts as experts_take_tile16, the dense forms as the dense calls (launch_prefill)
-    const bool t16 = (ids ? experts_take_tile16(N, topk, n_experts) : g.use_prefill16 && N >= 64) && t.fits16;
+    const bool t16 = (c.routed ? experts_take_tile16(N, topk, n_experts) : g.use_prefill16 && N >= 64) && t.fits16;
     if (!t16 && !t.fits8) return fail(what + ": the tensor's blocks do not fit the int8 tile's shared memory");
     const int T = t16 ? kP16NT : kPfNT;
     const long long cap = S / T + std::min(n_experts, S);
     if (cap > 65535) return fail(what + ": N * topk too large for one launch");
     const int rows = slot_rows ? S : N, nag = K / L.act_group_size, nsteps = t16 ? t.nmain + t.nextra : t.nmain;
-    const bool act = U || nw;                      // a materialised fp32 input
+    const bool act = c.gate != kGateNone || c.norm;   // a materialised fp32 input
     const size_t recb = t16 ? (size_t)kP16BBytes : t.rec;
     if (g.d_moe_route.ensure((size_t)cap * sizeof(int4) + (size_t)S * sizeof(int)) || (act && g.d_moe_act.ensure((size_t)rows * K * sizeof(float))) ||
         g.d_qlut.ensure((size_t)rows * K * 4) || g.d_ls.ensure((size_t)rows * nag * 4) || g.d_lb.ensure((size_t)rows * nag * 4) ||
@@ -1533,15 +1528,16 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
     unsigned char *recs = (unsigned char *)g.d_tiles.p;
     const cudaStream_t st = g.stream();
 
-    pf_route_launch(ids, S, n_experts, T, (int)cap, tiles, perm, ids && !combine ? bp.C : nullptr, count, Mout, f16, st);
+    pf_route_launch(c.ids, S, n_experts, T, (int)cap, tiles, perm, c.routed && !combine ? bp.C : nullptr, count, Mout, f16, st);
     CUDA_OK(cudaGetLastError());
     if (act) {
-        if (U) pf_swiglu_launch(A, U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st, relu2);
-        if (nw) pf_rmsnorm_launch(U ? g.d_moe_act.p : A, U ? 0 : f16, nw, eps, rows, K, (float *)g.d_moe_act.p, st);   // U: in place
+        if (slot_rows) pf_swiglu_launch(c.A, c.U, f16, (size_t)rows * K, (float *)g.d_moe_act.p, st, c.gate == kGateRelu2);
+        if (c.norm)   // after a gate: in place
+            pf_rmsnorm_launch(slot_rows ? g.d_moe_act.p : c.A, slot_rows ? 0 : f16, c.w, c.eps, rows, K, (float *)g.d_moe_act.p, st);
         CUDA_OK(cudaGetLastError());
         if (launch_preprocessor(K, rows, L.act_group_size, TMAC_B200_F32, g.d_moe_act.p, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
-    } else if (launch_preprocessor(K, rows, L.act_group_size, dtype, A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
-    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts, combine ? nullptr : Rres, bp.bias};
+    } else if (launch_preprocessor(K, rows, L.act_group_size, c.dtype, c.A, (float *)ls, (float *)lb, (int8_t *)qlut)) return -1;
+    const PfRoute route{tiles, perm, bp.W, bp.C, n_experts, combine ? nullptr : c.R, bp.bias};
     const int div = slot_rows ? 1 : topk, out_f16 = combine ? 0 : f16;
     const dim3 grid(t.nrt, (unsigned)cap, count);
     if (t16) {
@@ -1558,7 +1554,7 @@ static int prefill_routed(const std::string &what, const std::string &gemv_name,
         if (launch_tile(false, fk.tile, grid, t, 1, L, S, p, route)) return -1;
     }
     if (combine) {
-        pf_combine_launch((const float *)g.d_moe_ws.p, ids, wts, topk, n_experts, Rres, C[0], N, Mout, f16, st);
+        pf_combine_launch((const float *)g.d_moe_ws.p, c.ids, c.wts, topk, n_experts, c.R, c.C[0], N, Mout, f16, st);
         CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -1568,84 +1564,70 @@ int tmac_b200_prefill_experts(const int64_t *handles, int count, int n_experts, 
                               int topk, void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_experts";
-    if (refuse_peer(what) || experts_check(what, handles, count, n_experts, N, dtype, topk, B, nullptr, ids, nullptr, nullptr, C)) return -1;
-    return prefill_routed(what, "gemv_experts", handles, count, n_experts, N, dtype, topk, B, nullptr, nullptr, 0.f, ids, nullptr, nullptr, C);
+    IoCall c("experts", handles, count, N, dtype, B, C);
+    c.routed = true; c.ids = ids; c.topk = topk; c.n_experts = n_experts;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_experts_glu(const int64_t *handles, int n_experts, int N, int dtype, const void *G, const void *U,
                                   const int32_t *ids, const float *weights, int topk, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_experts_glu";
-    if (!U || !weights || !C) return fail(what + ": bad arguments");
-    if (refuse_peer(what) || experts_check(what, handles, 1, n_experts, N, dtype, topk, G, U, ids, weights, R, &C)) return -1;
-    return prefill_routed(what, "gemv_experts_glu", handles, 1, n_experts, N, dtype, topk, G, U, nullptr, 0.f, ids, weights, R, &C);
+    IoCall c("experts_glu", handles, 1, N, dtype, G, &C);
+    c.routed = true; c.gate = kGateSilu; c.U = U; c.ids = ids; c.wts = weights; c.topk = topk; c.n_experts = n_experts; c.R = R;
+    return prefill_io(c);
 }
 
-// tmac_b200_prefill_rmsnorm / _glu / _residual / _subnorm / _subnorm_relu2: the arguments and checks of the gemv_* form, the launch of the routed tile as one
-// expert with the identity routing.
 int tmac_b200_prefill_rmsnorm(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                               void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_rmsnorm";
-    Gemv3Io io;
-    if (refuse_peer(what) || rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io)) return -1;
-    return prefill_routed(what, "gemv_rmsnorm", handles, count, 1, N, dtype, 1, H, nullptr, w, eps, nullptr, nullptr, nullptr, C);
+    IoCall c("rmsnorm", handles, count, N, dtype, H, C);
+    c.norm = true; c.w = w; c.eps = eps;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_rmsnorm_bias(const int64_t *handles, int count, int N, int dtype, const void *H, const float *w, float eps,
                                    const float *const *bias, void *const *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_rmsnorm_bias";
-    Gemv3Io io;
-    if (refuse_peer(what) || rmsnorm_check(what, handles, count, N, dtype, H, w, eps, C, &io) ||
-        bias_check(what, handles, count, N, dtype, bias, C))
-        return -1;
-    return prefill_routed(what, "gemv_rmsnorm_bias", handles, count, 1, N, dtype, 1, H, nullptr, w, eps, nullptr, nullptr, nullptr, C,
-                          false, bias);
+    IoCall c("rmsnorm_bias", handles, count, N, dtype, H, C);
+    c.norm = true; c.w = w; c.eps = eps; c.bias = true; c.biasv = bias;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_glu(int64_t handle, int N, int dtype, const void *G, const void *U, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_glu";
-    Gemv3Io io;
-    if (refuse_peer(what) || glu_check(what, handle, N, dtype, G, U, R, C, &io)) return -1;
-    return prefill_routed(what, "gemv_glu", &handle, 1, 1, N, dtype, 1, G, U, nullptr, 0.f, nullptr, nullptr, R, &C);
+    IoCall c("glu", &handle, 1, N, dtype, G, &C);
+    c.gate = kGateSilu; c.U = U; c.R = R;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_residual(int64_t handle, int N, int dtype, const void *B, const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_residual";
-    Gemv3Io io;
-    if (refuse_peer(what) || residual_check(what, handle, N, dtype, B, R, C, &io)) return -1;
-    return prefill_routed(what, "gemv_residual", &handle, 1, 1, N, dtype, 1, B, nullptr, nullptr, 0.f, nullptr, nullptr, R, &C);
+    IoCall c("residual", &handle, 1, N, dtype, B, &C);
+    c.needs_R = true; c.R = R;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_subnorm(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps, const void *R,
                               void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_subnorm";
-    Gemv3Io io;
-    if (refuse_peer(what) || rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
-    return prefill_routed(what, "gemv_subnorm", &handle, 1, 1, N, dtype, 1, G, U, w, eps, nullptr, nullptr, R, &C);
+    IoCall c("subnorm", &handle, 1, N, dtype, G, &C);
+    c.gate = U ? kGateSilu : kGateNone; c.U = U; c.norm = true; c.w = w; c.eps = eps; c.R = R;
+    return prefill_io(c);
 }
 
 int tmac_b200_prefill_subnorm_relu2(int64_t handle, int N, int dtype, const void *G, const void *U, const float *w, float eps,
                                     const void *R, void *C) {
     std::unique_lock<std::shared_mutex> lk(g_mu);
     if (ensure_init()) return -1;
-    const std::string what = "prefill_subnorm_relu2";
-    Gemv3Io io;
-    if (refuse_peer(what)) return -1;
-    if (!U) return fail(what + ": U must not be null (prefill_subnorm is the call for the attn sub-norm)");
-    if (rmsnorm_check(what, &handle, 1, N, dtype, G, w, eps, &C, &io, U, R)) return -1;
-    return prefill_routed(what, "gemv_subnorm_relu2", &handle, 1, 1, N, dtype, 1, G, U, w, eps, nullptr, nullptr, R, &C, true);
+    IoCall c("subnorm_relu2", &handle, 1, N, dtype, G, &C);
+    c.gate = kGateRelu2; c.U = U; c.norm = true; c.w = w; c.eps = eps; c.R = R;
+    return prefill_io(c);
 }
 
 int tmac_b200_gemv(int64_t handle, int N, int dtype, const void *B, void *C) {

@@ -519,6 +519,18 @@ struct Gemv3Params {
 // take a per-tensor bias (Qwen2's q/k/v projections).
 enum : int { kInTable = 0, kInRow = 1, kInNorm = 2, kInGlu = 3, kInExperts = 4, kInExpertsGlu = 5, kInGluNorm = 6, kInRelu2Norm = 7,
              kInNormBias = 8 };
+// What each kind does.  The kernel, its launch and the host's choice of kind for a call (io_kind) test these, never a list of kinds.
+enum : int { kGateNone = 0, kGateSilu = 1, kGateRelu2 = 2 };
+// kGateNone: the row of p.act; else the row gate(g, u) of p.act and the second input io.act2, swiglu or relu2.
+__host__ __device__ constexpr int in_gate(int in) {
+    return in == kInRelu2Norm ? kGateRelu2 : in == kInGlu || in == kInGluNorm || in == kInExpertsGlu ? kGateSilu : kGateNone;
+}
+// The RMS norm of that row with io.nw and io.eps.
+__host__ __device__ constexpr bool in_norm(int in) { return in == kInNorm || in == kInGluNorm || in == kInRelu2Norm || in == kInNormBias; }
+// The outputs take the tensor's bias from io.biasv.
+__host__ __device__ constexpr bool in_bias(int in) { return in == kInNormBias; }
+// Routed experts: each slot picks its tensor by the id it reads.
+__host__ __device__ constexpr bool in_experts(int in) { return in == kInExperts || in == kInExpertsGlu; }
 // The input transform and residual of the row kinds: the kernel's last parameter, so that Gemv3Params, wtx and wty keep their
 // parameter offsets.
 struct Gemv3Io {
@@ -658,7 +670,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
                                                                        const Gemv3Io io) {
     static_assert(IN == kInTable || SYM, "a LUT built from activation rows is symmetric");
     static_assert(IN == kInTable || IN == kInRow || AGQ > 0, "input transforms and experts: fp path only");
-    constexpr bool EXPERTS = IN == kInExperts || IN == kInExpertsGlu;
+    constexpr bool EXPERTS = in_experts(IN);
     constexpr int RW = 8 / PB;
     constexpr int RSB = 32 * RW;
     constexpr int TB = SYM ? 8 : 16;              // table bytes per group in shared memory
@@ -827,8 +839,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
             if (lane == 0) *bias_out = bias;       // forwarded to the leader with the partial sums below
         }
     }
-    float inv = 0.f;                              // kInNorm, kInGluNorm, kInRelu2Norm, kInNormBias: 1 / rms of the row
-    if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm || IN == kInNormBias) {
+    float inv = 0.f;                              // in_norm: 1 / rms of the row
+    if (in_norm(IN)) {
         // Every CTA computes inv itself.  All threads stage the row (kInGluNorm / kInRelu2Norm: its swiglu / relu2 of the row of g
         // and the row of u), widened to fp32, in shared memory (iscr [K] | inv), with their loads in flight together; warp 0 then
         // sums its squares in the order of rms_sumsq / rms_warp_sum.
@@ -839,8 +851,8 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
 #pragma unroll
             for (int j = 0; j < 4; ++j)
                 if (g0 + j * nth < ngrp) load_group((size_t)(g0 + j * nth) * 4, b[j]);
-            if (IN == kInGluNorm || IN == kInRelu2Norm) {
-                const auto act = [](float g, float u) { return IN == kInRelu2Norm ? relu2(g, u) : swiglu(g, u); };
+            if (in_gate(IN) != kGateNone) {
+                const auto act = [](float g, float u) { return in_gate(IN) == kGateRelu2 ? relu2(g, u) : swiglu(g, u); };
                 float4 u[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j)
@@ -874,13 +886,13 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
         if (IN != kInTable) {
             constexpr int NG = QCH * 4;            // lane = K-group of the chunk
             float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (IN == kInNorm || IN == kInGluNorm || IN == kInRelu2Norm || IN == kInNormBias) {
+            if (in_norm(IN)) {
                 if (lane < NG) {
                     const size_t g = (size_t)c * NG + lane;
                     const float4 h = reinterpret_cast<const float4 *>(iscr)[g], w = __ldg(reinterpret_cast<const float4 *>(io.nw) + g);
                     x = make_float4(rms_scale(h.x, inv, w.x), rms_scale(h.y, inv, w.y), rms_scale(h.z, inv, w.z), rms_scale(h.w, inv, w.w));
                 }
-            } else if (IN == kInGlu || IN == kInExpertsGlu) {
+            } else if (in_gate(IN) != kGateNone) {
                 if (lane < NG) {
                     float4 gv, uv;
                     load_group(((size_t)c * NG + lane) * 4, gv);
@@ -978,7 +990,7 @@ __global__ void __launch_bounds__(kG3MaxWarps * 32, MINB) gemv3_kernel(const Gem
                 const size_t o = (size_t)n * p.ldc + (size_t)(row - p.c_row0);
                 if (IN != kInTable && !INT_PATH && io.res)   // read, then written by this thread: the residual may be C itself
                     out = __fadd_rn(out, p.out_f16 ? __half2float(reinterpret_cast<const __half *>(io.res)[o]) : reinterpret_cast<const float *>(io.res)[o]);
-                if (IN == kInNormBias) out = __fadd_rn(out, __ldg(io.biasv[blockIdx.z] + (row - p.c_row0)));
+                if (in_bias(IN)) out = __fadd_rn(out, __ldg(io.biasv[blockIdx.z] + (row - p.c_row0)));
                 store_out(Cb, o, out, p.out_f16);
                 for (int q = 0; q < p.npeer; ++q)        // the all-gather, fused into the epilogue: one store per peer and row
                     store_out(p.Cpeer[q], o, out, p.out_f16);

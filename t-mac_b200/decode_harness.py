@@ -226,17 +226,8 @@ class DecodeLayer:
             return b["out"]
         if self.experts:
             return self.moe(x, linear, routed, b, 1)
-        if fused and self.sub_norms:
-            tb.gemv_subnorm(self.lin["o"].wt, 1, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
-            tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            down = tb.gemv_subnorm_relu2 if self.ffn_act_name == "relu2" else tb.gemv_subnorm
-            down(self.lin["down"].wt, 1, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
-            return b["out"]                                                                   # down(rmsnorm(act(gate, up)) * w_fs) + h
         if fused:
-            tb.gemv_residual(self.lin["o"].wt, 1, b["att"], x, b["h"])                          # h = o(att) + x
-            tb.gemv_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], 1, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            tb.gemv_glu(self.lin["down"].wt, 1, b["gate"], b["up"], b["out"], R=b["h"])        # down(silu(gate) * up) + h
-            return b["out"]
+            return self.post_attn(x, b, 1)
         lin("o", self.attn_sub_norm(b), b["o"])
         h = x + b["o"]
         b["h2"].copy_(self.rmsnorm(torch, h, self.norm2))
@@ -264,6 +255,25 @@ class DecodeLayer:
                 lin(m, b["h1"], b[m])
                 if self.qkv_b is not None:
                     b[m].add_(self.qkv_b[m])
+
+    def post_attn(self, x, b, n):
+        """The layer after attention of a fused_ops layer over the n rows of the buffers b (n = 1: the token step's GEMV forms, else
+        the prompt step's prefill forms), three launches into b["out"]: h = o(att) + x (sub_norms: o(rmsnorm(att) * w_as) + x), gate
+        and up of rmsnorm(h) * norm2, out = down(silu(gate) * up) + h (sub_norms: down(rmsnorm(act(gate, up)) * w_fs) + h)."""
+        decode, (o, gate, up, down) = b is self.buf, (self.lin[m].wt for m in ("o", "gate", "up", "down"))
+        subnorm = tb.gemv_subnorm if decode else tb.prefill_subnorm
+        if self.sub_norms:
+            subnorm(o, n, b["att"], self.w_as, self.EPS, b["h"], R=x)
+        else:
+            (tb.gemv_residual if decode else tb.prefill_residual)(o, n, b["att"], x, b["h"])
+        (tb.gemv_rmsnorm if decode else tb.prefill_rmsnorm)([gate, up], n, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
+        if not self.sub_norms:
+            (tb.gemv_glu if decode else tb.prefill_glu)(down, n, b["gate"], b["up"], b["out"], R=b["h"])
+        else:
+            if self.ffn_act_name == "relu2":
+                subnorm = tb.gemv_subnorm_relu2 if decode else tb.prefill_subnorm_relu2
+            subnorm(down, n, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
+        return b["out"]
 
     def attn_sub_norm(self, b):
         """The o projection's input from the buffers b: att, or rmsnorm(att) * w_as in a sub_norms layer (torch ops)."""
@@ -347,17 +357,8 @@ class DecodeLayer:
         b["att"].copy_(att.transpose(0, 1).reshape(P, -1))
         if self.experts:
             return self.moe(x, linear, routed, b, P)
-        if fused and self.sub_norms:
-            tb.prefill_subnorm(self.lin["o"].wt, P, b["att"], self.w_as, self.EPS, b["h"], R=x)  # h = o(rmsnorm(att) * w_as) + x
-            tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            down = tb.prefill_subnorm_relu2 if self.ffn_act_name == "relu2" else tb.prefill_subnorm
-            down(self.lin["down"].wt, P, b["gate"], self.w_fs, self.EPS, b["out"], U=b["up"], R=b["h"])
-            return b["out"]                                                                   # down(rmsnorm(act(gate, up)) * w_fs) + h
         if fused:
-            tb.prefill_residual(self.lin["o"].wt, P, b["att"], x, b["h"])                       # h = o(att) + x
-            tb.prefill_rmsnorm([self.lin["gate"].wt, self.lin["up"].wt], P, b["h"], self.norm2, self.EPS, [b["gate"], b["up"]])
-            tb.prefill_glu(self.lin["down"].wt, P, b["gate"], b["up"], b["out"], R=b["h"])     # down(silu(gate) * up) + h
-            return b["out"]
+            return self.post_attn(x, b, P)
         lin("o", self.attn_sub_norm(b), b["o"])
         b["h"].copy_(x + b["o"])
         b["h2"].copy_(self.rmsnorm(torch, b["h"], self.norm2))

@@ -224,146 +224,138 @@ def qgemm_lut(wt: Weights, N, qlut, lut_scales, lut_biases, Cout, row0=0, rows=N
           "tmac_b200_qgemm_lut")
 
 
+def _call(fn, *args):
+    check(getattr(load(), fn)(*args), fn)
+
+
+def _handles(wts):
+    return (C.c_int64 * len(wts))(*[w.handle for w in wts])
+
+
+def _ptrs(xs, n):
+    """The n-entry host array of the addresses of xs (None: a null array)."""
+    return None if xs is None else (C.c_void_p * n)(*[ptr(x) for x in xs])
+
+
+def _topk(ids):
+    return ids.shape[-1] if hasattr(ids, "shape") else 0
+
+
 def qgemm_lut_grouped(wts, N, qluts, lut_scales, lut_biases, outs, dtype=F32):
     """One launch for len(wts) problems of identical geometry (device tensors)."""
     n = len(wts)
-    H = (C.c_int64 * n)(*[w.handle for w in wts])
-    def arr(xs):
-        return (C.c_void_p * n)(*[ptr(x) for x in xs])
-    check(load().tmac_b200_qgemm_lut_grouped(H, n, N, dtype, arr(qluts), arr(lut_scales), arr(lut_biases), arr(outs)),
-          "tmac_b200_qgemm_lut_grouped")
+    _call("tmac_b200_qgemm_lut_grouped", _handles(wts), n, N, dtype, _ptrs(qluts, n), _ptrs(lut_scales, n), _ptrs(lut_biases, n),
+          _ptrs(outs, n))
 
 
 def gemv_grouped(wts, N, B, outs, dtype=F32):
     """len(wts) tensors of one geometry applied to the same activation rows B in ONE launch, LUT built inside (device tensors)."""
+    _call("tmac_b200_gemv_grouped", _handles(wts), len(wts), N, dtype, ptr(B), _ptrs(outs, len(wts)))
+
+
+# The bodies each gemv_* call with arrays shares with its prefill_* form, fn the C symbol.
+def _rmsnorm(fn, wts, N, H, w, eps, outs, dtype, *bias):
     n = len(wts)
-    H = (C.c_int64 * n)(*[w.handle for w in wts])
-    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
-    check(load().tmac_b200_gemv_grouped(H, n, N, dtype, ptr(B), O), "tmac_b200_gemv_grouped")
+    _call(fn, _handles(wts), n, N, dtype, ptr(H), ptr(w), float(eps), *[_ptrs(b, n) for b in bias], _ptrs(outs, n))
+
+
+def _experts(fn, tables, N, B, ids, outs, dtype):
+    count, n_experts = len(tables), len(tables[0]) if tables else 0
+    if any(len(t) != n_experts for t in tables):
+        raise ValueError(fn[len("tmac_b200_"):] + ": every tensor needs one entry per expert")
+    _call(fn, _handles([w for t in tables for w in t]), count, n_experts, N, dtype, ptr(B), ptr(ids), _topk(ids), _ptrs(outs, count))
+
+
+def _experts_glu(fn, wts, N, G, U, ids, weights, Cout, R, dtype):
+    _call(fn, _handles(wts), len(wts), N, dtype, ptr(G), ptr(U), ptr(ids), ptr(weights), _topk(ids), ptr(R), ptr(Cout))
 
 
 def gemv_rmsnorm(wts, N, H, w, eps, outs, dtype=F32):
     """gemv_grouped on the RMS norm of H: input (H[n] * inv_n) * w, inv_n = 1 / sqrt(mean(H[n]^2) + eps) with the sum of squares in
     the order tmac_b200_gemv_rmsnorm documents.  w: device fp32 [K], 16-byte aligned."""
-    n = len(wts)
-    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
-    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
-    check(load().tmac_b200_gemv_rmsnorm(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), O), "tmac_b200_gemv_rmsnorm")
+    _rmsnorm("tmac_b200_gemv_rmsnorm", wts, N, H, w, eps, outs, dtype)
 
 
 def gemv_rmsnorm_bias(wts, N, H, w, eps, bias, outs, dtype=F32):
     """gemv_rmsnorm plus a bias on each tensor's outputs, outs[i] = gemv_rmsnorm's row + bias[i] rounded once (Qwen2's q/k/v;
     tmac_b200_gemv_rmsnorm_bias).  bias: len(wts) device fp32 [Mout] vectors, 16-byte aligned."""
-    n = len(wts)
-    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
-    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
-    Bs = None if bias is None else (C.c_void_p * n)(*[ptr(b) for b in bias])
-    check(load().tmac_b200_gemv_rmsnorm_bias(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), Bs, O), "tmac_b200_gemv_rmsnorm_bias")
+    _rmsnorm("tmac_b200_gemv_rmsnorm_bias", wts, N, H, w, eps, outs, dtype, bias)
 
 
 def gemv_glu(wt: Weights, N, G, U, Cout, R=None, dtype=F32):
     """Cout = gemv(wt, silu(G) * U) (+ R), the down projection of a SwiGLU FFN and its residual add (device tensors)."""
-    check(load().tmac_b200_gemv_glu(wt.handle, N, dtype, ptr(G), ptr(U), ptr(R), ptr(Cout)), "tmac_b200_gemv_glu")
+    _call("tmac_b200_gemv_glu", wt.handle, N, dtype, ptr(G), ptr(U), ptr(R), ptr(Cout))
 
 
 def gemv_residual(wt: Weights, N, B, R, Cout, dtype=F32):
     """Cout = gemv(wt, B) + R (device tensors; R may be Cout)."""
-    check(load().tmac_b200_gemv_residual(wt.handle, N, dtype, ptr(B), ptr(R), ptr(Cout)), "tmac_b200_gemv_residual")
+    _call("tmac_b200_gemv_residual", wt.handle, N, dtype, ptr(B), ptr(R), ptr(Cout))
 
 
 def gemv_subnorm(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
     """Cout = gemv(wt, rmsnorm(X) * w) (+ R), X = G, or silu(G) * U when U is given: a BitNet layer's o projection behind its
     attn_sub_norm, or its down projection behind its ffn_sub_norm (tmac_b200_gemv_subnorm; device tensors, R may be Cout)."""
-    check(load().tmac_b200_gemv_subnorm(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
-          "tmac_b200_gemv_subnorm")
+    _call("tmac_b200_gemv_subnorm", wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout))
 
 
 def gemv_subnorm_relu2(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
     """Cout = gemv(wt, rmsnorm(relu(G)^2 * U) * w) (+ R): the down projection of a squared-ReLU BitNet FFN (b1.58 2B4T) behind its
     ffn_sub_norm (tmac_b200_gemv_subnorm_relu2; gemv_subnorm's argument order, U required; device tensors, R may be Cout)."""
-    check(load().tmac_b200_gemv_subnorm_relu2(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
-          "tmac_b200_gemv_subnorm_relu2")
+    _call("tmac_b200_gemv_subnorm_relu2", wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout))
 
 
 def gemv_experts(tables, N, B, ids, outs, dtype=F32):
     """Routed experts: tables[i][e] is tensor i of expert e (e.g. i = 0 gate, 1 up).  outs[i] [N][topk][Mout] gets
     gemv(tables[i][ids[n][j]], B[n]) in row (n, j); ids: device int32 [N][topk], read only on the device."""
-    count, n_experts = len(tables), len(tables[0]) if tables else 0
-    if any(len(t) != n_experts for t in tables):
-        raise ValueError("gemv_experts: every tensor needs one entry per expert")
-    H = (C.c_int64 * (count * n_experts))(*[w.handle for t in tables for w in t])
-    O = (C.c_void_p * count)(*[ptr(x) for x in outs])
-    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
-    check(load().tmac_b200_gemv_experts(H, count, n_experts, N, dtype, ptr(B), ptr(ids), topk, O), "tmac_b200_gemv_experts")
+    _experts("tmac_b200_gemv_experts", tables, N, B, ids, outs, dtype)
 
 
 def gemv_experts_glu(wts, N, G, U, ids, weights, Cout, R=None, dtype=F32):
     """Cout[n] = sum_j weights[n][j] * gemv(wts[ids[n][j]], silu(G[n][j]) * U[n][j]) (+ R[n]), the down projection of routed
     experts and their combine in ascending j (device tensors; ids int32 and weights fp32 [N][topk])."""
-    H = (C.c_int64 * len(wts))(*[w.handle for w in wts])
-    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
-    check(load().tmac_b200_gemv_experts_glu(H, len(wts), N, dtype, ptr(G), ptr(U), ptr(ids), ptr(weights), topk, ptr(R), ptr(Cout)),
-          "tmac_b200_gemv_experts_glu")
+    _experts_glu("tmac_b200_gemv_experts_glu", wts, N, G, U, ids, weights, Cout, R, dtype)
 
 
 def prefill_experts(tables, N, B, ids, outs, dtype=F32):
     """gemv_experts' arguments and output, run on the prefill tiles with each expert's tokens grouped on the device (the form for
     large N * topk, tmac_b200_prefill_experts)."""
-    count, n_experts = len(tables), len(tables[0]) if tables else 0
-    if any(len(t) != n_experts for t in tables):
-        raise ValueError("prefill_experts: every tensor needs one entry per expert")
-    H = (C.c_int64 * (count * n_experts))(*[w.handle for t in tables for w in t])
-    O = (C.c_void_p * count)(*[ptr(x) for x in outs])
-    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
-    check(load().tmac_b200_prefill_experts(H, count, n_experts, N, dtype, ptr(B), ptr(ids), topk, O), "tmac_b200_prefill_experts")
+    _experts("tmac_b200_prefill_experts", tables, N, B, ids, outs, dtype)
 
 
 def prefill_experts_glu(wts, N, G, U, ids, weights, Cout, R=None, dtype=F32):
     """gemv_experts_glu's arguments and output, run on the prefill tiles (tmac_b200_prefill_experts_glu)."""
-    H = (C.c_int64 * len(wts))(*[w.handle for w in wts])
-    topk = ids.shape[-1] if hasattr(ids, "shape") else 0
-    check(load().tmac_b200_prefill_experts_glu(H, len(wts), N, dtype, ptr(G), ptr(U), ptr(ids), ptr(weights), topk, ptr(R), ptr(Cout)),
-          "tmac_b200_prefill_experts_glu")
+    _experts_glu("tmac_b200_prefill_experts_glu", wts, N, G, U, ids, weights, Cout, R, dtype)
 
 
 def prefill_rmsnorm(wts, N, H, w, eps, outs, dtype=F32):
     """gemv_rmsnorm's arguments and output, run on the prefill tiles with all len(wts) tensors in one launch (the form for a prompt,
     tmac_b200_prefill_rmsnorm)."""
-    n = len(wts)
-    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
-    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
-    check(load().tmac_b200_prefill_rmsnorm(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), O), "tmac_b200_prefill_rmsnorm")
+    _rmsnorm("tmac_b200_prefill_rmsnorm", wts, N, H, w, eps, outs, dtype)
 
 
 def prefill_rmsnorm_bias(wts, N, H, w, eps, bias, outs, dtype=F32):
     """gemv_rmsnorm_bias's arguments and output, run on the prefill tiles (tmac_b200_prefill_rmsnorm_bias)."""
-    n = len(wts)
-    Hs = (C.c_int64 * n)(*[w_.handle for w_ in wts])
-    O = (C.c_void_p * n)(*[ptr(x) for x in outs])
-    Bs = None if bias is None else (C.c_void_p * n)(*[ptr(b) for b in bias])
-    check(load().tmac_b200_prefill_rmsnorm_bias(Hs, n, N, dtype, ptr(H), ptr(w), float(eps), Bs, O), "tmac_b200_prefill_rmsnorm_bias")
+    _rmsnorm("tmac_b200_prefill_rmsnorm_bias", wts, N, H, w, eps, outs, dtype, bias)
 
 
 def prefill_glu(wt: Weights, N, G, U, Cout, R=None, dtype=F32):
     """gemv_glu's arguments and output, run on the prefill tiles (tmac_b200_prefill_glu)."""
-    check(load().tmac_b200_prefill_glu(wt.handle, N, dtype, ptr(G), ptr(U), ptr(R), ptr(Cout)), "tmac_b200_prefill_glu")
+    _call("tmac_b200_prefill_glu", wt.handle, N, dtype, ptr(G), ptr(U), ptr(R), ptr(Cout))
 
 
 def prefill_residual(wt: Weights, N, B, R, Cout, dtype=F32):
     """gemv_residual's arguments and output, run on the prefill tiles (tmac_b200_prefill_residual)."""
-    check(load().tmac_b200_prefill_residual(wt.handle, N, dtype, ptr(B), ptr(R), ptr(Cout)), "tmac_b200_prefill_residual")
+    _call("tmac_b200_prefill_residual", wt.handle, N, dtype, ptr(B), ptr(R), ptr(Cout))
 
 
 def prefill_subnorm(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
     """gemv_subnorm's arguments and output, run on the prefill tiles (tmac_b200_prefill_subnorm)."""
-    check(load().tmac_b200_prefill_subnorm(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
-          "tmac_b200_prefill_subnorm")
+    _call("tmac_b200_prefill_subnorm", wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout))
 
 
 def prefill_subnorm_relu2(wt: Weights, N, G, w, eps, Cout, U=None, R=None, dtype=F32):
     """gemv_subnorm_relu2's arguments and output, run on the prefill tiles (tmac_b200_prefill_subnorm_relu2)."""
-    check(load().tmac_b200_prefill_subnorm_relu2(wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout)),
-          "tmac_b200_prefill_subnorm_relu2")
+    _call("tmac_b200_prefill_subnorm_relu2", wt.handle, N, dtype, ptr(G), ptr(U), ptr(w), float(eps), ptr(R), ptr(Cout))
 
 
 def gemv(wt: Weights, N, B, Cout, dtype=F32):

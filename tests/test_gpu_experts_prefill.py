@@ -6,13 +6,13 @@ rows in ascending slot order, forced onto the same tile (prefill_min_n = 1; pref
 expert's own to 64 when the fp16 tile needs them -- the padding comes after the real rows, so it moves none of them).  The GLU
 form's rows are the GLU input materialised on the GPU as g / (1 + exp(-g)) * u, and its combine is the numpy restatement of the
 GEMV form's suite.  kfactor = act_group_size / 4 everywhere, as in the sequence tests."""
-import contextlib
 
 import numpy as np
 import pytest
 
 import act_rows
 import tmac_b200 as tb
+from fused_util import dense_tile, knobs, tdt
 from seq_util import DENSE_NMSE, TIGHT_TOL, mk, oracle_gemv, same_bits, stream
 from test_gpu_experts import Table, combine, dev, glu_ref, nan_out, normal, rand_ids, softmax_weights
 
@@ -25,37 +25,6 @@ TILE_IDS = ["fp16", "int8"]
 GROUPINGS = [(128, 128), (128, 64), (128, 32), (64, 64), (64, 32), (32, 32)]    # every fp grouping the tiles take
 G_CASES = [(g, a, b) for g, a in GROUPINGS for b in (2, 4)] + [(128, 64, 3)]
 G_IDS = ["g%d-ags%d-w%d" % c for c in G_CASES]
-
-
-@contextlib.contextmanager
-def knobs(**kv):
-    """Set library knobs for the block, then put back the defaults (prefill16 = 1, prefill_min_n = 0)."""
-    for k, v in kv.items():
-        tb.debug_set(k, v)
-    try:
-        yield
-    finally:
-        for k in kv:
-            tb.debug_set(k, {"prefill16": 1, "prefill_min_n": 0}[k])
-
-
-def tdt(dtype):
-    return tb.F16 if dtype == torch.float16 else tb.F32
-
-
-def dense_tile(wt, X, t16, dtype=torch.float32):
-    """tmac_b200_gemv of the rows X (device [n][K]) on the fp16 (t16) or the int8 tile: numpy [n][Mout]."""
-    n = X.shape[0]
-    pad = max(0, 64 - n) if t16 else 0
-    if pad:
-        X = torch.cat([X, X[:1].expand(pad, -1)])
-    out = nan_out(n + pad, wt.cfg.M, dtype=dtype)
-    with knobs(prefill_min_n=1, prefill16=int(t16)):
-        tb.gemv(wt, n + pad, X.to(dtype).contiguous(), out, dtype=tdt(dtype))
-        launch = tb.last_launch()
-    assert launch["cluster"] == (16 if t16 else 1) and launch["batch"] == -(n + pad), launch
-    torch.cuda.synchronize()
-    return out[:n].cpu().numpy()
 
 
 def expert_slots(hids, E):

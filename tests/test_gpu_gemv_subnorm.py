@@ -12,6 +12,7 @@ import pytest
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
+from fused_util import serial_input
 from seq_util import EPS, TIGHT_TOL, kc, mk, norm_weight, oracle_gemv, rms_input, same_bits, stream
 from test_gpu_gemv_fused_io import dev, expect, glu_ref, grouped, nan_out
 
@@ -95,16 +96,6 @@ def test_bitnet_grouping(bitnet, M, K, N):
 
 
 # ---- 2: the order of the sum of squares, and the zero row -----------------------------------------------------------------------
-def serial_input(x, w, eps):
-    """rmsnorm(x) * w with the sum of squares of the 4-groups taken serially: an order the call does not use."""
-    g = x.reshape(-1, 4)
-    q = (g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1]) + (g[:, 2] * g[:, 2] + g[:, 3] * g[:, 3])
-    s = np.float32(0.0)
-    for v in q:
-        s = np.float32(s + v)
-    return (x * (np.float32(1.0) / np.sqrt(s / np.float32(x.size) + np.float32(eps)))) * w
-
-
 def test_order_and_zero_row(mk):
     """A row whose SwiGLU values have two magnitudes: one K-group of squares near 2^28 and 639 of squares near 1, each below half
     an ulp of the large one.  A serial sum of squares drops every small group; the documented order sums them per lane first and

@@ -11,8 +11,8 @@ import pytest
 
 import act_rows
 import tmac_b200 as tb
+from fused_util import dense_tile, knobs, tdt
 from seq_util import A_CASES, A_IDS, EPS, mk, norm_weight, rms_input, same_bits, stream
-from test_gpu_experts_prefill import knobs
 from test_gpu_gemv_fused_io import dev, expect, glu_ref, nan_out, normal
 
 torch = pytest.importorskip("torch")
@@ -25,24 +25,9 @@ TILE_CASES = [c for c in A_CASES if c[2] != 1]    # every fp grouping the tiles 
 TILE_CASE_IDS = [i for c, i in zip(A_CASES, A_IDS) if c in TILE_CASES]
 
 
-def tdt(dtype):
-    return tb.F16 if dtype == torch.float16 else tb.F32
-
-
 def takes16(prefill16, N):
     """The tile the prefill forms pick: the dense calls' rule."""
     return bool(prefill16) and N >= 64
-
-
-def dense_tile(wt, N, a, t16):
-    """tmac_b200_gemv of the fp32 rows a (device [N][K]) on the fp16 (t16) or the int8 tile: numpy float32 [N][Mout]."""
-    out = nan_out(N, wt.cfg.M)
-    with knobs(prefill_min_n=1, prefill16=int(t16)):
-        tb.gemv(wt, N, a.float().contiguous(), out)
-        launch = tb.last_launch()
-    assert launch["cluster"] == (16 if t16 else 1) and launch["batch"] == -N, launch
-    torch.cuda.synchronize()
-    return out.cpu().numpy()
 
 
 def run_norm(wts, N, H, w, eps, prefill16, dtype=torch.float32):
@@ -61,7 +46,7 @@ def check_norm(wts, N, H, w, prefill16, eps=EPS, dtype=torch.float32):
     assert launch["cluster"] == (16 if t16 else 1) and launch["batch"] == -N, launch
     a = rms_input(H.float().cpu().numpy(), w, eps)
     for i, (wt, o) in enumerate(zip(wts, outs)):
-        expect(o, dense_tile(wt, N, dev(a), t16), f16=dtype == torch.float16, what="prefill_rmsnorm tensor %d" % i)
+        expect(o, dense_tile(wt, dev(a), t16), f16=dtype == torch.float16, what="prefill_rmsnorm tensor %d" % i)
     return a
 
 
@@ -72,7 +57,7 @@ def check_glu(wt, N, G, U, prefill16, R=None, dtype=torch.float32):
         tb.prefill_glu(wt, N, G, U, out, R=R, dtype=tdt(dtype))
         assert tb.last_launch()["cluster"] == (16 if t16 else 1)
     torch.cuda.synchronize()
-    expect(out, dense_tile(wt, N, glu_ref(G, U), t16), None if R is None else R.float().cpu().numpy(), dtype == torch.float16, "prefill_glu")
+    expect(out, dense_tile(wt, glu_ref(G, U), t16), None if R is None else R.float().cpu().numpy(), dtype == torch.float16, "prefill_glu")
 
 
 def check_residual(wt, N, B, R, prefill16, dtype=torch.float32):
@@ -82,7 +67,7 @@ def check_residual(wt, N, B, R, prefill16, dtype=torch.float32):
         tb.prefill_residual(wt, N, B, R, out, dtype=tdt(dtype))
         assert tb.last_launch()["cluster"] == (16 if t16 else 1)
     torch.cuda.synchronize()
-    expect(out, dense_tile(wt, N, B, t16), R.float().cpu().numpy(), dtype == torch.float16, "prefill_residual")
+    expect(out, dense_tile(wt, B, t16), R.float().cpu().numpy(), dtype == torch.float16, "prefill_residual")
 
 
 # ---- 1: every fp grouping, both tiles ----------------------------------------------------------------------------------------------

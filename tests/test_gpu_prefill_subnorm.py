@@ -14,8 +14,8 @@ import pytest
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
+from fused_util import bm_of, dense_tile, knobs, launched, serial_input, tdt
 from seq_util import DENSE_NMSE, EPS, TIGHT_TOL, mk, norm_weight, rms_input, same_bits, stream
-from test_gpu_experts_prefill import knobs
 from test_gpu_gemv_fused_io import dev, expect, glu_ref, nan_out, normal
 
 torch = pytest.importorskip("torch")
@@ -24,14 +24,6 @@ pytestmark = pytest.mark.gpu
 TILES = [True, False]
 TILE_IDS = ["fp16", "int8"]
 SCALE0 = float(np.float32(np.float16(0.037)))
-
-
-def tdt(dtype):
-    return tb.F16 if dtype == torch.float16 else tb.F32
-
-
-def bm_of(M, bits):
-    return next(b for b in ((192, 384, 576, 768) if bits == 3 else (256, 128, 512, 1024, 320, 640)) if (M * bits) % b == 0)
 
 
 @pytest.fixture
@@ -54,11 +46,6 @@ def pair(stream):
     yield make
     for wt in made:
         wt.free()
-
-
-def launched(t16, N):
-    launch = tb.last_launch()
-    assert launch["cluster"] == (16 if t16 else 1) and launch["batch"] == -N, launch
 
 
 def twin_forms(p, N, rng, t16, ags):
@@ -171,16 +158,6 @@ def test_chunk64_on_the_int8_tile(pair, oracle, M, K, ags, N):
 
 
 # ---- 3: prefill_subnorm on per-row-scale tensors -------------------------------------------------------------------------------------
-def dense_tile(wt, N, a, t16):
-    """tmac_b200_gemv of the fp32 rows a (numpy [N][K]) on the fp16 (t16) or the int8 tile: numpy float32 [N][Mout]."""
-    out = nan_out(N, wt.cfg.M)
-    with knobs(prefill_min_n=1, prefill16=int(t16)):
-        tb.gemv(wt, N, dev(a), out)
-        launched(t16, N)
-    torch.cuda.synchronize()
-    return out.cpu().numpy()
-
-
 def check_subnorm(wt, N, G, w, t16, U=None, R=None, eps=EPS, dtype=torch.float32, out=None):
     """prefill_subnorm of host rows G (U, R) passed as dtype against dense_tile on the materialised input; returns a."""
     f16 = dtype == torch.float16
@@ -192,19 +169,9 @@ def check_subnorm(wt, N, G, w, t16, U=None, R=None, eps=EPS, dtype=torch.float32
     torch.cuda.synchronize()
     x = dG.float() if dU is None else glu_ref(dG, dU)
     a = rms_input(x.cpu().numpy(), w, eps)
-    expect(out, dense_tile(wt, N, a, t16 and N >= 64), None if dR is None else dR.float().cpu().numpy(), f16,
+    expect(out, dense_tile(wt, dev(a), t16 and N >= 64), None if dR is None else dR.float().cpu().numpy(), f16,
            "prefill_subnorm (U %s, R %s, %s)" % (U is not None, R is not None, "F16" if f16 else "F32"))
     return a
-
-
-def serial_input(x, w, eps):
-    """rmsnorm(x) * w with the sum of squares of the 4-groups taken serially: an order the call does not use."""
-    g = x.reshape(-1, 4)
-    q = (g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1]) + (g[:, 2] * g[:, 2] + g[:, 3] * g[:, 3])
-    s = np.float32(0.0)
-    for v in q:
-        s = np.float32(s + v)
-    return (x * (np.float32(1.0) / np.sqrt(s / np.float32(x.size) + np.float32(eps)))) * w
 
 
 SUB_CASES = [("w2zp-g128-a64", 2, 128, 64, True), ("w4-g32-a32", 4, 32, 32, False)]

@@ -4,7 +4,6 @@ projections carry a bias (Qwen2), and the decode harness's qkv_bias layers.
 Every check is bit for bit against the equivalence the header documents: each output equals the call without a bias
 (gemv_rmsnorm at the same decomposition, prefill_rmsnorm on the same tile) with F32 outputs, followed by a numpy float32 add of the
 bias, rounded once to fp16 for an F16 call."""
-import contextlib
 import types
 
 import numpy as np
@@ -13,6 +12,7 @@ import pytest
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
+from fused_util import knobs
 from seq_util import DENSE_NMSE, EPS, kc, mk, norm_weight, rms_input, stream
 from test_gpu_gemv_fused_io import dev, expect, nan_out
 
@@ -22,18 +22,6 @@ pytestmark = pytest.mark.gpu
 K = 1280                                        # 10 chunks of 128 K, 40 of 32 K
 M = 768
 PF16_TOL, INT8_TOL = 5e-4, 2e-5                 # the tiles' bounds against the oracle, max |got - ref| / max |ref| (DESIGN 3.3)
-
-
-@contextlib.contextmanager
-def knobs(**kv):
-    """Set library knobs for the block, then put back their defaults."""
-    for k, v in kv.items():
-        tb.debug_set(k, v)
-    try:
-        yield
-    finally:
-        for k in kv:
-            tb.debug_set(k, {"prefill16": 1, "cs": 0, "wpc": 0}[k])
 
 
 def biases(rng, count, m=M, big=True):

@@ -15,6 +15,7 @@ import pytest
 import act_rows
 import tmac_b200 as tb
 import tmac_oracle as T
+from fused_util import bm_of, knobs, launched, serial_input, tdt
 from seq_util import DENSE_NMSE, EPS, Op, norm_weight, rms_input, same_bits, stream
 from test_gpu_gemv_fused_io import dev, expect, nan_out, normal
 
@@ -23,26 +24,6 @@ pytestmark = pytest.mark.gpu
 
 SCALE0 = float(np.float32(np.float16(0.037)))
 H2B, F2B = 2560, 6912                                   # BitNet b1.58 2B4T: hidden, FFN (the down projection is H2B x F2B)
-
-
-@contextlib.contextmanager
-def knobs(**kv):
-    """Set library knobs for the block, then put back the defaults (prefill16 = 1, prefill_min_n = 0)."""
-    for k, v in kv.items():
-        tb.debug_set(k, v)
-    try:
-        yield
-    finally:
-        for k in kv:
-            tb.debug_set(k, {"prefill16": 1, "prefill_min_n": 0}[k])
-
-
-def tdt(dtype):
-    return tb.F16 if dtype == torch.float16 else tb.F32
-
-
-def bm_of(M, bits):
-    return next(b for b in ((192, 384, 576, 768) if bits == 3 else (256, 128, 512, 1024, 320, 640)) if (M * bits) % b == 0)
 
 
 @pytest.fixture
@@ -82,11 +63,6 @@ def relu2_input(dG, dU, w, eps=EPS):
     """The documented input a from the device rows G and U (fp16 widened): numpy float32 [N][K]."""
     with np.errstate(invalid="ignore", over="ignore"):
         return rms_input(relu2_np(dG.float().cpu().numpy(), dU.float().cpu().numpy()), w, eps)
-
-
-def launched(t16, N):
-    launch = tb.last_launch()
-    assert launch["cluster"] == (16 if t16 else 1) and launch["batch"] == -N, launch
 
 
 def dense(wt, N, a, t16=None):
@@ -182,16 +158,6 @@ def test_prompt_form(tensors, oracle, kind, N, t16):
 
 
 # ---- 3: the order is pinned -----------------------------------------------------------------------------------------------------
-def serial_input(x, w, eps):
-    """rmsnorm(x) * w with the sum of squares of the 4-groups taken serially: an order the calls do not use."""
-    g = x.reshape(-1, 4)
-    q = (g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1]) + (g[:, 2] * g[:, 2] + g[:, 3] * g[:, 3])
-    s = np.float32(0.0)
-    for v in q:
-        s = np.float32(s + v)
-    return (x * (np.float32(1.0) / np.sqrt(s / np.float32(x.size) + np.float32(eps)))) * w
-
-
 def pinned_rows(rng, K, ags):
     """G, U [6][K]: act_rows' fp32 and mixed gates, a two-magnitude row (one K-group of s near 2^17, the others near 1), a row of
     negative, +-0 and large gates, an all-negative row (with +-0), and a plain normal row (row 5, for the NaN test)."""
